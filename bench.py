@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Benchmark of the deep-spectral hot path: images/sec for extract_features + extract_eigs
-(480x480, dino_vits16, K=5, dense affinity -- BASELINE.json configs[1]) on N B200s, one process per GPU.
+(480x480, dino_vits16, K=5, dense affinity -- BASELINE.json configs[1]) on N H100s, one process per GPU.
 
     python bench.py --gpus 1 --steps 4 --warmup 3
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
@@ -32,8 +32,8 @@ METRIC = "images/sec (features+eigs, 480px dino_vits16 K=5)"
 
 
 def usable_cpus() -> int:
-    """CPUs this job may use: affinity mask and cgroup quota, not os.cpu_count() (the B200 hosts show 128 hardware
-    threads to a container whose CPU quota is 16; a pool sized for 128 is throttled by the scheduler)."""
+    """CPUs this job may use: affinity mask and cgroup quota, not os.cpu_count() (a container may see many more hardware
+    threads than its CPU quota allows; a pool sized for all of them is throttled by the scheduler)."""
     n = os.cpu_count() or 1
     try:
         n = min(n, len(os.sched_getaffinity(0)))
@@ -64,7 +64,7 @@ def parse():
                     help="c2 = configs[1] (the metric's config, default); c3 = dino_vitb8 480px colour-KNN K=15; "
                          "c4 = VOC-shaped variable sizes, dino_vits16 K=5; c5 = dino_vitb8 640px K=32 + N sweep")
     ap.add_argument("--images-per-step", type=int, default=0,
-                    help="per GPU; 0 = workload default (c2: 296 = 2 x 148 SMs, c3: 148, c4: 592, c5: 148)")
+                    help="per GPU; 0 = workload default (c2: 264 = 2 x 132 SMs, c3: 132, c4: 528, c5: 132)")
     ap.add_argument("--size", type=int, default=480)
     ap.add_argument("--K", type=int, default=5)
     ap.add_argument("--model", default="dino_vits16")
@@ -74,6 +74,8 @@ def parse():
     ap.add_argument("--no-as-shipped", action="store_true", help="skip the eager-GPU-ViT + CPU-eigsh baseline")
     ap.add_argument("--ref-images-per-step", type=int, default=0, help="0 = 2 x worker processes")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the timed path returned in its last step as DIR/<name>.npy (float32 / float64)")
     return ap.parse_args()
 
 
@@ -146,7 +148,8 @@ def load_peaks():
         d = json.loads(p.read_text())
         return {"hbm_gbs": d["hbm_gbs"], "tflops_burst": d["bf16_tflops"], "tflops_sustained": d["bf16_tflops_sustained"],
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tflops_burst": 1590.0, "tflops_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tflops_burst": 989.0, "tflops_sustained": 989.0,
+            "source": "NVIDIA H100 SXM data sheet (dense FP16, 700 W), not measured"}
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -209,8 +212,8 @@ def _affinity_eigs_task(job):
 
 
 class CpuPool:
-    """Process pool with every host core busy: cores / threads_per_worker workers (2 threads per worker measured best
-    on the 2 x 32-core / 128-thread host of the B200 box for the ViT + eigsh mix: 9.3 img/s vs 7.6 at 4, 5.9 at 8)."""
+    """Process pool with every host core busy: cores / threads_per_worker workers (2 BLAS threads per worker by
+    default for the ViT + eigsh mix)."""
 
     def __init__(self, model_name, threads_per_worker=2, max_workers=64, need_vit=True):
         import multiprocessing as mp
@@ -461,7 +464,7 @@ class Ctx:
 
 
 def ln_fused(d):
-    return d == 384 and os.environ.get("DSS_VIT_FUSED_LN", "1") != "0"
+    return d == 384 and os.environ.get("DSS_VIT_FUSED_LN", "0") != "0"
 
 
 def vit_alg(P, d, depth_full, N, n_images):
@@ -499,23 +502,27 @@ def eig_alg(B, N, d, K, m_steps, with_degree_pass=False):
     }
 
 
-def load_traffic():
-    for name in ("r2_traffic.json", "r1_traffic.json"):
-        p = ROOT / "profiles" / name
-        if p.is_file():
-            try:
-                return json.loads(p.read_text()), name
-            except Exception:
-                pass
-    return None, None
-
-
 # ---------------------------------------------------------------------------------------------------------------
+def dump_outputs(out_dir, arrays, limit=64 << 20):
+    """Each tensor as out_dir/<name>.npy: floating point as float32 (float64 stays float64), integers as float64. A
+    tensor whose share of the 64 MB budget is exceeded is replaced by a fixed, seeded sample of its first-axis rows."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    share = limit // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().cpu().numpy()
+        a = a.astype(np.float64 if a.dtype == np.float64 or not np.issubdtype(a.dtype, np.floating) else np.float32)
+        if a.nbytes > share and a.ndim > 0:
+            rows = max(1, int(a.shape[0] * share // a.nbytes))
+            a = a[np.sort(np.random.default_rng(0).choice(a.shape[0], rows, replace=False))]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
+
+
 def run_c2(ctx: Ctx):
     args, torch, dev = ctx.args, ctx.torch, ctx.dev
     import numpy as np
     sd = ctx.weights(args.model)
-    B = args.images_per_step or 296      # 2 x 148: the eigensolver (one CTA per image, two per SM) fills every SM slot
+    B = args.images_per_step or 264      # 2 x 132: the eigensolver (one CTA per image, two per SM) fills every SM slot
     if args.vit_batch <= 0:
         args.vit_batch = B
     pipe = ctx.pipeline.SpectralPipeline(args.model, K=args.K, device=dev, state_dict=sd, vit_batch=args.vit_batch)
@@ -535,6 +542,12 @@ def run_c2(ctx: Ctx):
         last["out"] = pipe.run_device(dev_imgs)
     ms, launches = ctx.timed(step_dev, steps, W)
     value = ctx.world * B * steps / (ms * 1e-3)
+    if args.dump_outputs and ctx.rank == 0:
+        evals, evecs, info = last["out"]
+        # the K features of the step (ViT output, [B, N, d]) stay on the device next to the eigenpairs; a seeded sample of
+        # images is written when they exceed their share of the budget
+        dump_outputs(args.dump_outputs, {"eigenvalues": evals, "eigenvectors": evecs, "solver_info": info,
+                                         "features": pipe._bufs["feats"]})
     info = last["out"][2]
     conv = int(info[:, 1].sum().item())
     steps_mean = float(info[:, 0].float().mean().item())
@@ -567,19 +580,7 @@ def run_c2(ctx: Ctx):
     n_vit = (B + args.vit_batch - 1) // args.vit_batch
     alg = {**vit_alg(P, d, depth - 1, N, B), **eig_alg(B, N, d, K, steps_mean)}
     kernels = ctx.kernel_table(prof, alg)
-    traffic_db, traffic_file = load_traffic()
-
-    def traffic_lookup(kernel):
-        if not traffic_db:
-            return None
-        per_img = traffic_db.get("per_image_bytes", {}).get(kernel)
-        if not per_img:
-            return None
-        per_launch_images = B if kernel in ("eigsh", "affinity", "rownorm") else args.vit_batch
-        return per_img * per_launch_images
-    roofline = ctx.roofline(kernels, traffic_lookup)
-    if roofline is not None:
-        roofline["traffic_source"] = traffic_file
+    roofline = ctx.roofline(kernels)
 
     line = {"metric": METRIC, "value": value, "unit": "images/s", "n_gpus": ctx.world, "steps": steps, "warmup": W,
             "ms_per_step": ms / steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -692,7 +693,7 @@ def run_c3(ctx: Ctx):
     import numpy as np
     model_name, S, K, lam = "dino_vitb8", 480, 15, 10.0
     sd = ctx.weights(model_name)
-    B = args.images_per_step or 148      # one eigensolver CTA per SM
+    B = args.images_per_step or 132      # one eigensolver CTA per SM
     vb = 16                              # ViT launch sequence per 16 images (61 MB of workspace per image at T = 3601)
     model = ctx.vit.DinoViT(model_name, sd, device=dev)
     P, d, depth = model.patch_size, model.dim, model.depth
@@ -792,7 +793,7 @@ def run_c4(ctx: Ctx):
     from collections import Counter
     model_name, K = "dino_vits16", 5
     sd = ctx.weights(model_name)
-    B = args.images_per_step or 592
+    B = args.images_per_step or 528
     model = ctx.vit.DinoViT(model_name, sd, device=dev)
     P, d, depth = model.patch_size, model.dim, model.depth
     total = 50_000
@@ -857,7 +858,7 @@ def run_c5(ctx: Ctx):
     import numpy as np
     model_name, K = "dino_vitb8", 32
     sd = ctx.weights(model_name)
-    B = args.images_per_step or 148      # one eigensolver CTA per SM
+    B = args.images_per_step or 132      # one eigensolver CTA per SM
     model = ctx.vit.DinoViT(model_name, sd, device=dev)
     P, d, depth = model.patch_size, model.dim, model.depth
     W, steps = max(args.warmup, 3), args.steps
@@ -936,7 +937,9 @@ def run_c5(ctx: Ctx):
 
 def main():
     args = parse()
-    try:   # this process's own CPU work (fp64 checks of the parity block, pinned-buffer fills): not 128 threads on 16 CPUs
+    if args.dump_outputs and (args.workload != "c2" or args.impl != "ours"):
+        raise SystemExit("--dump-outputs is implemented for --workload c2 --impl ours")
+    try:   # this process's own CPU work (fp64 checks of the parity block, pinned-buffer fills): no more threads than usable CPUs
         import torch
         if torch.get_num_threads() > usable_cpus():
             torch.set_num_threads(usable_cpus())

@@ -99,7 +99,7 @@ def load() -> C.CDLL:
         return _lib
     if not LIB_PATH.is_file():
         raise DssError(f"{LIB_PATH} not found: build it with `python {_HERE.name}/build.py` "
-                       "(nvcc, sm_100a). There is no fallback implementation.")
+                       "(nvcc, sm_90a). There is no fallback implementation.")
     lib = C.CDLL(str(LIB_PATH))
     for name, (res, args) in PROTOTYPES.items():
         fn = getattr(lib, name)  # AttributeError if the .so does not export a declared symbol

@@ -1,8 +1,8 @@
-"""In-tree build of libdss_b200.so with nvcc for sm_100a (cross-compiles without a GPU).
+"""In-tree build of libdss_b200.so with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python deep-spectral-segmentation_b200/build.py [--force]
 
-The shared object lands next to this file (git-ignored, but shipped to the GPU box by gpurun).
+The shared object lands next to this file (git-ignored); object files and the compiler log go to build/.
 """
 from __future__ import annotations
 
@@ -15,7 +15,7 @@ HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 LIB = HERE / "libdss_b200.so"
 SOURCES = ["api.cu", "gemm.cu", "gemm_ln.cu", "vit_kernels.cu", "attention_tc.cu", "vit.cu", "affinity.cu", "eigsh.cu", "knn.cu", "segment.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "-DDSS_BUILD", "-Xptxas", "-v", *os.environ.get("DSS_EXTRA_NVCC_FLAGS", "").split()]
 
 
@@ -58,7 +58,7 @@ def build(force: bool = False, verbose: bool = False) -> Path:
         print("\n".join(log))
     if failed:
         raise RuntimeError("nvcc failed, see above")
-    cmd = [nvcc, "-shared", "-o", str(LIB), *objs, "-cudart", "static"]
+    cmd = [nvcc, *NVCC_FLAGS[:2], "-shared", "-o", str(LIB), *objs, "-cudart", "static"]
     subprocess.check_call(cmd)
     return LIB
 

@@ -1,13 +1,13 @@
 // Patch-affinity build: W = relu(F^ F^T) / max (+ lambda * colour counts)   (reference extract/extract.py:148,191-221)
 //
-// The Gram product runs on the tcgen05 tensor cores at fp32-equivalent accuracy. The eigenvectors of the graph
+// The Gram product runs on the tensor cores (wgmma) at fp32-equivalent accuracy. The eigenvectors of the graph
 // Laplacian move by 2e-4..8e-4 when the features are merely rounded to bf16 (SURVEY 8a-4), so each normalised
 // feature x is split as x = hi + lo with hi = fp16(x), lo = x - hi (|lo| <= 2^-12 |x|) and
 //     x.y ~= hi.hi' + (hi/64).(64 lo') + (64 lo).(hi'/64)              (lo.lo' ~ 2^-24 is dropped)
 // i.e. ONE fp16 GEMM with K = 3d over S = [hi | hi/64 | 64 lo] against the same array with the last two groups of
 // K slabs swapped. The 2^+-6 factors keep every operand inside the fp16 normal range. Measured error of the split
 // against a float64 product: 7e-8, smaller than a plain fp32 product's 1e-6 (DESIGN.md section 3).
-// The GEMM itself is gemm.cu's TMA/tcgen05 kernel in batched mode with the affinity epilogue (relu, /max,
+// The GEMM itself is gemm.cu's TMA/wgmma kernel in batched mode with the affinity epilogue (relu, /max,
 // + lambda*counts, zero padding of the row pitch) fused.
 #include "common.cuh"
 

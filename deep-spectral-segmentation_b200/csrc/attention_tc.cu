@@ -1,33 +1,15 @@
-// Multi-head attention (head dim 64) on the 5th-generation tensor cores: O = softmax(Q K^T / 8) V.
+// Multi-head attention (head dim 64) on the Hopper tensor cores: O = softmax(Q K^T / 8) V.
 //
-// Persistent kernel, one CTA per SM. A work item is one (image, head, PAIR of 128-query tiles); the CTA walks its items
-// with every ring / barrier phase carried across item boundaries, so the loads and the first score tile of the next
-// item overlap the tail of the current one.
-//   warp 0      TMA producer: Q tiles (double buffered per query tile) and K_j / V_j tiles straight out of the packed
-//               qkv activations [B*T, 3d] (box 64 x 128, 128 B swizzle) through a 3-stage ring shared by both
-//               query tiles
-//   warps 1, 2  tcgen05.mma issuers of query tile A / B (warp 1 also owns the TMEM allocation); per key tile j:
-//                 S_g = Q_g K_j^T   (UMMA 128 x kc x 16, x4, both operands K-major)               -> TMEM S_g
-//                 O_g += P_g V_j    (UMMA 128 x 64 x 16, x kc/16, A = P from TMEM, B = V MN-major) -> TMEM O_g
-//               kc = 128 except in the last key tile, where it is the number of existing keys rounded up to 16
-//               (T = 901: 16 instead of 128).
-//   warps 4..7  softmax of query tile A, warps 8..11 of query tile B: ONE thread per query row (tcgen05.ld 32x32b), no
-//               cross-thread exchange. The 128 scores of the row are read from TMEM once and S_g is released at once
-//               (the next score tile is computed while this one is exponentiated); P = 2^(s c - m c) (MUFU.EX2) goes
-//               back to TMEM as packed fp16 pairs (tcgen05.st) and is the A operand of the PV MMA: P never touches
-//               shared memory, whose bandwidth the K / V / Q operand reads need.
-//               The output accumulates in TMEM across key tiles. The reference maximum m is only raised (and O, l
-//               rescaled, by the owning thread through tcgen05.ld/st) when a tile's row maximum exceeds it by more than
-//               2^8 -- softmax is shift invariant and fp16 P / fp32 sums have the headroom -- so in the steady state the
-//               softmax warps never touch O until the epilogue.
-// The two softmax groups run out of phase (B's first tile is held back until A is half way through its first tile), so one
-// group's MUFU-bound exp phase overlaps the other's TMEM loads / maxima / fences. The kernel is bound by the MUFU pipe
-// (128 x 128 exp2 per tile at 16 per clock per SM), not by the tensor pipe.
+// One CTA per (128-query tile, head, image), two warp groups, each owning 64 query rows. Thread 0 drives the TMA: the
+// Q tile and the K_j / V_j tiles come straight out of the packed qkv activations [B*T, 3d] (box 64 x 128, 128 B
+// swizzle) through a 2-stage ring shared by both warp groups. Per key tile j, per warp group:
+//   S = Q K^T    wgmma m64 x 128 x 16, x4, both operands K-major in shared memory        -> registers
+//   online softmax in registers (row max / sum over the 4 lanes of a quad), P = 2^(s c - m c) packed to fp16 in the
+//   register layout of the wgmma A operand: P never touches shared memory
+//   O += P V     wgmma m64 x 64 x 16, x8, A = P from registers, B = V (MN-major: keys x head dims) -> registers
+// Keys past T are masked to -inf; the output leaves through the (then free) Q tile with one 3-D TMA store (rows past T
+// clipped per image).
 #include <math.h>
-#include <stdio.h>
-#include <stdlib.h>
-
-#include <type_traits>
 
 #include "common.cuh"
 
@@ -43,508 +25,183 @@ __device__ __forceinline__ float ex2_approx(float x) {
   return y;
 }
 
-// warp group 0: TMA warp, two MMA warps, one idle warp; warp groups 1 / 2: softmax of query tile A / B.
-// Register budget (setmaxnreg, per warp group): 168 at launch -> 56 for group 0, 224 for the softmax groups
-// (4 x 32 x (56 + 224 + 224) = 64512 <= 65536).
-// exp2 of two values on the FMA pipe (Cody-Waite split + degree-4 minimax polynomial on [-0.5, 0.5], max relative error
-// 2.7e-6 -- far below the fp16 rounding of P): a share of the exponentials is taken off the MUFU unit, which at 16 per
-// clock per SM is the busiest unit of this kernel. Inputs are <= ~8; anything below -125 (masked keys) clamps to 2^-125,
-// which packs to an fp16 zero.
-__device__ __forceinline__ void ex2_poly_x2(float x0, float x1, float& p0, float& p1) {
-  const uint64_t x = pack_f32x2(fmaxf(x0, -125.0f), fmaxf(x1, -125.0f));
-  const uint64_t xf = add_f32x2(x, pack_f32x2(12582912.0f, 12582912.0f));          // integer part in the low mantissa bits
-  const uint64_t n = add_f32x2(xf, pack_f32x2(-12582912.0f, -12582912.0f));
-  const uint64_t f = fma_f32x2(n, pack_f32x2(-1.0f, -1.0f), x);                    // x - round(x) in [-0.5, 0.5]
-  uint64_t p = fma_f32x2(pack_f32x2(0.009570100344717503f, 0.009570100344717503f), f,
-                         pack_f32x2(0.05591786280274391f, 0.05591786280274391f));
-  p = fma_f32x2(p, f, pack_f32x2(0.240247443318367f, 0.240247443318367f));
-  p = fma_f32x2(p, f, pack_f32x2(0.6931217908859253f, 0.6931217908859253f));
-  p = fma_f32x2(p, f, pack_f32x2(0.9999992847442627f, 0.9999992847442627f));
-  float pa, pb, xa, xb;
-  unpack_f32x2(p, pa, pb);
-  unpack_f32x2(xf, xa, xb);
-  p0 = __int_as_float(__float_as_int(pa) + (__float_as_int(xa) << 23));             // p * 2^n through the exponent field
-  p1 = __int_as_float(__float_as_int(pb) + (__float_as_int(xb) << 23));
-}
-constexpr int FA_POLY_OF_4 = 1;   // of every 4 consecutive key pairs, this many go through ex2_poly_x2
-
-constexpr int FA_BM = 128, FA_BN = 128, FA_D = 64, FA_THREADS = 384;
+constexpr int FA_BM = 128, FA_BN = 128, FA_D = 64, FA_THREADS = 256;
 constexpr int FA_TILE = FA_BM * FA_D * 2;             // 16 KB: one [128 x 64] fp16 tile
-constexpr int FA_KV_STAGES = 3;
-// Q[g][2] | K ring | V ring | output staging[g] = 12 tiles = 192 KB (P never touches shared memory)
-constexpr int FA_SMEM = FA_TILE * (4 + 2 * FA_KV_STAGES + 2);
-constexpr int FA_TMEM_COLS = 512;
-constexpr int FA_S_COL = 0, FA_O_COL = 256, FA_P_COL = 384;   // S_A, S_B at 0 / 128; O_A, O_B at 256 / 320; P_A, P_B at 384 / 448
-constexpr float FA_RESCALE_LOG2 = 8.0f;       // raise the reference maximum only when exceeded by more than 2^8
-#ifdef DSS_ATTN_ABLATION
-__device__ long long* g_attn_trace = nullptr;   // tuning only: per-phase clock64 stamps of CTA 0
-#define FA_TRACE(slot) do { if (trace) trace[(slot)] = clock64(); } while (0)
-#else
-#define FA_TRACE(slot) do { } while (0)
-#endif
-constexpr int FA_NBARS = 8 + 2 * FA_KV_STAGES + 10;
+constexpr int FA_KV_STAGES = 2;
+// Q (reused as the output box) | K ring | V ring = 80 KB: two CTAs per SM
+constexpr int FA_SMEM = FA_TILE * (1 + 2 * FA_KV_STAGES) + 1024;
 
-// ABL: timing-ablation bits (tuning only; any non-zero value computes garbage): 1 no exp2, 2 no P stores / fence,
-// 4 no row maximum, 8 no P V MMAs, 16 no score MMAs, 32 no row sum
-template <int ABL>
-__global__ void __launch_bounds__(FA_THREADS, 1)
-attention_tcgen05_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO, int T, int heads,
-                         int nq2, int total_items, int flags) {
-  // flags (tuning switches, both on by default): 1 = rotate the query-pair index over the items, 2 = take the exponentials
-  // of tiles j > 0 against the reference maximum of the earlier tiles (no separate row-maximum pass)
-  const bool f_rotate = flags & 1, f_lazy = flags & 2;
-  extern __shared__ __align__(1024) uint8_t fa_smem[];
-  __shared__ __align__(8) uint64_t bars[FA_NBARS];
-  __shared__ uint32_t tmem_ptr_s;
-
-  const uint32_t base = smem_u32(fa_smem);
-  if ((base & 1023u) != 0) __trap();  // the 128 B swizzle pattern is a function of address bits [7,10)
-  const uint32_t sQ = base, sK = base + 4 * FA_TILE, sV = sK + FA_KV_STAGES * FA_TILE, sO = sV + FA_KV_STAGES * FA_TILE;
+__global__ void __launch_bounds__(FA_THREADS, 2)
+attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO, int T,
+                       int heads) {
+  extern __shared__ uint8_t fa_smem[];
+  __shared__ __align__(8) uint64_t bars[1 + 2 * FA_KV_STAGES];
+  const uint32_t raw = smem_u32(fa_smem);
+  const uint32_t base = (raw + 1023u) & ~1023u;   // the 128 B swizzle pattern is a function of address bits [7,10)
+  const uint32_t sQ = base, sK = base + FA_TILE, sV = sK + FA_KV_STAGES * FA_TILE;
   const uint32_t bar0 = smem_u32(bars);
-  auto q_full = [&](int g, int i) { return bar0 + 8u * (g * 2 + i); };
-  auto q_empty = [&](int g, int i) { return bar0 + 8u * (4 + g * 2 + i); };
-  auto kv_full = [&](int s) { return bar0 + 8u * (8 + s); };
-  auto kv_empty = [&](int s) { return bar0 + 8u * (8 + FA_KV_STAGES + s); };
-  auto s_full = [&](int g) { return bar0 + 8u * (8 + 2 * FA_KV_STAGES + g); };
-  auto p_full = [&](int g) { return bar0 + 8u * (10 + 2 * FA_KV_STAGES + g); };
-  auto o_full = [&](int g) { return bar0 + 8u * (12 + 2 * FA_KV_STAGES + g); };
-  auto s_free = [&](int g) { return bar0 + 8u * (16 + 2 * FA_KV_STAGES + g); };
+  const uint32_t q_full = bar0;
+  auto kv_full = [&](int s) { return bar0 + 8u * (1 + s); };
+  auto kv_empty = [&](int s) { return bar0 + 8u * (1 + FA_KV_STAGES + s); };
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#ifdef DSS_ATTN_ABLATION
-  long long* trace = (blockIdx.x == 0 && lane == 0 && (warp == 1 || warp == 2 || warp >= 4)) ? g_attn_trace : nullptr;
-#endif
+  const int tid = threadIdx.x, lane = tid & 31;
+  const int wg = tid >> 7, wi = (tid >> 5) & 3;
+  const int q0 = blockIdx.x * FA_BM, h = blockIdx.y, b = blockIdx.z;
   const int d = heads * FA_D;
   const int nt = (T + FA_BN - 1) / FA_BN;
-  const int kc_last = (T - (nt - 1) * FA_BN + 15) & ~15;   // key columns of the last tile that are worth computing
+  const int row0 = b * T;   // first row of this image in [B*T, 3d]
 
-  if (warp == 0 && lane == 0) {
+  auto load_kv = [&](int j) {
+    const int s = j % FA_KV_STAGES;
+    mbar_arrive_expect_tx(kv_full(s), 2 * FA_TILE);
+    tma_load_2d(sK + s * FA_TILE, &tmQKV, kv_full(s), d + h * FA_D, row0 + j * FA_BN);
+    tma_load_2d(sV + s * FA_TILE, &tmQKV, kv_full(s), 2 * d + h * FA_D, row0 + j * FA_BN);
+  };
+  if (tid == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmO);
-    for (int i = 0; i < 4; ++i) {
-      mbar_init(q_full(i >> 1, i & 1), 1);
-      mbar_init(q_empty(i >> 1, i & 1), 1);
-    }
+    mbar_init(q_full, 1);
     for (int s = 0; s < FA_KV_STAGES; ++s) {
       mbar_init(kv_full(s), 1);
-      mbar_init(kv_empty(s), 2);   // one commit per query tile's MMA warp
-    }
-    for (int g = 0; g < 2; ++g) {
-      mbar_init(s_full(g), 1);
-      mbar_init(p_full(g), 4);   // one arrival per softmax warp: 128 per-thread arrivals on one barrier serialise
-      mbar_init(s_free(g), 4);   // (measured: ~1300 cycles until the phase flips)
-      mbar_init(o_full(g), 1);
+      mbar_init(kv_empty(s), 2);   // one arrival per warp group
     }
     mbar_fence_init();
+    mbar_arrive_expect_tx(q_full, FA_TILE);
+    tma_load_2d(sQ, &tmQKV, q_full, h * FA_D, row0 + q0);
+    for (int j = 0; j < FA_KV_STAGES && j < nt; ++j) load_kv(j);
   }
-  if (warp == 1) {
-    tmem_alloc(smem_u32(&tmem_ptr_s), FA_TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(&tmem_ptr_s);
 
-  // Producer and MMA warps run their loops with ALL lanes on warp-uniform values and let one elected lane issue: the
-  // smem addresses, coordinates and descriptors then live in uniform registers and each UMMA / TMA issue is a couple
-  // of instructions instead of a register-to-uniform "waterfall" loop.
-  if (warp < 4) {
-  asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-  if (warp == 0) {
-    const uint32_t uQ = __shfl_sync(0xffffffffu, sQ, 0), uK = __shfl_sync(0xffffffffu, sK, 0),
-                   uV = __shfl_sync(0xffffffffu, sV, 0);
-    int s = 0;
-    uint32_t ph = 0;   // K/V ring position, carried across items
-    int qi = 0;        // item counter of this CTA
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x, ++qi) {
-      // item w -> (image * heads + head, pair of query tiles). The pair index is rotated by the (image, head) index:
-      // with the plain w % nq2 a CTA (w = blockIdx + k * 148, 148 % 4 == 0) would get the SAME pair index in every item,
-      // and the CTAs that only ever see the light last pair (a 5-row tail tile at T = 901) idle at the end of the
-      // kernel while the others are still on full pairs (ncu: 8.5 % of the stall samples on EXIT)
-      const int bh = w / nq2, qp = f_rotate ? (w % nq2 + bh) % nq2 : w % nq2;
-      const int h = bh % heads, row0 = (bh / heads) * T;   // first row of this image in the [B*T, 3d] matrix
-      const int qb = qi & 1;
-      const uint32_t qph = (qi >> 1) & 1;
+  // softmax in base 2: p = 2^(s c - m c), c = log2(e) / sqrt(64)
+  const float sc = 1.4426950408889634f * 0.125f;
+  const int fc = 2 * (lane & 3);                    // column of this thread inside an 8-column block
+  float m_run[2] = {-INFINITY, -INFINITY};           // rows lane/4 and lane/4 + 8 of this warp's 16
+  float l_run[2] = {0.f, 0.f};
+  float o[32];
 #pragma unroll
-      for (int g = 0; g < 2; ++g) {
-        mbar_wait(q_empty(g, qb), qph ^ 1u);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(q_full(g, qb), FA_TILE);
-          tma_load_2d(uQ + (g * 2 + qb) * FA_TILE, &tmQKV, q_full(g, qb), h * FA_D, row0 + (2 * qp + g) * FA_BM);
-        }
-        __syncwarp();
-      }
-      for (int j = 0; j < nt; ++j) {
-        mbar_wait(kv_empty(s), ph ^ 1u);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(kv_full(s), 2 * FA_TILE);
-          tma_load_2d(uK + s * FA_TILE, &tmQKV, kv_full(s), d + h * FA_D, row0 + j * FA_BN);
-          tma_load_2d(uV + s * FA_TILE, &tmQKV, kv_full(s), 2 * d + h * FA_D, row0 + j * FA_BN);
-        }
-        __syncwarp();
-        if (++s == FA_KV_STAGES) { s = 0; ph ^= 1u; }
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  const uint64_t qdesc = wgmma_desc_sw128(sQ + wg * 64 * 128);
+  mbar_wait(q_full, 0);
+  __syncwarp();
+
+  for (int j = 0; j < nt; ++j) {
+    const int s = j % FA_KV_STAGES;
+    mbar_wait(kv_full(s), (j / FA_KV_STAGES) & 1);
+    __syncwarp();   // wgmma is warp-aligned: reconverge after the per-thread barrier spin / thread 0's refill
+    float sacc[64];
+    const uint64_t kdesc = wgmma_desc_sw128(sK + s * FA_TILE);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < FA_D / 16; ++k) wgmma_m64n128_ss(sacc, qdesc + 2u * k, kdesc + 2u * k, k != 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(sacc);
+    // mask keys beyond T (only the last tile can be partial)
+    const int kbase = j * FA_BN;
+    if (kbase + FA_BN > T) {
+#pragma unroll
+      for (int i = 0; i < 16; ++i) {
+        const int key = kbase + 8 * i + fc;
+        if (key >= T) sacc[4 * i] = sacc[4 * i + 2] = -INFINITY;
+        if (key + 1 >= T) sacc[4 * i + 1] = sacc[4 * i + 3] = -INFINITY;
       }
     }
-  } else if (warp == 1 || warp == 2) {
-    // one MMA-issuing warp per query tile (a single warp serving both tiles was the bottleneck of the kernel: ~1000
-    // cycles per batch of UMMAs, four batches per step). Per tile the events strictly alternate in time
-    // (S_g released early in key tile n, P_g published at its end), so plain blocking waits in program order suffice.
-    const int g = warp - 1;
-    constexpr uint32_t idesc_qk0 = umma_idesc_f16(FA_BM, 0);                    // A, B K-major; N filled in per tile
-    constexpr uint32_t idesc_pv = umma_idesc_f16(FA_BM, FA_D) | (1u << 16);     // B (= V) MN-major
-    const uint32_t uQ = __shfl_sync(0xffffffffu, sQ, 0) + g * 2 * FA_TILE, uK = __shfl_sync(0xffffffffu, sK, 0),
-                   uV = __shfl_sync(0xffffffffu, sV, 0),
-                   utmem = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const uint32_t s_acc = utmem + FA_S_COL + g * FA_BN, o_acc = utmem + FA_O_COL + g * FA_D;
-    const uint32_t p_tm = utmem + FA_P_COL + g * (FA_BN / 2);   // P_g: 128 rows x 128 fp16 = 64 columns
-    const int my_items = (total_items - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) /
-                         static_cast<int>(gridDim.x);
-    const int m_total = my_items * nt;   // key-tile steps of this CTA, over all of its items
-    int sj = 0, sq = 0, ss = 0;          // cursor of the next score tile: key tile, item, ring stage
-    uint32_t sph = 0;
-    auto issue_s = [&]() {   // S_g = Q_g K_j^T
-      if (sj == 0) mbar_wait(q_full(g, sq & 1), (sq >> 1) & 1);
-      mbar_wait(kv_full(ss), sph);
-      tc_fence_after();
-      const uint64_t qdesc = umma_desc_sw128(uQ + (sq & 1) * FA_TILE);
-      const uint64_t kdesc = umma_desc_sw128(uK + ss * FA_TILE);
-      const int kc = sj == nt - 1 ? kc_last : FA_BN;
-      const uint32_t idesc = idesc_qk0 | (static_cast<uint32_t>(kc >> 3) << 17);
-      if (elect_one()) {
+    float mx[2] = {m_run[0], m_run[1]};
 #pragma unroll
-        for (int k = 0; k < FA_D / 16; ++k)   // +32 B per 16-wide K step = +2 in the descriptor's address field
-          if (!(ABL & 16)) umma_f16_ss(s_acc, qdesc + 2u * k, kdesc + 2u * k, idesc, k != 0 ? 1u : 0u);
-        umma_commit(s_full(g));
-        if (sj == nt - 1) umma_commit(q_empty(g, sq & 1));   // last score tile of the item: Q_g may be replaced
-      }
-      __syncwarp();
-      if (++sj == nt) { sj = 0; ++sq; }
-      if (++ss == FA_KV_STAGES) { ss = 0; sph ^= 1u; }
-    };
-    if (m_total > 0) issue_s();
-    int pj = 0, ps = 0;
-    for (int n = 0; n < m_total; ++n) {
-      if (n + 1 < m_total) {   // S_g(n+1) as soon as the softmax warps hold S_g(n) in registers
-        mbar_wait(s_free(g), n & 1);
-        FA_TRACE(8192 + g * 2048 + (n < 500 ? n : 500) * 4 + 0);
-        issue_s();
-        FA_TRACE(8192 + g * 2048 + (n < 500 ? n : 500) * 4 + 1);
-      }
-      // O_g (+)= P_g V_j once the softmax warps have published P_g(n) (and rescaled O_g if they had to)
-      mbar_wait(p_full(g), n & 1);
-      tc_fence_after();
-      FA_TRACE(8192 + g * 2048 + (n < 500 ? n : 500) * 4 + 2);
-      const int ksteps = (pj == nt - 1 ? kc_last : FA_BN) >> 4;
-      const uint64_t vdesc = umma_desc_sw128(uV + ps * FA_TILE);   // +16 key rows = +2048 B = +128
-      const bool first = pj == 0;   // first key tile of the item: overwrite
-      if (elect_one()) {
+    for (int i = 0; i < 16; ++i) {
+      mx[0] = fmaxf(mx[0], fmaxf(sacc[4 * i], sacc[4 * i + 1]));
+      mx[1] = fmaxf(mx[1], fmaxf(sacc[4 * i + 2], sacc[4 * i + 3]));
+    }
+    float corr[2], msc[2];
 #pragma unroll
-        for (int k = 0; k < FA_BN / 16; ++k)
-          if (k < ksteps && !(ABL & 8))
-            umma_f16_ts(o_acc, p_tm + 8u * k, vdesc + 128u * k, idesc_pv, (k != 0 || !first) ? 1u : 0u);
-        umma_commit(o_full(g));
-        umma_commit(kv_empty(ps));   // this query tile is done with K_j / V_j (the ring slot needs both tiles' commits)
-      }
-      __syncwarp();
-      FA_TRACE(8192 + g * 2048 + (n < 500 ? n : 500) * 4 + 3);
-      if (++pj == nt) pj = 0;
-      if (++ps == FA_KV_STAGES) ps = 0;
+    for (int r = 0; r < 2; ++r) {
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+      corr[r] = ex2_approx((m_run[r] - mx[r]) * sc);   // first tile: 2^-inf = 0
+      m_run[r] = mx[r];
+      msc[r] = mx[r] * sc;
+      l_run[r] *= corr[r];
+    }
+    // accumulator layout of two adjacent 8-key blocks == register A-operand layout of one 16-key step
+    uint32_t pf[8][4];
+    float rs[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const float p0 = ex2_approx(fmaf(sacc[4 * i], sc, -msc[0]));
+      const float p1 = ex2_approx(fmaf(sacc[4 * i + 1], sc, -msc[0]));
+      const float p2 = ex2_approx(fmaf(sacc[4 * i + 2], sc, -msc[1]));
+      const float p3 = ex2_approx(fmaf(sacc[4 * i + 3], sc, -msc[1]));
+      rs[0] += p0 + p1;
+      rs[1] += p2 + p3;
+      pf[i >> 1][(i & 1) * 2 + 0] = pack_half2(p0, p1);
+      pf[i >> 1][(i & 1) * 2 + 1] = pack_half2(p2, p3);
+    }
+    l_run[0] += rs[0];
+    l_run[1] += rs[1];
+#pragma unroll
+    for (int i = 0; i < 8; ++i) {
+      o[4 * i] *= corr[0]; o[4 * i + 1] *= corr[0];
+      o[4 * i + 2] *= corr[1]; o[4 * i + 3] *= corr[1];
+    }
+    const uint64_t vdesc = wgmma_desc_sw128(sV + s * FA_TILE);   // +16 key rows = +2048 B
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < FA_BN / 16; ++ks) wgmma_m64n64_rs_tb(o, pf[ks], vdesc + 128u * ks);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(o);
+    // this warp group is done with K_j / V_j; thread 0 refills the slot once both groups are
+    __syncwarp();
+    if ((tid & 127) == 0) mbar_arrive(kv_empty(s));
+    if (tid == 0 && j + FA_KV_STAGES < nt) {
+      mbar_wait(kv_empty(s), (j / FA_KV_STAGES) & 1);
+      load_kv(j + FA_KV_STAGES);
     }
   }
-  } else {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    const int g = (warp - 4) >> 2;        // query tile of the pair
-    const int q = warp & 3;               // TMEM lane quarter this warp may access
-    const int r = q * 32 + lane;          // query row inside the tile
-    const uint32_t lane_addr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    const uint32_t s_col = lane_addr + FA_S_COL + g * FA_BN;
-    const uint32_t o_col = lane_addr + FA_O_COL + g * FA_D;
-    const uint32_t p_col = lane_addr + FA_P_COL + g * (FA_BN / 2);   // this row of P_g (fp16 pairs, 64 columns)
-    const float sc = 1.4426950408889634f * 0.125f;  // log2(e) / sqrt(64)
-    uint32_t m = 0;   // key-tile step counter of this CTA (all barrier phases derive from it)
-    for (int w = blockIdx.x; w < total_items; w += gridDim.x) {
-      // item w -> (image * heads + head, pair of query tiles). The pair index is rotated by the (image, head) index:
-      // with the plain w % nq2 a CTA (w = blockIdx + k * 148, 148 % 4 == 0) would get the SAME pair index in every item,
-      // and the CTAs that only ever see the light last pair (a 5-row tail tile at T = 901) idle at the end of the
-      // kernel while the others are still on full pairs (ncu: 8.5 % of the stall samples on EXIT)
-      const int bh = w / nq2, qp = f_rotate ? (w % nq2 + bh) % nq2 : w % nq2;
-      const int h = bh % heads;
-      const int q0 = (2 * qp + g) * FA_BM;
-      const bool dead = q0 >= T || ((ABL & 64) && g == 1);   // odd number of query tiles: nothing to do for B in the last pair
-      // a warp whose 32 query rows all lie beyond T (T = 901: three of the four warps of the 8th tile, which has 5 live
-      // rows) only keeps the barrier protocol going: its exponentials would occupy the MUFU unit -- the busiest unit of
-      // the kernel -- for rows the output tensor map clips anyway
-      const bool wdead = dead || q0 + q * 32 >= T;
-      float m_ref = -INFINITY, l_run = 0.f;   // reference maximum of the exponent, row sum relative to it
-      for (int j = 0; j < nt; ++j, ++m) {
-        // tile B starts every item half a key tile behind tile A (A signals from the middle of its first tile): left
-        // alone, the two groups drift into lock step within ~10 items and both sit in their MUFU phase together
-        if (j == 0 && g == 1) { __syncwarp(); asm volatile("bar.sync 3, 256;" ::: "memory"); }
-        mbar_wait(s_full(g), m & 1);
-        tc_fence_after();
-        [[maybe_unused]] const int tb = (warp - 4) * 1024 + (m < 120 ? m : 120) * 8;   // trace slot (ablation builds)
-        FA_TRACE(tb + 0);
-        if (!wdead) {
-          // one key tile, in four chunks of 32 key columns; only the last tile of a row of tiles can be short
-          // (kc < 128 columns computed, nvalid <= kc of them real keys)
-          const bool tail = j == nt - 1 && (T & (FA_BN - 1)) != 0;
-          const int kc = tail ? kc_last : FA_BN;
-          const int nvalid = tail ? T - j * FA_BN : FA_BN;
-          uint32_t v[128];
-          float mxc[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};   // four independent maximum chains
-          uint64_t rs2[2] = {0ull, 0ull};                                 // packed partial row sums, two chains
-          // chunk c of the tile: (tail mask) -> running maximum of the raw scores -> P = 2^(s*c - m_ref*c) -> row sum
-          // -> packed fp16 pairs into TMEM (the A operand of the P V product). The maximum is tracked alongside the
-          // exponentials (FMNMX3 on the ALU pipe) instead of in a pass of its own.
-          auto chunk = [&](const int c, const float msc, const bool track_max) {
-            if (tail) {   // keys beyond T: score -inf -> probability exactly 0
+
+  // finalise: row sums across the 4 lanes of a quad, normalise, fp16 into this group's half of the Q tile (swizzled
+  // as the output box), one TMA store of the 128 x 64 box
 #pragma unroll
-              for (int i = c * 32; i < c * 32 + 32; ++i)
-                if (i >= nvalid) v[i] = 0xff800000u;
-            }
-            if (track_max) {
-#pragma unroll
-              for (int i = c * 32; i < c * 32 + 32; ++i)
-                if (!(ABL & 4)) mxc[i & 3] = fmaxf(mxc[i & 3], __uint_as_float(v[i]));
-            }
-            const uint64_t sc2 = pack_f32x2(sc, sc), nmsc2 = pack_f32x2(-msc, -msc);
-            uint32_t pk[16];
-#pragma unroll
-            for (int e = 0; e < 32; e += 2) {
-              const int i = c * 32 + e;
-              float x0, x1;
-              unpack_f32x2(fma_f32x2(pack_f32x2(__uint_as_float(v[i]), __uint_as_float(v[i + 1])), sc2, nmsc2), x0, x1);
-              constexpr int npoly = (ABL & 1024) ? 0 : ((ABL >> 8) & 3) ? ((ABL >> 8) & 3) : FA_POLY_OF_4;
-              float p0, p1;
-              if (((e >> 1) & 3) < npoly) {
-                ex2_poly_x2(x0, x1, p0, p1);
-              } else {
-                p0 = (ABL & 1) ? x0 : ex2_approx(x0);
-                p1 = (ABL & 1) ? x1 : ex2_approx(x1);
-              }
-              if (!(ABL & 32)) rs2[(e >> 1) & 1] = add_f32x2(rs2[(e >> 1) & 1], pack_f32x2(p0, p1));
-              pk[e >> 1] = pack_half2(p0, p1);
-            }
-            if (!(ABL & 2)) tmem_st_32x16(p_col + c * 16, pk);
-            else rs2[0] += pk[0] ^ pk[5] ^ pk[10] ^ pk[15];   // keep the values alive
-          };
-#pragma unroll
-          for (int c = 0; c < 4; ++c)
-            if (c * 32 < kc) tmem_ld_32x32(s_col + c * 32, *reinterpret_cast<uint32_t (*)[32]>(&v[c * 32]));
-          tmem_ld_wait();
-          FA_TRACE(tb + 1);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(s_free(g));   // S_g is in registers: the next score tile may overwrite it
-          if (j == 0 || !f_lazy) {
-            // ---- the row maximum first (always for the first key tile of an item: there is no reference yet)
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              if (c * 32 < kc) {
-#pragma unroll
-                for (int i = c * 32; i < c * 32 + 32; ++i) {
-                  if (tail && i >= nvalid) v[i] = 0xff800000u;
-                  if (!(ABL & 4)) mxc[i & 3] = fmaxf(mxc[i & 3], __uint_as_float(v[i]));
-                }
-              }
-            }
-            const float mx = fmaxf(fmaxf(mxc[0], mxc[1]), fmaxf(mxc[2], mxc[3]));
-            FA_TRACE(tb + 2);
-            if (j > 0) {
-              // P_g is single buffered and O_g accumulates in place: P_g V_{j-1} must be complete (issued long ago)
-              mbar_wait(o_full(g), (m - 1) & 1);
-              tc_fence_after();
-              const bool raise = (mx - m_ref) * sc > FA_RESCALE_LOG2;
-              if (__any_sync(0xffffffffu, raise)) {   // rare: rescale this warp's rows of O_g in TMEM
-                const float f = raise ? ex2_approx((m_ref - mx) * sc) : 1.0f;
-                uint32_t t[32];
-#pragma unroll
-                for (int c = 0; c < 2; ++c) {
-                  tmem_ld_32x32(o_col + c * 32, t);
-                  tmem_ld_wait();
-#pragma unroll
-                  for (int i = 0; i < 32; ++i) t[i] = __float_as_uint(__uint_as_float(t[i]) * f);
-                  tmem_st_32x32(o_col + c * 32, t);
-                }
-                tmem_st_wait();
-                l_run *= f;
-                if (raise) m_ref = mx;
-              }
-            } else {
-              m_ref = mx;
-            }
-            FA_TRACE(tb + 3);
-            const float msc = m_ref * sc;
-#pragma unroll
-            for (int c = 0; c < 4; ++c) {
-              if (c * 32 < kc) {
-                chunk(c, msc, false);
-                // release tile B's first key tile when tile A is half way through its first exponentials: the two
-                // groups then stay about half a period apart (one in its MUFU phase, the other loading / reducing)
-                if (c == 1 && j == 0 && g == 0) { __syncwarp(); asm volatile("bar.arrive 3, 256;" ::: "memory"); }
-              }
-            }
-            if (kc <= 32 && j == 0 && g == 0) { __syncwarp(); asm volatile("bar.arrive 3, 256;" ::: "memory"); }   // (short first tile)
-          } else {
-            // ---- later key tiles: exponentials are taken relative to the reference maximum of the EARLIER tiles right
-            // away (softmax is shift invariant; fp16 P and the fp32 sums have 2^8 of headroom) with the row maximum
-            // tracked alongside (FMNMX3, ALU pipe); only if this tile turns out to exceed the reference by more than
-            // 2^8 is the reference raised and the tile redone (rare).
-            mbar_wait(o_full(g), (m - 1) & 1);   // P_g is single buffered: P_g V_{j-1} must be complete
-            tc_fence_after();
-            FA_TRACE(tb + 2);
-            float msc = m_ref * sc;
-#pragma unroll
-            for (int c = 0; c < 4; ++c)
-              if (c * 32 < kc) chunk(c, msc, true);
-            FA_TRACE(tb + 3);
-            const float mx = fmaxf(fmaxf(mxc[0], mxc[1]), fmaxf(mxc[2], mxc[3]));
-            const bool raise = (mx - m_ref) * sc > FA_RESCALE_LOG2;
-            if (__any_sync(0xffffffffu, raise)) {   // rare: rescale this warp's rows of O_g in TMEM, redo the tile
-              const float f = raise ? ex2_approx((m_ref - mx) * sc) : 1.0f;
-              tmem_st_wait();
-              uint32_t t[32];
-#pragma unroll
-              for (int c = 0; c < 2; ++c) {
-                tmem_ld_32x32(o_col + c * 32, t);
-                tmem_ld_wait();
-#pragma unroll
-                for (int i = 0; i < 32; ++i) t[i] = __float_as_uint(__uint_as_float(t[i]) * f);
-                tmem_st_32x32(o_col + c * 32, t);
-              }
-              tmem_st_wait();
-              l_run *= f;
-              if (raise) m_ref = mx;
-              msc = m_ref * sc;
-              rs2[0] = rs2[1] = 0ull;
-#pragma unroll
-              for (int c = 0; c < 4; ++c)
-                if (c * 32 < kc) chunk(c, msc, false);
-            }
-          }
-          float rs, rs_hi;
-          unpack_f32x2(add_f32x2(rs2[0], rs2[1]), rs, rs_hi);
-          rs += rs_hi;
-          FA_TRACE(tb + 4);
-          l_run += rs;
-          tmem_st_wait();
-          tc_fence_before();          // order this thread's TMEM accesses before the MMA that accumulates into O_g
-          __syncwarp();
-          if (lane == 0) mbar_arrive(p_full(g));
-          FA_TRACE(tb + 5);
-        } else {
-          // nothing to compute, but keep the protocol: P_g(m) may only be announced once P_g V(m-1) has been issued
-          // (the MMA warp probes p_full by parity and must never be lapped by two phases)
-          if (j == 0 && g == 0) { __syncwarp(); asm volatile("bar.arrive 3, 256;" ::: "memory"); }   // tile B's start signal (see above)
-          if (m > 0) mbar_wait(o_full(g), (m - 1) & 1);
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) {
-            mbar_arrive(s_free(g));
-            mbar_arrive(p_full(g));
-          }
-        }
-      }
-      if (!wdead) {
-        mbar_wait(o_full(g), (m - 1) & 1);   // last P V product of this item
-        tc_fence_after();
-        uint32_t t[FA_D];
-        tmem_ld_32x32(o_col, *reinterpret_cast<uint32_t (*)[32]>(&t[0]));
-        tmem_ld_32x32(o_col + 32, *reinterpret_cast<uint32_t (*)[32]>(&t[32]));
-        tmem_ld_wait();
-        tc_fence_before();
-        float inv;
-        asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(inv) : "f"(l_run));
-        // normalised [128 x 64] fp16 tile -> swizzled staging tile -> one TMA store (rows >= T are clipped by the
-        // 3D tensor map). The elected thread first makes sure the previous item's store has finished reading.
-        if (q == 0 && lane == 0) tma_store_wait_read<0>();
-        __syncwarp();   // named barriers are warp-aligned: reconverge after lane-conditional code
-        asm volatile("bar.sync %0, 128;" ::"r"(4 + g) : "memory");
-        const uint32_t srow = sO + g * FA_TILE + r * 128;
-#pragma unroll
-        for (int i = 0; i < FA_D; i += 8) {
-          const uint32_t w0 = pack_half2(__uint_as_float(t[i + 0]) * inv, __uint_as_float(t[i + 1]) * inv);
-          const uint32_t w1 = pack_half2(__uint_as_float(t[i + 2]) * inv, __uint_as_float(t[i + 3]) * inv);
-          const uint32_t w2 = pack_half2(__uint_as_float(t[i + 4]) * inv, __uint_as_float(t[i + 5]) * inv);
-          const uint32_t w3 = pack_half2(__uint_as_float(t[i + 6]) * inv, __uint_as_float(t[i + 7]) * inv);
-          asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(srow + ((((i >> 3) ^ (r & 7))) << 4)), "r"(w0),
-                       "r"(w1), "r"(w2), "r"(w3)
-                       : "memory");
-        }
-        fence_proxy_async_smem();
-        __syncwarp();   // named barriers are warp-aligned: reconverge after lane-conditional code
-        asm volatile("bar.sync %0, 128;" ::"r"(4 + g) : "memory");
-        if (q == 0 && lane == 0) {
-          tma_store_3d(&tmO, sO + g * FA_TILE, h * FA_D, q0, bh / heads);
-          tma_store_commit();
-        }
-      } else if (!dead) {
-        // rows beyond T inside a live tile (never lane quarter 0): only the two staging-tile barriers of the group
-        __syncwarp();   // named barriers are warp-aligned: reconverge after lane-conditional code
-        asm volatile("bar.sync %0, 128;" ::"r"(4 + g) : "memory");
-        __syncwarp();   // named barriers are warp-aligned: reconverge after lane-conditional code
-        asm volatile("bar.sync %0, 128;" ::"r"(4 + g) : "memory");
-      }
-    }
-    if (q == 0 && lane == 0) tma_store_wait_all<0>();   // the staging tile must outlive the last store
+  for (int r = 0; r < 2; ++r) {
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
+    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
   }
-  tc_fence_before();
+  const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
+  const int r0 = 64 * wg + 16 * wi + (lane >> 2);
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int row = r0 + 8 * hh;
+      const float inv = hh ? inv1 : inv0;
+      const uint32_t addr = sQ + row * 128 + ((i ^ (row & 7)) << 4) + (lane & 3) * 4;
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_half2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv))
+                   : "memory");
+    }
+  }
+  fence_proxy_async_smem();
   __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, FA_TMEM_COLS);
+  if (tid == 0) {
+    tma_store_3d(&tmO, sQ, h * FA_D, q0, b);
+    tma_store_commit();
+    tma_store_wait_all<0>();
+  }
 }
 
 int launch_attention_tc(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st) {
   DSS_REQUIRE(B > 0 && T > 0 && heads > 0, "attention: empty problem");
-  static int flags = 3;
-  static int abl = -1;
-  if (abl < 0) {
-    if (const char* e = getenv("DSS_ATTN_FLAGS")) flags = atoi(e);   // tuning: bit 0 item rotation, bit 1 lazy reference
-    const char* e = getenv("DSS_ATTN_ABL");   // tuning only
-    abl = e ? atoi(e) : 0;
-    DSS_CHECK_CUDA(cudaFuncSetAttribute(attention_tcgen05_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
-#ifdef DSS_ATTN_ABLATION
-#define DSS_ABL_ATTR(n) DSS_CHECK_CUDA(cudaFuncSetAttribute(attention_tcgen05_kernel<n>, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
-    DSS_ABL_ATTR(1) DSS_ABL_ATTR(2) DSS_ABL_ATTR(4) DSS_ABL_ATTR(8) DSS_ABL_ATTR(16) DSS_ABL_ATTR(32) DSS_ABL_ATTR(3) DSS_ABL_ATTR(7) DSS_ABL_ATTR(39) DSS_ABL_ATTR(24) DSS_ABL_ATTR(63) DSS_ABL_ATTR(64) DSS_ABL_ATTR(65) DSS_ABL_ATTR(127) DSS_ABL_ATTR(88) DSS_ABL_ATTR(256) DSS_ABL_ATTR(512) DSS_ABL_ATTR(768) DSS_ABL_ATTR(1024)
-#endif
+  static bool attr_set = false;
+  if (!attr_set) {
+    DSS_CHECK_CUDA(cudaFuncSetAttribute(attention_wgmma_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FA_SMEM));
+    attr_set = true;
   }
   CUtensorMap tm, tmO;
   int rc = make_tmap_f16(&tm, qkv, B * T, 3 * heads * FA_D, FA_BM);
   if (rc) return rc;
   if ((rc = make_tmap_out3d_f16(&tmO, out, B, T, heads * FA_D))) return rc;
-  static int sm_count = 0;
-  if (!sm_count) {
-    int dev = 0;
-    DSS_CHECK_CUDA(cudaGetDevice(&dev));
-    DSS_CHECK_CUDA(cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev));
-  }
-  const int nq2 = cdiv(cdiv(T, FA_BM), 2);   // pairs of 128-query tiles per (image, head)
-  const int total = B * heads * nq2;
-  const int grid = total < sm_count ? total : sm_count;   // persistent: one CTA per SM
+  dim3 grid(cdiv(T, FA_BM), heads, B);
   LaunchScope scope(st, KC_ATTENTION);
-#ifdef DSS_ATTN_ABLATION
-  static long long* trace_dev = nullptr;
-  const char* trace_path = getenv("DSS_ATTN_TRACE");
-  if (trace_path && !trace_dev) {
-    DSS_CHECK_CUDA(cudaMalloc(&trace_dev, 16384 * sizeof(long long)));
-    DSS_CHECK_CUDA(cudaMemset(trace_dev, 0, 16384 * sizeof(long long)));
-    DSS_CHECK_CUDA(cudaMemcpyToSymbol(g_attn_trace, &trace_dev, sizeof(trace_dev)));
-  }
-#define DSS_ABL_CASE(n) case n: attention_tcgen05_kernel<n><<<grid, FA_THREADS, FA_SMEM, st>>>(tm, tmO, T, heads, nq2, total, flags); break;
-  switch (abl) {
-    DSS_ABL_CASE(1) DSS_ABL_CASE(2) DSS_ABL_CASE(4) DSS_ABL_CASE(8) DSS_ABL_CASE(16) DSS_ABL_CASE(32) DSS_ABL_CASE(3) DSS_ABL_CASE(7) DSS_ABL_CASE(39) DSS_ABL_CASE(24) DSS_ABL_CASE(63) DSS_ABL_CASE(64) DSS_ABL_CASE(65) DSS_ABL_CASE(127) DSS_ABL_CASE(88) DSS_ABL_CASE(256) DSS_ABL_CASE(512) DSS_ABL_CASE(768) DSS_ABL_CASE(1024)
-    default: attention_tcgen05_kernel<0><<<grid, FA_THREADS, FA_SMEM, st>>>(tm, tmO, T, heads, nq2, total, flags);
-  }
-  if (trace_path) {
-    static long long host[16384];
-    DSS_CHECK_CUDA(cudaStreamSynchronize(st));
-    DSS_CHECK_CUDA(cudaMemcpy(host, trace_dev, sizeof(host), cudaMemcpyDeviceToHost));
-    FILE* f = fopen(trace_path, "wb");
-    if (f) { fwrite(host, sizeof(host), 1, f); fclose(f); }
-  }
-#else
-  attention_tcgen05_kernel<0><<<grid, FA_THREADS, FA_SMEM, st>>>(tm, tmO, T, heads, nq2, total, flags);
-#endif
+  attention_wgmma_kernel<<<grid, FA_THREADS, FA_SMEM, st>>>(tm, tmO, T, heads);
   DSS_CHECK_CUDA(cudaGetLastError());
   return DSS_OK;
 }

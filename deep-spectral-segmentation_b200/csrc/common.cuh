@@ -1,5 +1,5 @@
-// Shared device/host helpers for libdss_b200 (sm_100a only).
-// PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA + TMEM), cp.async, ldmatrix, mma.sync.
+// Shared device/host helpers for libdss_b200 (sm_90a only).
+// PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor), wgmma, cp.async, ldmatrix, mma.sync.
 #pragma once
 #include <cuda.h>  // CUtensorMap (types only; the driver entry point is resolved at run time, no -lcuda)
 #include <cuda_fp16.h>
@@ -8,8 +8,8 @@
 
 #include "../../include/dss_b200.h"
 
-#if defined(__CUDA_ARCH__) && !defined(__CUDA_ARCH_FEAT_SM100_ALL)
-#error "libdss_b200 is written for sm_100a only: compile with -gencode arch=compute_100a,code=sm_100a"
+#if defined(__CUDA_ARCH__) && !defined(__CUDA_ARCH_FEAT_SM90_ALL)
+#error "libdss_b200 is written for sm_90a only: compile with -gencode arch=compute_90a,code=sm_90a"
 #endif
 
 namespace dss {
@@ -174,6 +174,15 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// arrive on the mbarrier at this shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(bar), "r"(rank)
+      : "memory");
+}
 // 2D tiled load, multicast: the box lands at the same shared-memory offset in every CTA of `cta_mask`, and each
 // destination CTA's mbarrier (same offset) receives the complete_tx for the bytes written into that CTA
 __device__ __forceinline__ void tma_load_2d_mc(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1,
@@ -186,165 +195,78 @@ __device__ __forceinline__ void tma_load_2d_mc(uint32_t smem_dst, const CUtensor
       : "memory");
 }
 
-// ---- tcgen05 / TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols)
-               : "memory");
+// ---- wgmma (warp-group MMA): D[64 x N] (+)= A[64 x 16] * B[16 x N], fp16 operands, fp32 accumulators in registers.
+// Accumulator layout (per warp w of the group, lane l): for each 8-column block i, d[4i], d[4i+1] are row 16w + l/4,
+// columns 8i + 2(l%4) + {0, 1}; d[4i+2], d[4i+3] the same columns of row 16w + l/4 + 8.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
+// Shared-memory matrix descriptor for a tile stored as rows of 128 bytes with the 128B swizzle (what a TMA box
+// {64 x b16, rows} with CU_TENSOR_MAP_SWIZZLE_128B writes): 8-row groups 1024 B apart.
+//   bits [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for these layouts) | [32,46) SBO>>4 (=64) | [62,64) 1 = SWIZZLE_128B
+// K-major operands advance K by 16 elements as +32 B of start address; an MN-major operand (B = V in P V, 64 columns
+// wide) advances K by 16 rows as +2048 B.
+__device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
+  return (static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4)) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// D[tmem] (+)= A[smem desc] * B[smem desc], kind::f16 (fp16/bf16 operands, fp32 accumulate), one CTA.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
+// d[i .. i+7] as read-write asm operands
+#define DSS_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
+                    "+f"(d[i + 6]), "+f"(d[i + 7])
+// D[64 x 128] (+)= A(smem) * B(smem), both K-major
+__device__ __forceinline__ void wgmma_m64n128_ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : DSS_ACC8(0), DSS_ACC8(8), DSS_ACC8(16), DSS_ACC8(24), DSS_ACC8(32), DSS_ACC8(40), DSS_ACC8(48), DSS_ACC8(56)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// D[tmem] (+)= A[tmem] * B[smem desc]: the A operand (128 rows x 16 fp16) is read from TMEM -- lane = row, 8 consecutive
-// 32-bit columns holding the 16 K-values of the row as packed pairs (what tcgen05.st 32x32b of half2 words writes)
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
+// D[64 x 192] (+)= A(smem) * B(smem), both K-major
+__device__ __forceinline__ void wgmma_m64n192_ss(float (&d)[96], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %98, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n192k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95}, "
+      "%96, %97, p, 1, 1, 0, 0;\n\t}"
+      : DSS_ACC8(0), DSS_ACC8(8), DSS_ACC8(16), DSS_ACC8(24), DSS_ACC8(32), DSS_ACC8(40), DSS_ACC8(48), DSS_ACC8(56), DSS_ACC8(64), DSS_ACC8(72), DSS_ACC8(80), DSS_ACC8(88)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-// mbarrier arrives once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// same, arriving on the mbarrier at this offset in every CTA of `cta_mask`
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"(cta_mask)
-               : "memory");
-}
-// ---- CTA-pair ("2-SM") forms: one MMA spans the tensor cores of both CTAs of a cluster pair (M = 256: each CTA owns 128
-// rows and its own TMEM accumulator; B is split along N between the two CTAs' shared memories). Issued by ONE thread
-// of the even CTA; completion is multicast to a barrier at the same offset in both CTAs.
-__device__ __forceinline__ void umma_f16_ss_cg2(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                uint32_t accumulate) {
+// D[64 x 256] (+)= A(smem) * B(smem), both K-major
+__device__ __forceinline__ void wgmma_m64n256_ss(float (&d)[128], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, "
+      "%128, %129, p, 1, 1, 0, 0;\n\t}"
+      : DSS_ACC8(0), DSS_ACC8(8), DSS_ACC8(16), DSS_ACC8(24), DSS_ACC8(32), DSS_ACC8(40), DSS_ACC8(48), DSS_ACC8(56), DSS_ACC8(64), DSS_ACC8(72), DSS_ACC8(80), DSS_ACC8(88), DSS_ACC8(96), DSS_ACC8(104), DSS_ACC8(112), DSS_ACC8(120)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit_cg2_mc(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"(cta_mask)
-               : "memory");
-}
-// TMEM allocation for a CTA pair: executed by the same-numbered warp of BOTH CTAs with the same shared-memory offset
-__device__ __forceinline__ void tmem_alloc_cg2(uint32_t smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish_cg2() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_cg2(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// TMA load whose completion bytes are credited to the mbarrier at the same offset in the EVEN CTA of the pair
-// (bit 24 of a shared::cluster address selects the CTA of the pair)
-__device__ __forceinline__ void tma_load_2d_cg2(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1) {
+// D[64 x 64] += A(registers, the mma.sync m16n8k16 A fragment of each warp's 16 rows) * B(smem, MN-major)
+__device__ __forceinline__ void wgmma_m64n64_rs_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t bdesc) {
   asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      :
-      : "r"(smem_dst), "l"(reinterpret_cast<uint64_t>(tm)), "r"(bar & 0xFEFFFFFFu), "r"(c0), "r"(c1)
-      : "memory");
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, 1, 1, 1, 1;"
+      : DSS_ACC8(0), DSS_ACC8(8), DSS_ACC8(16), DSS_ACC8(24)
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc));
 }
-// arrive on the mbarrier at this shared-memory offset in CTA `rank` of the cluster
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank) {
-  asm volatile(
-      "{\n\t.reg .b32 ra;\n\t"
-      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
-      "mbarrier.arrive.release.cluster.shared::cluster.b64 _, [ra];\n\t}"
-      ::"r"(bar), "r"(rank)
-      : "memory");
-}
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp receives lane (base_lane + i), columns c..c+31
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// narrower variants: 32 lanes x 8 / 16 consecutive columns
-__device__ __forceinline__ void tmem_ld_32x8(uint32_t taddr, uint32_t (&r)[8]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-// registers -> TMEM: lane = this thread's row of its warp's lane quarter, 32 consecutive 32-bit columns
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+#undef DSS_ACC8
+template <int N> struct Wgmma;
+template <> struct Wgmma<128> { static __device__ __forceinline__ void ss(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128_ss(d, a, b, acc); } };
+template <> struct Wgmma<192> { static __device__ __forceinline__ void ss(float (&d)[96], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n192_ss(d, a, b, acc); } };
+template <> struct Wgmma<256> { static __device__ __forceinline__ void ss(float (&d)[128], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n256_ss(d, a, b, acc); } };
 
-// UMMA shared-memory matrix descriptor for a K-major tile stored as rows of 128 bytes with the 128B swizzle
-// (exactly what a TMA box {64 x b16, rows} with CU_TENSOR_MAP_SWIZZLE_128B writes): 8-row groups are 1024 B apart.
-//   bits [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (=64)
-//   bits [46,48) version=1 (sm_100) | [61,64) layout type (2 = SWIZZLE_128B)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t smem_addr) {
-  const uint32_t lo = ((smem_addr & 0x3FFFFu) >> 4) | (1u << 16);
-  const uint32_t hi = 64u | (1u << 14) | (2u << 29);
-  return (static_cast<uint64_t>(hi) << 32) | lo;
-}
-// Instruction descriptor, kind::f16: [4,6) D fmt (1=f32) | [7,10) A fmt (0=f16,1=bf16) | [10,13) B fmt |
-// [15] A major (0=K) | [16] B major (0=K) | [17,23) N>>3 | [24,29) M>>4
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (static_cast<uint32_t>(N >> 3) << 17) |
-         (static_cast<uint32_t>(M >> 4) << 24);
-}
+// per-warp-group register budget (the TMA producer group gives its registers to the MMA groups)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ---- Ampere-style async copy + legacy tensor-core path (used by the attention kernel)
 __device__ __forceinline__ void cp_async_16(uint32_t smem_dst, const void* gsrc, bool valid) {
@@ -380,71 +302,29 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   return *reinterpret_cast<uint32_t*>(&h);
 }
 
-// ---- packed fp32 pairs (sm_100: FFMA2 / FADD2 process two floats per instruction)
-__device__ __forceinline__ uint64_t pack_f32x2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-__device__ __forceinline__ void unpack_f32x2(uint64_t v, float& lo, float& hi) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v));
-}
-__device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t r;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-  return r;
-}
-__device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-__device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b) {
-  uint64_t r;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(r) : "l"(a), "l"(b));
-  return r;
-}
-
 // Exact-erf GELU, branch-free:  gelu(x) = x Phi(x) = relu(x) - |x| q(|x|),  q(a) = 0.5 erfc(a / sqrt 2) = 2^P(u),
 // u = min(a / sqrt 2, 5), P = degree-4 minimax fit of log2(erfc(u)) - 1 on [0, 5] weighted by the error it causes in
 // gelu (|x| q ln 2 dP). Max |gelu error| 6.4e-6 over the whole fp32 range, relative error <= 1e-3 for x >= -3
 // (tests/test_cpu_host.py emulates this arithmetic in float32 against torch's float64 GELU); the value is then rounded
 // to fp16 (relative 4.9e-4, smallest normal 6.1e-5).
-// Cost per element: 7 FMA-pipe lane operations (bias add, scale, 4 Horner steps, final fma -- issued as packed FFMA2),
-// one MUFU.EX2 and three ALU-pipe operations (sign, min, max), spread over three pipes. History: Abramowitz-Stegun
-// 7.1.26 (round 1: MUFU.RCP + MUFU.EX2 + ~14 scalar FMA-pipe instructions; ncu XU pipe 38 % vs tensor pipe 27 %) ->
-// u P(u^2) erf polynomial of degree 8 on the FMA pipe only (14 lane operations: ncu showed the epilogue warps stalled on
-// the FMA pipe, 2 500 cycles per 128 x 64 box against 2 300 cycles of MMA per tile; packed FFMA2 with register operands
-// issues at the same lane rate as scalar FFMA) -> this form.
+// Cost per element: 7 FMA-pipe operations (bias add, scale, 4 Horner steps, final fma), one MUFU.EX2 and three ALU-pipe
+// operations (sign, min, max), spread over three pipes.
 #define DSS_GELU_P0 -1.0004795789718628f
 #define DSS_GELU_P1 -1.6226296424865723f
 #define DSS_GELU_P2 -0.9360293745994568f
 #define DSS_GELU_P3 -0.12467514723539352f
 #define DSS_GELU_P4 0.015465063974261284f
 #define DSS_GELU_CLAMP 5.0f
-__device__ __forceinline__ void gelu_erf_x2(float x0, float x1, float& y0, float& y1) {
-  const float na0 = __uint_as_float(__float_as_uint(x0) | 0x80000000u);   // -|x|
-  const float na1 = __uint_as_float(__float_as_uint(x1) | 0x80000000u);
-  const uint64_t na = pack_f32x2(na0, na1);
-  float u0, u1;
-  unpack_f32x2(mul_f32x2(na, pack_f32x2(-0.70710678118654752440f, -0.70710678118654752440f)), u0, u1);
-  u0 = fminf(u0, DSS_GELU_CLAMP);
-  u1 = fminf(u1, DSS_GELU_CLAMP);
-  const uint64_t u = pack_f32x2(u0, u1);
-  uint64_t p = fma_f32x2(pack_f32x2(DSS_GELU_P4, DSS_GELU_P4), u, pack_f32x2(DSS_GELU_P3, DSS_GELU_P3));
-  p = fma_f32x2(p, u, pack_f32x2(DSS_GELU_P2, DSS_GELU_P2));
-  p = fma_f32x2(p, u, pack_f32x2(DSS_GELU_P1, DSS_GELU_P1));
-  p = fma_f32x2(p, u, pack_f32x2(DSS_GELU_P0, DSS_GELU_P0));
-  float p0, p1, q0, q1;
-  unpack_f32x2(p, p0, p1);
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(q0) : "f"(p0));
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(q1) : "f"(p1));
-  unpack_f32x2(fma_f32x2(na, pack_f32x2(q0, q1), pack_f32x2(fmaxf(x0, 0.f), fmaxf(x1, 0.f))), y0, y1);
-}
 __device__ __forceinline__ float gelu_erf(float x) {
-  float y0, y1;
-  gelu_erf_x2(x, x, y0, y1);
-  return y0;
+  const float na = __uint_as_float(__float_as_uint(x) | 0x80000000u);   // -|x|
+  const float u = fminf(__fmul_rn(na, -0.70710678118654752440f), DSS_GELU_CLAMP);
+  float p = __fmaf_rn(DSS_GELU_P4, u, DSS_GELU_P3);
+  p = __fmaf_rn(p, u, DSS_GELU_P2);
+  p = __fmaf_rn(p, u, DSS_GELU_P1);
+  p = __fmaf_rn(p, u, DSS_GELU_P0);
+  float q;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(q) : "f"(p));
+  return __fmaf_rn(na, q, fmaxf(x, 0.f));
 }
 
 __device__ __forceinline__ float warp_sum(float v) {

@@ -1,7 +1,7 @@
 // Smallest-K eigenpairs of the graph Laplacian pencil (D - W) v = lambda D v   (reference extract/extract.py:222-240,
 // which calls scipy.sparse.linalg.eigsh(D - W, k=K, sigma=0, which='LM', M=D): dense LU + ARPACK shift-invert).
 //
-// B200 design: no factorisation. With S = D^-1/2 W D^-1/2 the pencil's smallest eigenvalues are 1 - (largest
+// Design: no factorisation. With S = D^-1/2 W D^-1/2 the pencil's smallest eigenvalues are 1 - (largest
 // eigenvalues of S) and v = D^-1/2 u. The top eigenpair of S is known in closed form (u0 = D^1/2 1 / sqrt(sum D),
 // mu0 = 1) and is deflated analytically; the next K-1 come from Lanczos with full re-orthogonalisation (two
 // classical Gram-Schmidt passes) -- ~16-50 symmetric mat-vecs per image instead of an N^3 LU.
@@ -30,9 +30,8 @@ constexpr int EIG_MAX_K = 64;
 constexpr int EIG_STRIP_CH = 4;                    // float4 column chunks per lane and strip
 constexpr int EIG_STRIP = 32 * 4 * EIG_STRIP_CH;   // 512 columns per strip
 // Up to this N two CTAs (images) could share an SM with the <2, 2> instantiation (64 registers, 2 x 2 loads in flight per
-// lane). Measured on the 296-image step at N = 900 it loses to <4, 1> -- one CTA per SM, 128 registers, all 16 loads of
-// a row group's column blocks in flight per lane: 2.27 ms vs 1.94 ms -- so it is only kept for tuning
-// (DSS_EIG_VARIANT=1).
+// lane). The default is <4, 1> -- one CTA per SM, 128 registers, all 16 loads of a row group's column blocks in flight
+// per lane; <2, 2> is only kept for tuning (DSS_EIG_VARIANT=1).
 constexpr int EIG_SMALL_N = 0;
 
 struct EigParams {
@@ -250,8 +249,8 @@ lanczos_laplacian_kernel(EigParams p) {
             const int chd = r >> 2;                          // chunk that holds the diagonal elements of these rows
             // warp-uniform range of k blocks (32 chunks each) that intersect columns [max(r, s0), s1): the blocks left
             // of the diagonal are skipped as a whole, and the per-element masks of the diagonal chunk are only evaluated
-            // in the one block that contains it (round 2, first version: ncu showed 1.2 G warp instructions per launch,
-            // 14 % of them FFMA -- the predicated mask / address arithmetic of all eight blocks was issued for every row)
+            // in the one block that contains it (otherwise the predicated mask / address arithmetic of all eight blocks
+            // would be issued for every row)
             const int cb = s0 >> 2, nch = s1 >> 2;
             const int k_first = chd > cb ? (chd - cb) >> 5 : 0;
             const int k_end = ((s1 - s0) + 127) >> 7;
@@ -582,7 +581,7 @@ static int eig_per_sm(int Npad, int mmax) {
 
 static int eig_grid(int B, int Npad, int mmax) {
   int sms = device_sm_count();
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   const int g = sms * eig_per_sm(Npad, mmax);
   return B < g ? B : g;
 }

@@ -1,17 +1,16 @@
-// out = epilogue(A[M,K] * Wt[N,K]^T + bias) with fp16 operands, fp32 accumulation in Tensor Memory.
+// out = epilogue(A[M,K] * Wt[N,K]^T + bias) with fp16 operands, fp32 accumulation in registers (Hopper wgmma).
 //
-// Persistent kernel, one CTA per SM, 128x128 output tiles handed out round-robin (n fastest, so CTAs that run
+// Persistent kernel, one CTA per SM, 128 x BN output tiles handed out round-robin (n fastest, so CTAs that run
 // together share the A rows in L2 and the whole weight matrix stays L2-resident):
-//   warp 0      : TMA producer   (cp.async.bulk.tensor 2D, 128B swizzle, 64-wide K slabs); the 4-stage ring keeps
-//                 running across tile boundaries, so loads for the next tile are in flight during the epilogue
-//   warp 1      : TMEM allocator + single-thread tcgen05.mma issuer (UMMA 128x128x16, kind::f16) into one of TWO
-//                 128-column accumulators, so the MMAs of tile i+1 overlap the epilogue of tile i
-//   warps 2..9  : epilogue, two groups of 4 warps (one per TMEM lane quarter), each group owns 64 columns:
-//                 tcgen05.ld 32 lanes x 32 columns -> +bias / exact-erf GELU -> fp32 staging chunk in smem ->
-//                 row-contiguous (coalesced) global reads of the residual and writes of the result
+//   warp group 0     : TMA producer (one warp: cp.async.bulk.tensor 2D, 128B swizzle, 64-wide K slabs); the ring keeps
+//                      running across tile boundaries, so loads for the next tile are in flight during the epilogue.
+//                      It gives most of its registers to the MMA groups (setmaxnreg).
+//   warp groups 1, 2 : wgmma m64 x BN x 16 on 64 rows each of the tile (both operands straight from the swizzled
+//                      slabs), then the epilogue from the register accumulators: +bias / exact-erf GELU -> 128 B-swizzled
+//                      staging box -> TMA store (or TMA reduce-add for the residual)
 // CTAs run as CLUSTERS OF TWO that work on vertically adjacent tiles (same n, m and m+1): each CTA fetches half of
-// the weight tile and TMA-multicasts it into both CTAs' shared memory, which cuts the L2 -> SM operand traffic (the
-// bound of this kernel) by 25-33 %. The slot-free signal (tcgen05.commit) is multicast to both CTAs as well.
+// the weight tile and TMA-multicasts it into both CTAs' shared memory, which halves the L2 -> SM traffic of the weight
+// operand. A slab is free once the MMA groups of both CTAs have retired their wgmmas on it.
 // Both operands are K-major, which is the native layout of activations [rows, features] and of torch Linear
 // weights [out, in]; no transposes anywhere.
 #include <math.h>
@@ -21,18 +20,15 @@
 
 namespace dss {
 
-constexpr int BM = 128, BK = 64, UMMA_K = 16;   // BK: one 128-byte swizzle atom of fp16 (one TMA box / 4 UMMAs)
+constexpr int BM = 128, BK = 64, MMA_K = 16;   // BK: one 128-byte swizzle atom of fp16 (one TMA box / 4 wgmma k-steps)
 constexpr int A_ATOM_BYTES = BM * BK * 2;
-// swizzle atoms (64-deep K slabs) per pipeline stage. 128-wide tiles: 2 (128-deep stages halve the MMA warp's
-// per-FLOP wait/elect/commit overhead: +12 % measured); 256-wide tiles: 1 (their UMMAs are already twice as long and
-// only 2 x 96 KB stages would fit, which hides less load latency than 4 x 48 KB: 790 vs 828 TFLOP/s measured).
-constexpr int slabs_per_stage(int bn) { return bn == 128 ? 2 : 1; }
-constexpr int EPI_WARPS = 16;            // 4 TMEM lane quarters x 4 column slices
-constexpr int GEMM_THREADS = 64 + EPI_WARPS * 32;
-constexpr int MANUAL_EPI_WARPS = 8;      // the row-remapping / affinity epilogues use the first 8 epilogue warps
+constexpr int CONSUMER_WGS = 2;                 // MMA + epilogue warp groups, each owns 64 rows of the 128-row tile
+constexpr int EPI_THREADS = CONSUMER_WGS * 128;
+constexpr int GEMM_THREADS = 128 + EPI_THREADS; // warp group 0: TMA producer (one warp issues, three idle)
 constexpr int STG_LD = 36;               // manual path staging chunk: 128 rows x 32 cols fp32, row pitch 36
 constexpr int STG_BYTES = BM * STG_LD * 4;
 constexpr int BOX_BYTES = BM * 128;      // TMA-store path staging box: 128 rows x 128 bytes (swizzled)
+constexpr int SMEM_LIMIT = 232448;       // 227 KB of dynamic shared memory per block (sm_90)
 
 // epilogues whose output rows are the GEMM rows: written with TMA (the row-remapping ones keep the manual path)
 constexpr int EPI_AFFINITY_F32 = 100;    // internal epilogue id (not in the public enum): batched patch-affinity tile
@@ -40,23 +36,20 @@ __host__ __device__ constexpr bool epi_uses_tma_store(int epi) {
   return epi == DSS_EPI_BIAS_F16 || epi == DSS_EPI_BIAS_GELU_F16 || epi == DSS_EPI_BIAS_RESID_F32 ||
          epi == DSS_EPI_BIAS_F32 || epi == EPI_AFFINITY_F32;
 }
-constexpr int default_stages(int bn, bool tma) { return tma ? (bn == 128 ? 3 : 4) : 2; }
-// Shared-memory bandwidth is what bounds the kernel (DESIGN.md section 3): wide tiles and a deep ring are what matter.
-// CG = 1: one CTA per output tile, the pair shares the weight tile by TMA multicast (each CTA still holds all of it).
-// CG = 2: tcgen05.mma.cta_group::2, each CTA holds only ITS half of the weight tile, which halves the B operand traffic
-// per FLOP; the smaller stages buy a deeper ring. Used for the long-K residual GEMM (fc2), see launch_tc.
-template <int BN, bool TMA_OUT, int ST = default_stages(BN, TMA_OUT), int CG = 1> struct TileCfg {
-  static constexpr int KS = slabs_per_stage(BN);
-  static constexpr int A_TILE_BYTES = KS * A_ATOM_BYTES;
-  static constexpr int B_ATOM_BYTES = BN * BK * 2 / CG;   // CG = 2: BN/2 rows per CTA
-  static constexpr int B_TILE_BYTES = KS * B_ATOM_BYTES;
-  static constexpr int STAGE_BYTES = A_TILE_BYTES + B_TILE_BYTES;   // [A atom 0 | A atom 1 | B atom 0 | B atom 1]
-  static constexpr int STAGING_BYTES = TMA_OUT ? 2 * BOX_BYTES : 4 * STG_BYTES;
-  static constexpr int MAX_STAGES = (232448 - 1024 - 1024 - 256 - STAGING_BYTES) / STAGE_BYTES;
-  static constexpr int STAGES = CG == 1 ? ST : (MAX_STAGES > 8 ? 8 : MAX_STAGES);
-  static constexpr int TMEM_COLS = BN == 128 ? 256 : 512;   // two fp32 accumulators, power-of-two allocation
+// Ring stage = one 64-deep K slab of A (128 rows) and B (BN rows); as many stages as the shared-memory budget leaves
+// next to the output staging (at most 6).
+template <int EPI, int BN> struct TileCfg {
+  static constexpr int B_ATOM_BYTES = BN * BK * 2;
+  static constexpr int STAGE_BYTES = A_ATOM_BYTES + B_ATOM_BYTES;   // [A slab | B slab]
+  // TMA path: two swizzled output boxes (+ the affinity epilogue's row-major fp32 copy of one box); manual path: two
+  // fp32 chunks
+  static constexpr int STAGING_BYTES = epi_uses_tma_store(EPI) ? 2 * BOX_BYTES + (EPI == EPI_AFFINITY_F32 ? STG_BYTES : 0)
+                                                              : 2 * STG_BYTES;
+  static constexpr int MAX_STAGES = (SMEM_LIMIT - 1024 - 256 - STAGING_BYTES) / STAGE_BYTES;
+  static constexpr int STAGES = MAX_STAGES > 6 ? 6 : MAX_STAGES;
   // ring | staging | barriers | alignment slack
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 256 + 1024;
+  static_assert(STAGES >= 2, "shared memory budget");
 };
 
 
@@ -156,15 +149,18 @@ __device__ __forceinline__ TileCoord decode_tile(int t, int pairs_m, int tiles_n
   return TileCoord{((rem / tiles_n) * 2 + rank) * BM, (rem % tiles_n) * BN, z};
 }
 
-template <int EPI, int BN, int ST = default_stages(BN, epi_uses_tma_store(EPI)), int CG = 1>
+// Accumulator fragment helpers. Warp group wg, warp wi (0..3 inside the group), lane l hold for each 8-column block i
+// of the tile: acc[4i], acc[4i+1] = row 64 wg + 16 wi + l/4, columns 8i + 2(l%4) + {0,1}; acc[4i+2], acc[4i+3] = the
+// same columns 8 rows further down.
+__device__ __forceinline__ int frag_row(int wg, int wi, int lane) { return 64 * wg + 16 * wi + (lane >> 2); }
+
+template <int EPI, int BN>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_f16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                        const __grid_constant__ CUtensorMap tmC, int M, int N, int K, int pairs_m, int tiles_n,
-                        int total_items, EpiParams p) {
-  using Cfg = TileCfg<BN, epi_uses_tma_store(EPI), ST, CG>;
-  constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES, TMEM_COLS = Cfg::TMEM_COLS;
-  constexpr int KS = Cfg::KS, A_TILE_BYTES = Cfg::A_TILE_BYTES;
-  static_assert(CG == 1 || epi_uses_tma_store(EPI), "the CTA-pair MMA path is only wired to the TMA-store epilogues");
+gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                      const __grid_constant__ CUtensorMap tmC, int M, int N, int K, int pairs_m, int tiles_n,
+                      int total_items, EpiParams p) {
+  using Cfg = TileCfg<EPI, BN>;
+  constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
   // SWIZZLE_128B tiles need 1024 B alignment (the swizzle pattern is a function of address bits [7,10))
   const uint32_t raw = smem_u32(smem_raw);
@@ -172,18 +168,13 @@ gemm_f16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
   uint8_t* gbase = smem_raw + (base - raw);
   float* stage_base = reinterpret_cast<float*>(gbase + STAGES * STAGE_BYTES);
   const uint32_t bar_base = base + STAGES * STAGE_BYTES + Cfg::STAGING_BYTES;
-  // barrier block: full[STAGES] | empty[STAGES] | tmem_full[2] | tmem_empty[2] | tmem_ptr(u32)
+  // barrier block: full[STAGES] | empty[STAGES]
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto tfull_bar = [&](int i) { return bar_base + 8u * (2 * STAGES + i); };
-  auto tempty_bar = [&](int i) { return bar_base + 8u * (2 * STAGES + 2 + i); };
-  const uint32_t tmem_ptr_addr = bar_base + 8u * (2 * STAGES + 4);
-  volatile uint32_t* tmem_ptr_gen =
-      reinterpret_cast<volatile uint32_t*>(gbase + STAGES * STAGE_BYTES + Cfg::STAGING_BYTES + 8 * (2 * STAGES + 4));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int num_kb = (K + KS * BK - 1) / (KS * BK);   // pipeline stages per tile (128-deep)
+  const int num_kb = (K + BK - 1) / BK;
   const int rank = (int)cluster_ctarank();          // 0 / 1 inside the CTA pair
   const int cid = blockIdx.x >> 1, ncl = gridDim.x >> 1;
 
@@ -193,197 +184,149 @@ gemm_f16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
     if constexpr (epi_uses_tma_store(EPI)) tma_prefetch_desc(&tmC);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      // CG 1: released by the MMA warps of BOTH CTAs (each writes into the other's slot); CG 2: one multicast commit
-      mbar_init(empty_bar(s), CG == 1 ? 2 : 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(tfull_bar(i), 1);
-      // CG 2: the issuing (even) CTA collects the "accumulator drained" arrivals of both CTAs' epilogue warps
-      mbar_init(tempty_bar(i), (epi_uses_tma_store(EPI) ? EPI_WARPS : MANUAL_EPI_WARPS) * CG);
+      // released by the MMA warp groups of BOTH CTAs (each CTA's producer writes half of the B slab into the other)
+      mbar_init(empty_bar(s), 2 * CONSUMER_WGS);
     }
     mbar_fence_init();
   }
-  if (warp == 1) {
-    if constexpr (CG == 1) {
-      tmem_alloc(tmem_ptr_addr, TMEM_COLS);
-      tmem_relinquish();
-    } else {
-      tmem_alloc_cg2(tmem_ptr_addr, TMEM_COLS);
-      tmem_relinquish_cg2();
-    }
-  }
-  tc_fence_before();
   __syncthreads();
   cluster_sync_all();   // both CTAs' barriers are initialised before any remote arrive / multicast can reach them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr_gen;
 
-  if (warp == 0) {
-    // The whole warp runs the loop with warp-uniform values (so addresses / coordinates stay in uniform registers and
-    // the TMA issue needs no register-to-uniform "waterfall"); one elected lane issues.
-    const uint32_t ubase = __shfl_sync(0xffffffffu, base, 0);
-    int s = 0;
-    uint32_t ph = 0;   // ring position, carried across tiles (no division in the loop)
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0) {
+      // The whole warp runs the loop with warp-uniform values; one elected lane issues.
+      const uint32_t ubase = __shfl_sync(0xffffffffu, base, 0);
+      int s = 0;
+      uint32_t ph = 0;   // ring position, carried across tiles
+      for (int t = cid; t < total_items; t += ncl) {
+        const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
+        const int row_base = tc.z * p.batch_rows;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(empty_bar(s), ph ^ 1u);
+          const uint32_t sa = ubase + s * STAGE_BYTES;
+          const uint32_t fb = full_bar(s);
+          // split-fp16 Gram product: A = [hi | hi/64 | 64 lo], B = [hi | 64 lo | hi/64] are the same array read with the
+          // last two groups of K slabs swapped
+          int kbB = kb;
+          if (p.perm_blocks > 0 && kb >= p.perm_blocks && kb < 3 * p.perm_blocks)
+            kbB = kb < 2 * p.perm_blocks ? kb + p.perm_blocks : kb - p.perm_blocks;
+          if (elect_one()) {
+            mbar_arrive_expect_tx(fb, STAGE_BYTES);
+            tma_load_2d(sa, &tmA, fb, kb * BK, row_base + tc.m0);
+            // this CTA's half of the weight slab (box 64 x BN/2 rows), delivered to both CTAs of the pair
+            tma_load_2d_mc(sa + A_ATOM_BYTES + rank * (Cfg::B_ATOM_BYTES / 2), &tmB, fb, kbB * BK,
+                           row_base + tc.n0 + rank * (BN / 2), (uint16_t)0x3);
+          }
+          __syncwarp();
+          if (++s == STAGES) { s = 0; ph ^= 1u; }
+        }
+      }
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    const int ct = threadIdx.x - 128;               // consumer thread 0..255
+    const int wg = ct >> 7, wi = (ct >> 5) & 3;
+    const int fr = frag_row(wg, wi, lane);          // first of this thread's two fragment rows
+    const int fc = 2 * (lane & 3);                  // column of this thread inside an 8-column block
+    const uint32_t stage_u32 = base + STAGES * STAGE_BYTES;
+    const bool issuer = ct == 0;
+    int s = 0, cc = 0;
+    uint32_t ph = 0;
+    float acc[BN / 2];
+    [[maybe_unused]] float aff_rowsum[2] = {0.f, 0.f};   // affinity: row sums of this thread's two column slices
+    [[maybe_unused]] float aff_mx = 1.f, aff_rmx = 1.f, aff_unscale = 1.f;
     for (int t = cid; t < total_items; t += ncl) {
       const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
-      const int row_base = tc.z * p.batch_rows;
+      // ---- main loop: 4 wgmma k-steps per 64-deep slab; a slab is released (in both CTAs) once the wgmmas of the
+      // NEXT slab have been issued and the older group has retired
+      int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(bar_base + 8u * (STAGES + s), ph ^ 1u);
-        const uint32_t sa = ubase + s * STAGE_BYTES;
-        const uint32_t fb = bar_base + 8u * s;
-        int ka[KS], kbB[KS];
+        mbar_wait(full_bar(s), ph);
+        __syncwarp();   // wgmma is warp-aligned: reconverge after the per-thread barrier spin
+        const uint32_t sa = base + s * STAGE_BYTES;
+        const uint64_t adesc = wgmma_desc_sw128(sa + wg * 64 * 128);
+        const uint64_t bdesc = wgmma_desc_sw128(sa + A_ATOM_BYTES);
+        wgmma_fence();
 #pragma unroll
-        for (int a = 0; a < KS; ++a) {
-          ka[a] = kb * KS + a;   // 64-deep slab index
-          // split-fp16 Gram product: A = [hi | hi/64 | 64 lo], B = [hi | 64 lo | hi/64] are the same array read
-          // with the last two groups of K slabs swapped
-          kbB[a] = ka[a];
-          if (p.perm_blocks > 0 && ka[a] >= p.perm_blocks && ka[a] < 3 * p.perm_blocks)
-            kbB[a] = ka[a] < 2 * p.perm_blocks ? ka[a] + p.perm_blocks : ka[a] - p.perm_blocks;
+        for (int k = 0; k < BK / MMA_K; ++k)
+          Wgmma<BN>::ss(acc, adesc + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && (ct & 127) == 0) {
+          mbar_arrive_cluster(empty_bar(prev), 0);
+          mbar_arrive_cluster(empty_bar(prev), 1);
         }
-        if (elect_one()) {
-          if constexpr (CG == 1) {
-            mbar_arrive_expect_tx(fb, STAGE_BYTES);
-#pragma unroll
-            for (int a = 0; a < KS; ++a) {
-              tma_load_2d(sa + a * A_ATOM_BYTES, &tmA, fb, ka[a] * BK, row_base + tc.m0);
-              // this CTA's half of the weight slab (box 64 x BN/2 rows), delivered to both CTAs of the pair
-              tma_load_2d_mc(sa + A_TILE_BYTES + a * Cfg::B_ATOM_BYTES + rank * (Cfg::B_ATOM_BYTES / 2), &tmB, fb,
-                             kbB[a] * BK, row_base + tc.n0 + rank * (BN / 2), (uint16_t)0x3);
-            }
-          } else {
-            // both CTAs' bytes are credited to the even CTA's barrier, which the issuing MMA warp waits on
-            if (rank == 0) mbar_arrive_expect_tx(fb, 2 * STAGE_BYTES);
-#pragma unroll
-            for (int a = 0; a < KS; ++a) {
-              tma_load_2d_cg2(sa + a * A_ATOM_BYTES, &tmA, fb, ka[a] * BK, row_base + tc.m0);
-              tma_load_2d_cg2(sa + A_TILE_BYTES + a * Cfg::B_ATOM_BYTES, &tmB, fb, kbB[a] * BK,
-                              row_base + tc.n0 + rank * (BN / 2));   // only THIS CTA's half of the weight slab
-            }
-          }
-        }
-        __syncwarp();
+        prev = s;
         if (++s == STAGES) { s = 0; ph ^= 1u; }
       }
-    }
-  } else if (warp == 1 && (CG == 1 || rank == 0)) {
-    // MMA issuer: the whole warp waits on the barriers, one elected lane issues. Descriptors are computed from
-    // warp-uniform values OUTSIDE the elected region: at 64-128 tensor cycles per UMMA the issue cost matters.
-    // (CG 2: only the even CTA issues; one instruction drives both CTAs' tensor cores, M = 256.)
-    constexpr uint32_t idesc = umma_idesc_f16(BM * CG, BN);
-    const uint32_t ubase = __shfl_sync(0xffffffffu, base, 0);
-    const uint32_t utmem = __shfl_sync(0xffffffffu, tmem_base, 0);
-    int s = 0, lt = 0;
-    uint32_t ph = 0;
-    for (int t = cid; t < total_items; t += ncl, ++lt) {
-      const int buf = lt & 1;
-      const uint32_t aph = (lt >> 1) & 1;
-      mbar_wait(tempty_bar(buf), aph ^ 1u);  // the epilogue has drained this accumulator
-      tc_fence_after();
-      const uint32_t acc = utmem + buf * BN;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(bar_base + 8u * s, ph);
-        tc_fence_after();
-        const uint32_t sa = ubase + s * STAGE_BYTES;
-        // advancing K inside a 128 B swizzle atom = advancing the descriptor's start-address field by 32 B >> 4;
-        // the second atom of the stage starts A_ATOM_BYTES / B_ATOM_BYTES further
-        const uint64_t adesc = umma_desc_sw128(sa);
-        const uint64_t bdesc = umma_desc_sw128(sa + A_TILE_BYTES);
-        const uint32_t eb = bar_base + 8u * (STAGES + s);
-        if (elect_one()) {
-#pragma unroll
-          for (int a = 0; a < KS; ++a)
-#pragma unroll
-            for (int k = 0; k < BK / UMMA_K; ++k) {
-              const uint64_t ad = adesc + (uint64_t)(a * (A_ATOM_BYTES >> 4) + 2 * k);
-              const uint64_t bd = bdesc + (uint64_t)(a * (Cfg::B_ATOM_BYTES >> 4) + 2 * k);
-              if constexpr (CG == 1) umma_f16_ss(acc, ad, bd, idesc, (kb | a | k) != 0 ? 1u : 0u);
-              else umma_f16_ss_cg2(acc, ad, bd, idesc, (kb | a | k) != 0 ? 1u : 0u);
-            }
-          // slot free once these MMAs have consumed it (CG 1: in this CTA, arriving in both; CG 2: in both CTAs)
-          if constexpr (CG == 1) umma_commit_mc(eb, (uint16_t)0x3);
-          else umma_commit_cg2_mc(eb, (uint16_t)0x3);
-        }
-        __syncwarp();
-        if (++s == STAGES) { s = 0; ph ^= 1u; }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc);
+      if ((ct & 127) == 0) {
+        mbar_arrive_cluster(empty_bar(prev), 0);
+        mbar_arrive_cluster(empty_bar(prev), 1);
       }
-      if (elect_one()) {   // accumulator complete (CG 2: in both CTAs)
-        if constexpr (CG == 1) umma_commit(tfull_bar(buf));
-        else umma_commit_cg2_mc(tfull_bar(buf), (uint16_t)0x3);
-      }
-      __syncwarp();
-    }
-  } else if (warp >= 2) {
-    // epilogue: group g owns columns [g*BN/2, (g+1)*BN/2) of the tile; a warp may only touch TMEM lanes [32*(warp%4), +32)
-    const int ew = warp - 2;
-    const int g = ew >> 2, wq = ew & 3;
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    if constexpr (epi_uses_tma_store(EPI)) {
-      // ---- All 16 epilogue warps cooperate on one 128-byte-wide output box at a time (32 fp32 or 64 fp16 columns):
-      // warp (quarter q, slice sl) moves TMEM lanes [32q, 32q+32) x columns [sl*W, sl*W+W) -> registers -> +bias
-      // (-> GELU) -> two 16-byte chunks of the 128 B-swizzled staging box; one thread then issues the TMA store.
-      // The residual epilogue uses the TMA *reduce-add* (performed at the L2): x += acc + bias never reads x.
-      constexpr bool OUT16 = (EPI == DSS_EPI_BIAS_F16 || EPI == DSS_EPI_BIAS_GELU_F16);
-      constexpr int BOXC = OUT16 ? 64 : 32;          // columns per 128-byte-wide store box
-      constexpr int W = BOXC / 4;                    // columns per warp slice (16 fp16 / 8 fp32 = 32 bytes)
-      constexpr int NBOX = BN / BOXC;
-      const int sl = ew >> 2;
-      const bool issuer = (ew == 0) && (lane == 0);
-      const uint32_t stage_u32 = base + STAGES * STAGE_BYTES;
-      int lt = 0, cc = 0;
-      [[maybe_unused]] float aff_rowsum = 0.f;       // affinity: this thread's row sum over the tile's columns
-      [[maybe_unused]] float aff_mx = 1.f, aff_rmx = 1.f, aff_unscale = 1.f;
-      for (int t = cid; t < total_items; t += ncl, ++lt) {
-        const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
-        const int buf = lt & 1;
-        const uint32_t aph = (lt >> 1) & 1;
-        mbar_wait(tfull_bar(buf), aph);
-        tc_fence_after();
+
+      if constexpr (epi_uses_tma_store(EPI)) {
+        // ---- 128-byte-wide output boxes (32 fp32 or 64 fp16 columns): fragments -> +bias (-> GELU) -> 128 B-swizzled
+        // staging box -> one TMA store. The residual epilogue uses the TMA *reduce-add* (performed at the L2):
+        // x += acc + bias never reads x.
+        constexpr bool OUT16 = (EPI == DSS_EPI_BIAS_F16 || EPI == DSS_EPI_BIAS_GELU_F16);
+        constexpr int BOXC = OUT16 ? 64 : 32;          // columns per 128-byte-wide store box
+        constexpr int NBOX = BN / BOXC;
         if constexpr (EPI == EPI_AFFINITY_F32) {
-          if (p.tri && tc.m0 > tc.n0) {
-            // the odd CTA's tile below the diagonal (computed only to keep the pair in lock step on the shared B tile):
-            // nothing is read or stored, the accumulator goes straight back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(tempty_bar(buf));
-            continue;
-          }
+          // the odd CTA's tile below the diagonal (computed only to keep the pair in lock step on the shared B tile)
+          if (p.tri && tc.m0 > tc.n0) continue;
         }
-#pragma unroll 1
+#pragma unroll
         for (int b = 0; b < NBOX; ++b) {
           const int nc = tc.n0 + b * BOXC;           // first global column of the box
           const bool live = nc < N;
-          float bias_r[W];                            // independent of the accumulator: issued before the TMEM wait
+          // the staging box is free once the store issued two boxes ago has finished READING it
+          if (issuer) tma_store_wait_read<1>();
+          __syncwarp();
+          asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+          const uint32_t sbuf = stage_u32 + (cc & 1) * BOX_BYTES;
+          if constexpr (EPI != EPI_AFFINITY_F32) {
 #pragma unroll
-          for (int j = 0; j < W; j += 4) {
-            float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (p.bias != nullptr && live) bv = __ldg(reinterpret_cast<const float4*>(p.bias + nc + sl * W + j));
-            bias_r[j] = bv.x; bias_r[j + 1] = bv.y; bias_r[j + 2] = bv.z; bias_r[j + 3] = bv.w;
-          }
-          uint32_t r[W];
-          const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * BN + b * BOXC + sl * W;
-          if constexpr (OUT16) tmem_ld_32x16(taddr, r); else tmem_ld_32x8(taddr, r);
-          tmem_ld_wait();
-          if (b == NBOX - 1) {  // this warp has read all of its TMEM: hand the accumulator back to the MMA warp
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) {
-              if constexpr (CG == 1) mbar_arrive(tempty_bar(buf));
-              else mbar_arrive_cluster(tempty_bar(buf), 0);   // the even CTA's MMA warp owns both accumulators' release
+            for (int i = 0; i < BOXC / 8; ++i) {
+              const int ci = b * (BOXC / 8) + i;       // 8-column block of the tile
+              const int col = nc + 8 * i + fc;         // global column of this thread's pair
+              float2 bv = make_float2(0.f, 0.f);
+              if (p.bias != nullptr && col < N) bv = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int row = fr + 8 * h;
+                float x0 = acc[4 * ci + 2 * h] + bv.x, x1 = acc[4 * ci + 2 * h + 1] + bv.y;
+                if constexpr (EPI == DSS_EPI_BIAS_GELU_F16) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
+                if constexpr (OUT16) {
+                  const uint32_t addr = sbuf + row * 128 + ((i ^ (row & 7)) << 4) + (lane & 3) * 4;
+                  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_half2(x0, x1)) : "memory");
+                } else {
+                  const int j = 2 * i + ((lane & 3) >> 1);
+                  const uint32_t addr = sbuf + row * 128 + ((j ^ (row & 7)) << 4) + (lane & 1) * 8;
+                  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x0), "f"(x1) : "memory");
+                }
+              }
             }
-          }
-          float x[W];
+          } else {
+            // ---- affinity: the box (32 fp32 columns) goes through a row-major copy so that each thread can own one row
+            // x 8 columns ("slice") as the degree fusion below needs: thread (quarter q = rows 32q.., slice pair sp)
+            // handles slices 2 sp and 2 sp + 1
+            float* rowbuf = stage_base + 2 * (BOX_BYTES / 4);
 #pragma unroll
-          for (int e = 0; e < W; e += 2) {
-            unpack_f32x2(add_f32x2(pack_f32x2(__uint_as_float(r[e]), __uint_as_float(r[e + 1])),
-                                   pack_f32x2(bias_r[e], bias_r[e + 1])), x[e], x[e + 1]);
-            if constexpr (EPI == DSS_EPI_BIAS_GELU_F16) gelu_erf_x2(x[e], x[e + 1], x[e], x[e + 1]);
-          }
-          if constexpr (EPI == EPI_AFFINITY_F32) {
-            // W[z, m, n] = relu(acc) / max (+ lambda * counts); columns >= M (row-pitch padding) are zeros; rows >= M
-            // are clipped by the per-image (3D) tensor map
-            const int m = tc.m0 + row, n = nc + sl * W;
+            for (int i = 0; i < 4; ++i) {
+              const int ci = b * 4 + i;
+#pragma unroll
+              for (int h = 0; h < 2; ++h)
+                *reinterpret_cast<float2*>(rowbuf + (fr + 8 * h) * STG_LD + 8 * i + fc) =
+                    make_float2(acc[4 * ci + 2 * h], acc[4 * ci + 2 * h + 1]);
+            }
+            __syncwarp();
+            asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+            const int q = (ct >> 5) & 3, sp = ct >> 7;
+            const int row = q * 32 + lane;
+            const int m = tc.m0 + row;
             if (b == 0) {   // per-tile constants (L2 round trips: not once per box)
               aff_mx = __uint_as_float(__ldg(p.img_max + tc.z));
               aff_rmx = __frcp_rn(aff_mx);
@@ -394,131 +337,136 @@ gemm_f16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
                 const float am = __uint_as_float(__ldg(p.img_absmax + tc.z));
                 if (am > 0.f) aff_unscale = exp2f(2.0f * ceilf(log2f(am)));
               }
-              aff_rowsum = 0.f;
+              aff_rowsum[0] = aff_rowsum[1] = 0.f;
             }
-            const float mx = aff_mx, rmx = aff_rmx, unscale = aff_unscale;
-            const bool relu = p.threshold & 1, nodiv = p.threshold & 2;
-            // y / mx without the compiler's IEEE division subroutine: its range check sends zero and tiny numerators --
-            // most of a thresholded affinity -- down a ~100-instruction slow path (ncu: 84 % of this kernel's 617 M warp
-            // instructions). mx is the largest Gram diagonal: exactly 1 for most normalised images (nothing to do), else
-            // q = y r, one residual correction: q + (y - q mx) r -- the correctly rounded quotient for these operand
-            // ranges (0 <= y <= ~mx, mx in the normal range).
-            const bool scale = !nodiv && mx != 1.0f;
-#pragma unroll
-            for (int e = 0; e < W; ++e) {
-              float y = x[e];
-              if (relu) y = fmaxf(y, 0.f);                  // W * (W > 0)
-              if (scale) {                                  // W / W.max()
-                const float q0 = y * rmx;
-                y = fmaf(fmaf(-q0, mx, y), rmx, q0);
-              }
-              if (nodiv) y *= unscale;
-              x[e] = y;
-            }
+            const bool upper = tc.m0 < tc.n0;
             // edge boxes only (last tile row / column of the image): the colour term and the bounds are per element
             const bool edge = nc + BOXC > M || tc.m0 + BM > M;   // (uniform)
             const bool rowok = !edge || m < M;
-            if (p.counts != nullptr && rowok) {
-              const uint8_t* cnt = p.counts + ((long long)tc.z * M + m) * M + n;
+            float* part = p.deg_part + (long long)tc.z * (8 * tiles_n) * p.ld_part;
+            float* Wz = reinterpret_cast<float*>(p.out) + (long long)tc.z * M * p.ldo;
 #pragma unroll
-              for (int e = 0; e < W; ++e)
-                if (!edge || n + e < M) x[e] += static_cast<float>(cnt[e]) * p.lambda;   // + W_color * lambda
-            }
-            if (edge) {
-#pragma unroll
-              for (int e = 0; e < W; ++e)
-                if (n + e >= M) x[e] = 0.f;
-            }
-            if (p.tri) {
-              // ---- symmetric mode. The matrix is exactly symmetric by construction (the same value is written to
-              // (m, n) and (n, m)), only tiles on or above the diagonal do any work, and the degree D = W 1 that the
-              // eigensolver starts from (extract_utils.py:207-220) is accumulated here instead of by another pass
-              // over W: per-thread row sums and per-warp column sums go to fixed partial slots (deterministic order).
-              // Tiles strictly above the diagonal: TMA store of the tile + mirrored direct stores. Diagonal tiles: the
-              // two halves of the tile come out of differently ordered accumulations (the split-fp16 K groups are
-              // swapped between the operands), so only the elements on or above the diagonal are stored -- each to
-              // both positions -- and the TMA store is skipped: W[i, j] and W[j, i] are the same bits everywhere.
-              // (The odd CTA's below-diagonal tile never gets here.)
-              const bool upper = tc.m0 < tc.n0;
-              float xm[W];
+            for (int hs = 0; hs < 2; ++hs) {
+              constexpr int W = 8;
+              const int sl = 2 * sp + hs;
+              const int n = nc + sl * W;
+              float x[W];
+              {
+                const float4 v0 = *reinterpret_cast<const float4*>(rowbuf + row * STG_LD + sl * W);
+                const float4 v1 = *reinterpret_cast<const float4*>(rowbuf + row * STG_LD + sl * W + 4);
+                x[0] = v0.x; x[1] = v0.y; x[2] = v0.z; x[3] = v0.w; x[4] = v1.x; x[5] = v1.y; x[6] = v1.z; x[7] = v1.w;
+              }
+              // W[z, m, n] = relu(acc) / max (+ lambda * counts); columns >= M (row-pitch padding) are zeros; rows >= M
+              // are clipped by the per-image (3D) tensor map
+              const float mx = aff_mx, rmx = aff_rmx, unscale = aff_unscale;
+              const bool relu = p.threshold & 1, nodiv = p.threshold & 2;
+              // y / mx without the compiler's IEEE division subroutine: its range check sends zero and tiny numerators
+              // -- most of a thresholded affinity -- down a long slow path. mx is the largest Gram diagonal: exactly 1 for
+              // most normalised images (nothing to do), else q = y r, one residual correction: q + (y - q mx) r -- the
+              // correctly rounded quotient for these operand ranges (0 <= y <= ~mx, mx in the normal range).
+              const bool scale = !nodiv && mx != 1.0f;
 #pragma unroll
               for (int e = 0; e < W; ++e) {
-                xm[e] = rowok ? x[e] : 0.f;
-                aff_rowsum += xm[e];
-              }
-              float* part = p.deg_part + (long long)tc.z * (8 * tiles_n) * p.ld_part;
-              float* Wz = reinterpret_cast<float*>(p.out) + (long long)tc.z * M * p.ldo;
-              if (b == NBOX - 1 && rowok)   // row partial slot of (column tile j, slice sl)
-                part[(long long)((tc.n0 / BN) * 4 + sl) * p.ld_part + m] = aff_rowsum;
-              if (!upper) {                 // diagonal tile: direct stores only, no staging / TMA store for this box
-                if (rowok) {
-                  float* rowp = Wz + (long long)m * p.ldo + n;      // (m, n + e)
-                  float* colp = Wz + (long long)n * p.ldo + m;      // (n + e, m)
-#pragma unroll
-                  for (int e = 0; e < W; ++e) {
-                    if (n + e >= m && n + e < p.ldo) rowp[e] = x[e];                          // on / above the diagonal
-                    if (n + e > m && n + e < M) colp[(long long)e * p.ldo] = x[e];            // its mirror image
-                  }
+                float y = x[e];
+                if (relu) y = fmaxf(y, 0.f);                  // W * (W > 0)
+                if (scale) {                                  // W / W.max()
+                  const float q0 = y * rmx;
+                  y = fmaf(fmaf(-q0, mx, y), rmx, q0);
                 }
-                continue;
+                if (nodiv) y *= unscale;
+                x[e] = y;
               }
-              // mirrored store W[z, n + e, m] = W[z, m, n + e]: lanes hold consecutive m -> 128 B per warp store
-              if (!edge || m < p.ldo) {
-                float* colp = Wz + (long long)n * p.ldo + m;
+              if (p.counts != nullptr && rowok) {
+                const uint8_t* cnt = p.counts + ((long long)tc.z * M + m) * M + n;
 #pragma unroll
                 for (int e = 0; e < W; ++e)
-                  if (!edge || n + e < M) colp[(long long)e * p.ldo] = xm[e];
+                  if (!edge || n + e < M) x[e] += static_cast<float>(cnt[e]) * p.lambda;   // + W_color * lambda
               }
-              // column sums over this warp's 32 rows: segmented butterfly (8 -> 4 -> 2 -> 1 values per lane)
-              float c4[4], c2[2], c1;
+              if (edge) {
 #pragma unroll
-              for (int e = 0; e < 4; ++e) {
-                const float mine = (lane & 16) ? xm[e + 4] : xm[e], theirs = (lane & 16) ? xm[e] : xm[e + 4];
-                c4[e] = mine + __shfl_xor_sync(0xffffffffu, theirs, 16);
+                for (int e = 0; e < W; ++e)
+                  if (n + e >= M) x[e] = 0.f;
               }
+              if (p.tri) {
+                // ---- symmetric mode. The matrix is exactly symmetric by construction (the same value is written to
+                // (m, n) and (n, m)), only tiles on or above the diagonal do any work, and the degree D = W 1 that the
+                // eigensolver starts from (extract_utils.py:207-220) is accumulated here instead of by another pass
+                // over W: per-thread row sums and per-warp column sums go to fixed partial slots (deterministic order).
+                // Tiles strictly above the diagonal: TMA store of the tile + mirrored direct stores. Diagonal tiles: the
+                // two halves of the tile come out of differently ordered accumulations (the split-fp16 K groups are
+                // swapped between the operands), so only the elements on or above the diagonal are stored -- each to
+                // both positions -- and the TMA store is skipped: W[i, j] and W[j, i] are the same bits everywhere.
+                float xm[W];
 #pragma unroll
-              for (int e = 0; e < 2; ++e) {
-                const float mine = (lane & 8) ? c4[e + 2] : c4[e], theirs = (lane & 8) ? c4[e] : c4[e + 2];
-                c2[e] = mine + __shfl_xor_sync(0xffffffffu, theirs, 8);
+                for (int e = 0; e < W; ++e) {
+                  xm[e] = rowok ? x[e] : 0.f;
+                  aff_rowsum[hs] += xm[e];
+                }
+                if (b == NBOX - 1 && rowok)   // row partial slot of (column tile j, slice sl)
+                  part[(long long)((tc.n0 / BN) * 4 + sl) * p.ld_part + m] = aff_rowsum[hs];
+                if (!upper) {                 // diagonal tile: direct stores only, no staging / TMA store for this box
+                  if (rowok) {
+                    float* rowp = Wz + (long long)m * p.ldo + n;      // (m, n + e)
+                    float* colp = Wz + (long long)n * p.ldo + m;      // (n + e, m)
+#pragma unroll
+                    for (int e = 0; e < W; ++e) {
+                      if (n + e >= m && n + e < p.ldo) rowp[e] = x[e];                          // on / above the diagonal
+                      if (n + e > m && n + e < M) colp[(long long)e * p.ldo] = x[e];            // its mirror image
+                    }
+                  }
+                  continue;
+                }
+                // mirrored store W[z, n + e, m] = W[z, m, n + e]: lanes hold consecutive m -> 128 B per warp store
+                if (!edge || m < p.ldo) {
+                  float* colp = Wz + (long long)n * p.ldo + m;
+#pragma unroll
+                  for (int e = 0; e < W; ++e)
+                    if (!edge || n + e < M) colp[(long long)e * p.ldo] = xm[e];
+                }
+                // column sums over this warp's 32 rows: segmented butterfly (8 -> 4 -> 2 -> 1 values per lane)
+                float c4[4], c2[2], c1;
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                  const float mine = (lane & 16) ? xm[e + 4] : xm[e], theirs = (lane & 16) ? xm[e] : xm[e + 4];
+                  c4[e] = mine + __shfl_xor_sync(0xffffffffu, theirs, 16);
+                }
+#pragma unroll
+                for (int e = 0; e < 2; ++e) {
+                  const float mine = (lane & 8) ? c4[e + 2] : c4[e], theirs = (lane & 8) ? c4[e] : c4[e + 2];
+                  c2[e] = mine + __shfl_xor_sync(0xffffffffu, theirs, 8);
+                }
+                {
+                  const float mine = (lane & 4) ? c2[1] : c2[0], theirs = (lane & 4) ? c2[0] : c2[1];
+                  c1 = mine + __shfl_xor_sync(0xffffffffu, theirs, 4);
+                }
+                c1 += __shfl_xor_sync(0xffffffffu, c1, 2);
+                c1 += __shfl_xor_sync(0xffffffffu, c1, 1);
+                // lane l now holds the sum of column e = 4 * bit4 + 2 * bit3 + bit2 of l (all four lanes l & 3 agree)
+                if ((lane & 3) == 0) {
+                  const int e = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
+                  // column partial slot of (row tile i = m0 / BM, lane quarter q); it belongs to matrix row n + e
+                  part[(long long)(4 * tiles_n + (tc.m0 / BM) * 4 + q) * p.ld_part + n + e] = c1;
+                }
               }
-              {
-                const float mine = (lane & 4) ? c2[1] : c2[0], theirs = (lane & 4) ? c2[0] : c2[1];
-                c1 = mine + __shfl_xor_sync(0xffffffffu, theirs, 4);
-              }
-              c1 += __shfl_xor_sync(0xffffffffu, c1, 2);
-              c1 += __shfl_xor_sync(0xffffffffu, c1, 1);
-              // lane l now holds the sum of column e = 4 * bit4 + 2 * bit3 + bit2 of l (all four lanes l & 3 agree)
-              if ((lane & 3) == 0) {
-                const int e = ((lane >> 4) & 1) * 4 + ((lane >> 3) & 1) * 2 + ((lane >> 2) & 1);
-                // column partial slot of (row tile i = m0 / BM, lane quarter q); it belongs to matrix row n + e
-                part[(long long)(4 * tiles_n + (tc.m0 / BM) * 4 + q) * p.ld_part + n + e] = c1;
+              const uint32_t srow = sbuf + row * 128;
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {   // two 16-byte chunks per slice
+                const int j = sl * 2 + h;
+                asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(srow + ((j ^ (row & 7)) << 4)),
+                             "f"(x[h * 4 + 0]), "f"(x[h * 4 + 1]), "f"(x[h * 4 + 2]), "f"(x[h * 4 + 3])
+                             : "memory");
               }
             }
-          }
-          // the staging box is free once the store issued two boxes ago has finished READING it
-          if (issuer) tma_store_wait_read<1>();
-          __syncwarp();   // named barriers are warp-aligned: reconverge after lane-conditional code
-          asm volatile("bar.sync 1, %0;" ::"n"(EPI_WARPS * 32) : "memory");
-          const uint32_t sbuf = stage_u32 + (cc & 1) * BOX_BYTES;
-          const uint32_t srow = sbuf + row * 128;
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {   // two 16-byte chunks per thread
-            const int j = sl * 2 + h;
-            const uint32_t addr = srow + ((j ^ (row & 7)) << 4);
-            if constexpr (OUT16) {
-              asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(pack_half2(x[h * 8 + 0], x[h * 8 + 1])),
-                           "r"(pack_half2(x[h * 8 + 2], x[h * 8 + 3])), "r"(pack_half2(x[h * 8 + 4], x[h * 8 + 5])),
-                           "r"(pack_half2(x[h * 8 + 6], x[h * 8 + 7]))
-                           : "memory");
-            } else {
-              asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(x[h * 4 + 0]), "f"(x[h * 4 + 1]),
-                           "f"(x[h * 4 + 2]), "f"(x[h * 4 + 3])
-                           : "memory");
+            // diagonal tiles of the symmetric mode store directly (above) and skip the staging box
+            if (p.tri && !upper) {
+              __syncwarp();
+              asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");   // row-major copy reused by the next box
+              continue;
             }
           }
           fence_proxy_async_smem();   // generic-proxy smem writes -> visible to the TMA (async proxy)
-          __syncwarp();   // named barriers are warp-aligned: reconverge after lane-conditional code
-          asm volatile("bar.sync 1, %0;" ::"n"(EPI_WARPS * 32) : "memory");
+          __syncwarp();
+          asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
           if (issuer) {
             if (live) {
               if constexpr (EPI == DSS_EPI_BIAS_RESID_F32)
@@ -532,87 +480,64 @@ gemm_f16_tcgen05_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
           }
           ++cc;   // (boxes that skip the staging buffers -- diagonal affinity tiles -- do not advance the buffer parity)
         }
-      }
-      if (issuer) tma_store_wait_all<0>();
-    } else if (ew < MANUAL_EPI_WARPS) {
-    constexpr int NCHUNK = BN / 64;            // 32-column chunks per group
-    int lt = 0, cc = 0;  // cc: running chunk counter -> consecutive chunks always use alternate staging buffers
-    for (int t = cid; t < total_items; t += ncl, ++lt) {
-      const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
-      const int buf = lt & 1;
-      const uint32_t aph = (lt >> 1) & 1;
-      mbar_wait(tfull_bar(buf), aph);
-      tc_fence_after();
-#pragma unroll 1
-      for (int c = 0; c < NCHUNK; ++c, ++cc) {
-        const int col0 = g * (BN / 2) + c * 32;  // first column of this chunk inside the tile
-        float* stg = stage_base + (g * 2 + (cc & 1)) * (STG_BYTES / 4);
-        uint32_t r[32];
-        tmem_ld_32x32(tmem_base + (static_cast<uint32_t>(q * 32) << 16) + buf * BN + col0, r);
-        tmem_ld_wait();
-        if (c == NCHUNK - 1) {  // this warp has read all of its TMEM: hand the accumulator back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty_bar(buf));
-        }
-        const int nc = tc.n0 + col0;           // global column of the chunk
-        // Phase 1: +bias (-> GELU) -> staging chunk (thread = row; pitch 36 floats -> conflict-free float4 writes)
+      } else {
+        // ---- row-remapping epilogues: 32-column chunks through a row-major fp32 staging buffer (double buffered),
+        // then row-contiguous (coalesced) global reads of the aux rows and writes of the result
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (p.bias != nullptr && nc < N) bv = __ldg(reinterpret_cast<const float4*>(p.bias + nc + j));
-          float4 v;
-          v.x = __uint_as_float(r[j + 0]) + bv.x;
-          v.y = __uint_as_float(r[j + 1]) + bv.y;
-          v.z = __uint_as_float(r[j + 2]) + bv.z;
-          v.w = __uint_as_float(r[j + 3]) + bv.w;
-          if constexpr (EPI == DSS_EPI_BIAS_GELU_F16) {
-            v.x = gelu_erf(v.x); v.y = gelu_erf(v.y); v.z = gelu_erf(v.z); v.w = gelu_erf(v.w);
+        for (int c = 0; c < BN / 32; ++c, ++cc) {
+          float* stg = stage_base + (cc & 1) * (STG_BYTES / 4);
+          const int nc = tc.n0 + c * 32;           // global column of the chunk
+          // Phase 1: +bias -> staging chunk (pitch 36 floats)
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const int ci = c * 4 + i;
+            float2 bv = make_float2(0.f, 0.f);
+            if (p.bias != nullptr && nc < N) bv = __ldg(reinterpret_cast<const float2*>(p.bias + nc + 8 * i + fc));
+#pragma unroll
+            for (int h = 0; h < 2; ++h)
+              *reinterpret_cast<float2*>(stg + (fr + 8 * h) * STG_LD + 8 * i + fc) =
+                  make_float2(acc[4 * ci + 2 * h] + bv.x, acc[4 * ci + 2 * h + 1] + bv.y);
           }
-          *reinterpret_cast<float4*>(stg + row * STG_LD + j) = v;
-        }
-        // group-local barrier (ids 1, 2). Double-buffered staging: one barrier per chunk is enough, because a
-        // thread reaches the barrier of chunk c only after finishing phase 2 of the previous user of buffer c^1.
-        __syncwarp();   // named barriers are warp-aligned: reconverge after lane-conditional code
-        asm volatile("bar.sync %0, 128;" ::"r"(2 + g) : "memory");
-        // Phase 2: 8 lanes x 16 B cover the 128 B of one row of the chunk, 4 rows per warp instruction
-        if (nc < N) {
-          const int cl = (lane & 7) * 4;
-          float4 v[8], y[8];
+          // Double-buffered staging: one barrier per chunk is enough, because a thread reaches the barrier of chunk c
+          // only after finishing phase 2 of the previous user of buffer c^1.
+          __syncwarp();
+          asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+          // Phase 2: 8 lanes x 16 B cover the 128 B of one row of the chunk, 4 rows per warp instruction
+          if (nc < N) {
+            const int cw = ct >> 5;
+            const int cl = (lane & 7) * 4;
+            float4 v[4], y[4];
 #pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = wq * 32 + i * 4 + (lane >> 3);
-            const int m = tc.m0 + rr;
-            v[i] = *reinterpret_cast<const float4*>(stg + rr * STG_LD + cl);
-            y[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (m < M) {
-              if constexpr (EPI == DSS_EPI_BIAS_RESID_F32)
-                y[i] = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(p.out) + (long long)m * p.ldo + nc + cl);
-              if constexpr (EPI == DSS_EPI_PATCH_F32)
-                y[i] = __ldg(reinterpret_cast<const float4*>(p.aux + (long long)((m % p.rin) + 1) * p.ldo + nc + cl));
+            for (int i = 0; i < 4; ++i) {
+              const int rr = cw * 16 + i * 4 + (lane >> 3);
+              const int m = tc.m0 + rr;
+              v[i] = *reinterpret_cast<const float4*>(stg + rr * STG_LD + cl);
+              y[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+              if (m < M) {
+                if constexpr (EPI == DSS_EPI_PATCH_F32)
+                  y[i] = __ldg(reinterpret_cast<const float4*>(p.aux + (long long)((m % p.rin) + 1) * p.ldo + nc + cl));
+              }
+            }
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const int rr = cw * 16 + i * 4 + (lane >> 3);
+              const int m = tc.m0 + rr;
+              if (m >= M) continue;
+              float4 x = v[i];
+              x.x += y[i].x; x.y += y[i].y; x.z += y[i].z; x.w += y[i].w;
+              store_row4<EPI>(x, m, nc + cl, p);
             }
           }
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int rr = wq * 32 + i * 4 + (lane >> 3);
-            const int m = tc.m0 + rr;
-            if (m >= M) continue;
-            float4 x = v[i];
-            x.x += y[i].x; x.y += y[i].y; x.z += y[i].z; x.w += y[i].w;
-            store_row4<EPI>(x, m, nc + cl, p);
-          }
         }
       }
     }
+    if constexpr (epi_uses_tma_store(EPI)) {
+      if (issuer) tma_store_wait_all<0>();
     }
   }
-  tc_fence_before();
+  __syncwarp();
   __syncthreads();
   cluster_sync_all();   // the peer may still multicast / arrive into this CTA's shared memory until it is done too
-  if (warp == 1) {
-    if constexpr (CG == 1) tmem_dealloc(tmem_base, TMEM_COLS);
-    else tmem_dealloc_cg2(tmem_base, TMEM_COLS);
-  }
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -657,11 +582,11 @@ static PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
-// Tile width used for an N-column GEMM (B operand = weights [N, K]): 256 if it divides N, else 128.
+// Tile width used for an N-column GEMM (B operand = weights [N, K]): the widest of 256 / 192 / 128 that divides N.
 int gemm_tile_n(int N) {
   static const char* force = getenv("DSS_GEMM_BN");  // tuning override (experiments only)
   if (force) return atoi(force);
-  // widest tile that divides N: operand bytes per FLOP (shared-memory bandwidth, the binding resource) fall with BN
+  // operand bytes per FLOP fall with BN
   return N % 256 == 0 ? 256 : (N % 192 == 0 ? 192 : 128);
 }
 
@@ -747,13 +672,13 @@ int make_tmap_out3d_f16(CUtensorMap* tm, const void* ptr, int images, int rows, 
   return DSS_OK;
 }
 
-template <int EPI, int BN, int ST = default_stages(BN, epi_uses_tma_store(EPI)), int CG = 1>
+template <int EPI, int BN>
 static int launch_tc_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, int M, int N, int K,
                         const EpiParams& p, cudaStream_t st, int kclass, int batch) {
-  using Cfg = TileCfg<BN, epi_uses_tma_store(EPI), ST, CG>;
+  using Cfg = TileCfg<EPI, BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    DSS_CHECK_CUDA(cudaFuncSetAttribute(gemm_f16_tcgen05_kernel<EPI, BN, ST, CG>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    DSS_CHECK_CUDA(cudaFuncSetAttribute(gemm_f16_wgmma_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                         Cfg::SMEM_BYTES));
     attr_set = true;
   }
@@ -765,7 +690,7 @@ static int launch_tc_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
   }
   const int total = per_img * batch;   // work items of a CTA pair
   int sms = device_sm_count();
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   const int clusters = total < sms / 2 ? total : sms / 2;
   if (epi_uses_tma_store(EPI) && tmC == nullptr) {
     set_error("gemm: this epilogue needs an output tensor map");
@@ -784,40 +709,25 @@ static int launch_tc_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  DSS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_tcgen05_kernel<EPI, BN, ST, CG>, tmA, tmB, tmC ? *tmC : tmA, M, N, K,
+  DSS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_wgmma_kernel<EPI, BN>, tmA, tmB, tmC ? *tmC : tmA, M, N, K,
                                     pairs_m, tiles_n, total, p));
   DSS_CHECK_CUDA(cudaGetLastError());
   return DSS_OK;
 }
 
-// bn = tile width the B tensor map was built for (its TMA box has bn rows)
+// bn = tile width the B tensor map was built for (its TMA box has bn / 2 rows)
 template <int EPI>
 static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, int M, int N, int K,
                      const EpiParams& p, cudaStream_t st, int kclass, int bn, int batch = 1) {
-  // CTA-pair MMA (tcgen05.mma.cta_group::2: each CTA holds only its half of the weight tile). Validated on hardware in
-  // round 2 (tests/test_ops_gpu.py under DSS_GEMM_2CTA=1); measured on the 296-image step against the multicast form:
-  // fc2 (K = 1536) 1028 vs 931 TFLOP/s, but qkv / fc1 / proj (K = 384) 844 / 720 / 411 vs 1019 / 760 / 439 -- the
-  // pair's shared accumulator-drain handshake costs more than the halved operand traffic saves when a tile has only
-  // six K slabs. Hence: on for the long-K residual GEMM, off elsewhere; DSS_GEMM_2CTA = 0 / 1 forces it.
-  static const int two_cta_env = [] { const char* e = getenv("DSS_GEMM_2CTA"); return e ? (atoi(e) != 0 ? 1 : 0) : -1; }();
-  const bool two_cta = two_cta_env >= 0 ? two_cta_env == 1 : (EPI == DSS_EPI_BIAS_RESID_F32 && K >= 1024);
-  if constexpr (epi_uses_tma_store(EPI) && EPI != EPI_AFFINITY_F32) {
-    if (two_cta) {
-      constexpr int D = 0;   // stage count is derived from the shared-memory budget for CG = 2
-      switch (bn) {
-        case 128: return launch_tc_bn<EPI, 128, D, 2>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
-        case 192: return launch_tc_bn<EPI, 192, D, 2>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
-        case 256: return launch_tc_bn<EPI, 256, D, 2>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
-      }
-    }
-  }
   switch (bn) {
     case 128: return launch_tc_bn<EPI, 128>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
     case 192:
-      if constexpr (epi_uses_tma_store(EPI)) return launch_tc_bn<EPI, 192>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
+      if constexpr (epi_uses_tma_store(EPI) && EPI != EPI_AFFINITY_F32)
+        return launch_tc_bn<EPI, 192>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
       break;
     case 256:
-      if constexpr (epi_uses_tma_store(EPI)) return launch_tc_bn<EPI, 256>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
+      if constexpr (epi_uses_tma_store(EPI) && EPI != EPI_AFFINITY_F32)
+        return launch_tc_bn<EPI, 256>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
       break;
   }
   set_error("gemm: unsupported tile width %d", bn);
@@ -922,7 +832,7 @@ extern "C" int dss_op_gemm_f16_simt(const void* A, const void* Wt, const float* 
   return DSS_ERR_BAD_ARG;
 }
 
-// Tuning probe (not used by the product path): plain bias epilogue with an explicit tile width / ring depth.
+// Tuning probe (not used by the product path): plain bias epilogue with an explicit tile width (`stages` is ignored).
 extern "C" int dss_debug_gemm_cfg(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K,
                                   int bn, int stages, dss_stream_t stream) {
   int rc = check_gemm_args(M, N, K, DSS_EPI_BIAS_F16, bias, out, nullptr, 0, 0);
@@ -933,13 +843,11 @@ extern "C" int dss_debug_gemm_cfg(const void* A, const void* Wt, const float* bi
   if ((rc = make_tmap_out(&tmC, out, M, N, 0))) return rc;
   EpiParams p{out, bias, nullptr, N, 0, 0, 0, nullptr, nullptr, nullptr, 0.f, 0, 0, 0, nullptr, 0};
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int key = bn * 10 + stages;
-  switch (key) {
-    case 1282: return launch_tc_bn<DSS_EPI_BIAS_F16, 128, 2>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, 1);
-    case 1283: return launch_tc_bn<DSS_EPI_BIAS_F16, 128, 3>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, 1);
-    case 1924: return launch_tc_bn<DSS_EPI_BIAS_F16, 192, 4>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, 1);
-    case 2563: return launch_tc_bn<DSS_EPI_BIAS_F16, 256, 3>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, 1);
-    case 2564: return launch_tc_bn<DSS_EPI_BIAS_F16, 256, 4>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, 1);
+  (void)stages;   // the ring depth follows from the shared-memory budget of the tile width
+  switch (bn) {
+    case 128: return launch_tc_bn<DSS_EPI_BIAS_F16, 128>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, 1);
+    case 192: return launch_tc_bn<DSS_EPI_BIAS_F16, 192>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, 1);
+    case 256: return launch_tc_bn<DSS_EPI_BIAS_F16, 256>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, 1);
   }
   set_error("debug_gemm_cfg: unsupported (bn=%d, stages=%d)", bn, stages);
   return DSS_ERR_BAD_ARG;

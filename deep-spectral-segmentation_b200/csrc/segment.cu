@@ -336,7 +336,7 @@ extern "C" int dss_segment_kmeans(const float* points, long long image_stride, l
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   DSS_CHECK_CUDA(cudaFuncSetAttribute(kmeans_segment_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   int sms = device_sm_count();
-  if (sms <= 0) sms = 148;
+  if (sms <= 0) sms = 132;
   const int grid = B < 2 * sms ? B : 2 * sms;
   LaunchScope scope(st, KC_MISC);
   kmeans_segment_kernel<<<grid, SEG_THREADS, smem, st>>>(p);

@@ -2,8 +2,8 @@
 // Replaces utils.get_model + model.get_intermediate_layers + the qkv forward hook of the reference
 // (extract/extract_utils.py:40-50, extract/extract.py:49-53,82-98).
 //
-// Per block:  LN1 -> [tcgen05 GEMM] qkv (f16) -> tcgen05 flash attention -> [tcgen05 GEMM + residual] proj
-//             LN2 -> [tcgen05 GEMM + GELU] fc1 (f16) -> [tcgen05 GEMM + residual] fc2
+// Per block:  LN1 -> [wgmma GEMM] qkv (f16) -> wgmma flash attention -> [wgmma GEMM + residual] proj
+//             LN2 -> [wgmma GEMM + GELU] fc1 (f16) -> [wgmma GEMM + residual] fc2
 // The residual stream stays fp32; GEMM operands are fp16 (11-bit significand, same as TF32), accumulation fp32.
 // The block the reference hooks is pruned to LN1 + the K third of its qkv projection, CLS row dropped in the
 // GEMM epilogue, which writes the fp32 features directly in the reference's [B, N, d] layout.
@@ -234,9 +234,10 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
     return rc;
   if ((rc = launch_cls_row(w.x, h->cls, pos, B, T, d, st))) return rc;
 
-  // K = 384 (ViT-S): LayerNorm is fused into the A-operand producer of the qkv / fc1 GEMMs (gemm_ln.cu); the
-  // stand-alone LayerNorm kernel remains for ViT-B (a 128 x 768 fp16 panel does not fit next to the weight ring)
-  static const bool fused_ln_env = [] { const char* e = getenv("DSS_VIT_FUSED_LN"); return !e || atoi(e) != 0; }();
+  // LayerNorm kernel + GEMM by default: on an H100 (400 W) this measured 3 526 - 3 554 images/s against 3 284 - 3 291
+  // with the LayerNorm fused into the A-operand producer of the qkv / fc1 GEMMs (gemm_ln.cu, DSS_VIT_FUSED_LN=1; K = 384
+  // only: a 128 x 768 fp16 panel does not fit next to the weight ring), whose panel turnover is not hidden
+  static const bool fused_ln_env = [] { const char* e = getenv("DSS_VIT_FUSED_LN"); return e && atoi(e) != 0; }();
   const bool fused_ln = fused_ln_env && d == 384;
   for (int l = 0; l < n_full; ++l) {
     const BlockW& bw = h->blocks[l];

@@ -12,7 +12,7 @@
                           threads; ``close()`` waits for them and re-raises the first error;
   * ``ProcessWriter``    the same on writer PROCESSES, fed one message per GPU batch: torch.save is ~0.1-0.4 ms of pure
                           Python per file, and writer threads would take the interpreter lock away from the thread that
-                          feeds the GPU (measured: the main thread spent 1.4 ms per image waiting for the lock).
+                          feeds the GPU.
 
 Pure host code: nothing here touches the device except ``PinnedRing.to_device``'s copy."""
 from __future__ import annotations
@@ -30,9 +30,9 @@ import torch
 
 def available_cpus() -> int:
     """CPUs this process may actually use: the scheduler affinity mask and the cgroup CPU quota (cpu.max of cgroup v2,
-    cfs_quota_us of v1), not os.cpu_count(). On the B200 hosts a container sees 128 hardware threads and has a quota of
-    16: with 32 decode threads the whole process group was throttled for ~100 ms at a time (cpu.stat nr_throttled), which
-    stalled the thread that feeds the GPU as well."""
+    cfs_quota_us of v1), not os.cpu_count(). A container may see far more hardware threads than its quota: with more decode threads than
+    the quota the whole process group gets throttled (cpu.stat nr_throttled), which stalls the thread that feeds the GPU
+    as well."""
     n = os.cpu_count() or 1
     try:
         n = min(n, len(os.sched_getaffinity(0)))
@@ -144,8 +144,8 @@ class PinnedRing:
         buf = self.bufs[slot][:len(images)]
         import numpy as np
         dst = self.np_bufs[slot]
-        # numpy's copy loop releases the interpreter lock (torch's Tensor.copy_ on CPU tensors does not: measured 2.9 GB/s
-        # for the whole staging step with 32 decode threads competing for the lock), so a few threads copy in parallel
+        # numpy's copy loop releases the interpreter lock (torch's Tensor.copy_ on CPU tensors does not), so a few threads
+        # copy in parallel
         if self._pool is None or len(images) < 2 * self.copy_threads:
             for j, im in enumerate(images):
                 np.copyto(dst[j], im.numpy())

@@ -1,4 +1,4 @@
-/* libdss_b200 -- C ABI of the B200-native deep-spectral hot path.
+/* libdss_b200 -- C ABI of the H100-native deep-spectral hot path.
  *
  * The reference (lukemelas/deep-spectral-segmentation) has no FFI/plugin interface: the hot path is two Python
  * callables, extract_features (extract/extract.py:21-116) and _extract_eig (extract/extract.py:119-244), that call
@@ -37,7 +37,7 @@ typedef enum {
 
 const char* dss_last_error(void);
 int dss_version(void);            /* 100 * major + minor */
-int dss_device_sm_count(void);    /* SM count of the current device (148 on B200), <0 on error */
+int dss_device_sm_count(void);    /* SM count of the current device (132 on H100 SXM), <0 on error */
 
 /* Launch accounting: number of kernels this library has launched in this process. */
 long long dss_kernel_launch_count(void);
@@ -126,7 +126,7 @@ typedef enum {
   DSS_EPI_DROPCLS_F32 = 5    /* out f32 row (m/rin)*rout + m%rin - 1 = acc + bias, rows with m%rin == 0 skipped */
 } dss_epilogue;
 
-/* out = epilogue(A[M,K] (f16) * Wt[N,K]^T (f16) + bias[N]) on tcgen05 tensor cores (TMA-fed, TMEM accumulator).
+/* out = epilogue(A[M,K] (f16) * Wt[N,K]^T (f16) + bias[N]) on Hopper tensor cores (TMA-fed wgmma, register accumulator).
  * K % 8 == 0, N % 32 == 0, lda == K, ldw == K. aux/rin/rout only for the row-remapping epilogues. */
 int dss_op_gemm_f16(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K, int epilogue,
                     const float* aux, int rin, int rout, dss_stream_t stream);
@@ -134,7 +134,7 @@ int dss_op_gemm_f16(const void* A, const void* Wt, const float* bias, void* out,
 int dss_op_gemm_f16_simt(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K,
                          int epilogue, const float* aux, int rin, int rout, dss_stream_t stream);
 /* Tuning probe: dss_op_gemm_f16 with the plain bias->f16 epilogue and an explicit tile width bn in {128,192,256}
- * and TMA ring depth (2..4). Not used by the product path. */
+ * (stages is ignored: the ring depth follows from the shared-memory budget of bn). Not used by the product path. */
 int dss_debug_gemm_cfg(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K, int bn,
                        int stages, dss_stream_t stream);
 /* LayerNorm fused into the GEMM's A-operand producer (the qkv / fc1 layers of ViT-S; K must be 384):
@@ -146,7 +146,7 @@ int dss_op_layernorm_f16(const float* x, const float* gamma, const float* beta, 
                          dss_stream_t stream);
 /* qkv f16 [B, T, 3*d] (q | k | v, heads of 64 inside each) -> out f16 [B, T, d] = softmax(q k^T / 8) v */
 int dss_op_attention_f16(const void* qkv, void* out, int B, int T, int heads, dss_stream_t stream);
-/* same contract on tcgen05 (TMA-fed QK^T and PV UMMAs, S and O in TMEM); the ViT forward uses this one */
+/* same contract on wgmma (TMA-fed QK^T and PV, S, P and O in registers); the ViT forward uses this one */
 int dss_op_attention_tc_f16(const void* qkv, void* out, int B, int T, int heads, dss_stream_t stream);
 /* images_u8 [B,H,W,3] -> patches f16 [B*N, 3*P*P], column order (c, py, px), normalised */
 int dss_op_im2col_f16(const uint8_t* images_u8, void* patches, int B, int H, int W, int P, dss_stream_t stream);

@@ -101,6 +101,41 @@ def make_segmentation_golden():
         print(name, "labels:", np.unique(multi), "single on:", int((single > 0).sum()))
 
 
+def make_live_reference_golden():
+    """Outputs of the reference's own _extract_eig and knn_affinity on the inputs of the two oracle-vs-reference tests
+    (tests/test_cpu_oracle.py), so that the comparison runs without the reference sources."""
+    from PIL import Image
+    feats = synth.structured_features(150, 64, 6, 42)
+    fd = {"k": feats[None], "indices": torch.tensor(0), "file": "x.jpg", "id": "x", "model_name": "dino_vits16",
+          "patch_size": 16, "shape": (1, 3, 160, 240)}
+    with tempfile.TemporaryDirectory() as td:
+        out = ref_shim.run_reference_extract_eig(fd, td, K=6)
+    np.savez_compressed(GOLDEN / "ref_extract_eig_150.npz", eigenvalues=np.asarray(out["eigenvalues"]),
+                        eigenvectors=out["eigenvectors"].numpy())
+    img = synth.blobs_image(12 * 16, 15 * 16, 7).numpy()
+    lr = np.array(Image.fromarray(img).resize((15, 12), Image.BILINEAR)) / 255.0
+    np.savez_compressed(GOLDEN / "ref_knn_affinity_12x15.npz", W=ref_shim.reference_knn_affinity(lr).toarray().astype(np.uint8))
+    # single- and multi-region segmentations of a planted 7 x 11 spectrum, and the border fractions of the latter
+    ref = ref_shim.load_reference()
+    vals, vecs, feats, band = planted_eigs(7, 11, 4, 17)
+    with tempfile.TemporaryDirectory() as td:
+        fdir, edir, o1, o2 = (Path(td) / n for n in ("f", "e", "s", "m"))
+        for d in (fdir, edir, o1, o2):
+            d.mkdir()
+        fd = {"k": feats[None], "indices": torch.tensor(0), "file": "x.jpg", "id": "x", "model_name": "dino_vits16",
+              "patch_size": 16, "shape": (1, 3, 7 * 16 + 3, 11 * 16)}
+        torch.save(fd, fdir / "x.pth")
+        torch.save({"eigenvalues": vals, "eigenvectors": vecs}, edir / "x.pth")
+        inp = ref.utils.get_paired_input_files(str(fdir), str(edir))[0]
+        ref._extract_single_region_segmentations(inp, threshold=0.0, output_dir=str(o1))
+        kw = dict(adaptive=True, non_adaptive_num_segments=4, infer_bg_index=True, kmeans_baseline=False, num_eigenvectors=3)
+        np.random.seed(7)
+        ref._extract_multi_region_segmentations(inp, output_dir=str(o2), **kw)
+        single, multi = np.array(Image.open(o1 / "x.png")), np.array(Image.open(o2 / "x.png"))
+    idx, frac = ref.utils.get_border_fraction(multi)
+    np.savez_compressed(GOLDEN / "ref_segment_7x11.npz", single=single, multi=multi, border_idx=np.asarray(idx),
+                        border_frac=np.asarray(frac))
+
 
 def main():
     assert ref_shim.available(), "reference sources not present"
@@ -136,6 +171,7 @@ def main():
                             eigenvectors=out["eigenvectors"].numpy())
         print(name, "lambda:", np.asarray(out["eigenvalues"]))
     make_segmentation_golden()
+    make_live_reference_golden()
 
 
 if __name__ == "__main__":

@@ -10,9 +10,9 @@ if str(ROOT) not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100: run with -m gpu)")
     # the CPU oracles (fp64 eigh, fp32 ViT) run on torch's intra-op pool: size it by the CPUs this container may use
-    # (the B200 hosts show 128 hardware threads behind a 16-CPU quota; 128 spinning threads get the process throttled)
+    # (a host may show many more hardware threads than the container's CPU quota; spinning threads get it throttled)
     try:
         import torch
         n = importlib.import_module("deep-spectral-segmentation_b200.io_pipeline").available_cpus()

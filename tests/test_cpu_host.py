@@ -126,36 +126,9 @@ def test_synthetic_inputs_are_seeded():
     assert torch.equal(f, synth.structured_features(100, 32, 4, 1)) and f.dtype == torch.float32
 
 
-def test_attention_exp2_polynomial_constants():
-    """The attention kernel takes a quarter of its exponentials off the MUFU unit with a Cody-Waite split + degree-4
-    polynomial (csrc/attention_tc.cu, ex2_poly_x2). Emulate exactly that float32 arithmetic with the constants parsed
-    out of the kernel source and bound its error against 2^x in float64 over the whole input range of the kernel."""
-    import re
-    src = (ROOT / "deep-spectral-segmentation_b200" / "csrc" / "attention_tc.cu").read_text()
-    body = src[src.index("void ex2_poly_x2("):src.index("constexpr int FA_POLY_OF_4")]
-    consts = [float(c) for c in re.findall(r"pack_f32x2\((\d\.\d+)f, \d\.\d+f\)", body)]
-    assert len(consts) == 5, consts          # c4, c3, c2, c1, c0 in Horner order
-    c = [np.float32(v) for v in consts]
-    magic = np.float32(12582912.0)
-    x = np.concatenate([np.linspace(-140.0, 9.0, 400001), -np.logspace(-8, 2, 2001)]).astype(np.float32)
-    xc = np.maximum(x, np.float32(-125.0))
-    xf = (xc + magic).astype(np.float32)
-    n = (xf - magic).astype(np.float32)
-    f = (n * np.float32(-1.0) + xc).astype(np.float32)
-    assert np.abs(f).max() <= 0.5
-    p = c[0]
-    for k in range(1, 5):
-        p = (p * f + c[k]).astype(np.float32)            # fma in float32 (numpy rounds the product once more: ~1 ulp)
-    res = (p.view(np.int32) + (xf.view(np.int32) << 23)).view(np.float32)
-    ref = np.exp2(xc.astype(np.float64))
-    rel = np.abs(res.astype(np.float64) / ref - 1.0)
-    assert rel.max() < 4e-6, rel.max()                    # far below the fp16 rounding of P (4.9e-4)
-    assert np.all(res[x < -125] < 3e-38)                  # masked keys (-inf -> clamp) pack to an fp16 zero
-
-
 def test_gemm_gelu_erf_constants():
     """The fc1 epilogue evaluates the exact-erf GELU as relu(x) - |x| 2^P(min(|x| / sqrt 2, c)) (csrc/common.cuh,
-    gelu_erf_x2). Emulate that float32 arithmetic with the constants parsed out of the kernel source against torch's
+    gelu_erf). Emulate that float32 arithmetic with the constants parsed out of the kernel source against torch's
     erf GELU in float64 over the whole range fp16 activations can take."""
     import re
     src = (ROOT / "deep-spectral-segmentation_b200" / "csrc" / "common.cuh").read_text()

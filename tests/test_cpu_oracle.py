@@ -1,6 +1,6 @@
 """CPU suite: the oracle (oracle/eigs_ref.py, oracle/dino_vit.py) is pinned against
   * the committed golden fixtures produced by the reference's own _extract_eig (tests/golden/, oracle/make_golden.py),
-  * the reference itself when /root/reference is present (dev container only),
+  * stored outputs of the reference's _extract_eig / knn_affinity on the same inputs (tests/golden/ref_*.npz),
   * analytic known-answer cases and an independent ViT implementation (transformers.ViTModel)."""
 import ast
 import io
@@ -11,7 +11,7 @@ import pytest
 import torch
 
 from conftest import ROOT, load_pkg
-from oracle import dino_vit, eigs_ref, ref_shim
+from oracle import dino_vit, eigs_ref
 
 GOLDEN = sorted((ROOT / "tests" / "golden").glob("lap_*.npz"))
 SEG_GOLDEN = sorted((ROOT / "tests" / "golden").glob("seg_*.npz"))
@@ -65,26 +65,24 @@ def test_oracle_reproduces_reference_golden(path):
     assert np.all(_aligned_err(vec.numpy(), z["eigenvectors"]) <= gap_tolerance(feats, int(z["K"]), kw))
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="reference sources only exist in the dev container")
-def test_oracle_matches_live_reference(tmp_path):
+def test_oracle_matches_live_reference():
+    """Against the reference's own _extract_eig on the same features (its outputs stored by oracle/make_golden.py)."""
     synth = load_pkg("synth")
     feats = synth.structured_features(150, 64, 6, 42)
-    fd = {"k": feats[None], "indices": torch.tensor(0), "file": "x.jpg", "id": "x", "model_name": "dino_vits16",
-          "patch_size": 16, "shape": (1, 3, 160, 240)}
-    out = ref_shim.run_reference_extract_eig(fd, tmp_path, K=6)
+    out = np.load(Path(__file__).parent / "golden" / "ref_extract_eig_150.npz")
     ev, vec = eigs_ref.extract_eig(feats, 6, rng_seed=1)
     assert np.abs(ev.numpy() - np.asarray(out["eigenvalues"])).max() <= 2e-6
-    assert _aligned_err(vec.numpy(), out["eigenvectors"].numpy()).max() <= 2e-5
-    assert out["eigenvectors"].dtype == torch.float32 and tuple(out["eigenvectors"].shape) == (6, 150)
+    assert _aligned_err(vec.numpy(), out["eigenvectors"]).max() <= 2e-5
+    assert out["eigenvectors"].dtype == np.float32 and tuple(out["eigenvectors"].shape) == (6, 150)
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="reference sources only exist in the dev container")
 def test_knn_affinity_restatement_matches_reference_function():
+    """Against the reference's knn_affinity on the same low-resolution image (stored by oracle/make_golden.py)."""
     synth = load_pkg("synth")
     img = synth.blobs_image(12 * 16, 15 * 16, 7).numpy()
     from PIL import Image
     lr = np.array(Image.fromarray(img).resize((15, 12), Image.BILINEAR)) / 255.0
-    W_ref = ref_shim.reference_knn_affinity(lr).toarray()
+    W_ref = np.load(Path(__file__).parent / "golden" / "ref_knn_affinity_12x15.npz")["W"].astype(np.float64)
     W = eigs_ref.knn_affinity(lr).toarray()
     assert np.array_equal(W, W_ref)
     assert np.array_equal(W, W.T) and set(np.unique(W)) <= {0.0, 1.0, 2.0, 3.0, 4.0} and np.all(np.diag(W) == 4)
@@ -200,32 +198,18 @@ def test_segmentation_oracle_reproduces_reference_golden(path):
     assert segment_ref.same_partition(multi, z["band"])          # and it is the planted partition
 
 
-@pytest.mark.skipif(not ref_shim.available(), reason="reference sources only exist in the dev container")
-def test_segmentation_oracle_matches_live_reference(tmp_path):
-    from PIL import Image
+def test_segmentation_oracle_matches_live_reference():
+    """Against the reference's single- / multi-region segmentations and border fractions of a planted spectrum (stored by
+    oracle/make_golden.py)."""
     from oracle import make_golden, segment_ref
-    ref = ref_shim.load_reference()
+    z = np.load(Path(__file__).parent / "golden" / "ref_segment_7x11.npz")
     vals, vecs, feats, band = make_golden.planted_eigs(7, 11, 4, 17)
-    fdir, edir, o1, o2 = (tmp_path / n for n in ("f", "e", "s", "m"))
-    for d in (fdir, edir, o1, o2):
-        d.mkdir()
-    fd = {"k": feats[None], "indices": torch.tensor(0), "file": "x.jpg", "id": "x", "model_name": "dino_vits16",
-          "patch_size": 16, "shape": (1, 3, 7 * 16 + 3, 11 * 16)}
-    torch.save(fd, fdir / "x.pth")
-    torch.save({"eigenvalues": vals, "eigenvectors": vecs}, edir / "x.pth")
-    inp = ref.utils.get_paired_input_files(str(fdir), str(edir))[0]
-    ref._extract_single_region_segmentations(inp, threshold=0.0, output_dir=str(o1))
     kw = dict(adaptive=True, non_adaptive_num_segments=4, infer_bg_index=True, kmeans_baseline=False, num_eigenvectors=3)
+    assert np.array_equal(z["single"], segment_ref.single_region(vecs.numpy(), 7, 11, 0.0))
     np.random.seed(7)
-    ref._extract_multi_region_segmentations(inp, output_dir=str(o2), **kw)
-    assert np.array_equal(np.array(Image.open(o1 / "x.png")), segment_ref.single_region(vecs.numpy(), 7, 11, 0.0))
-    np.random.seed(7)
-    assert np.array_equal(np.array(Image.open(o2 / "x.png")),
-                          segment_ref.multi_region(vals.numpy(), vecs.numpy(), feats.numpy(), 7, 11, **kw))
-    seg = np.array(Image.open(o2 / "x.png"))
-    i1, c1 = segment_ref.get_border_fraction(seg)
-    i2, c2 = ref.utils.get_border_fraction(seg)
-    assert np.array_equal(i1, i2) and np.array_equal(c1, c2)
+    assert np.array_equal(z["multi"], segment_ref.multi_region(vals.numpy(), vecs.numpy(), feats.numpy(), 7, 11, **kw))
+    i1, c1 = segment_ref.get_border_fraction(z["multi"])
+    assert np.array_equal(i1, z["border_idx"]) and np.array_equal(c1, z["border_frac"])
 
 
 def test_rw_affinity_restatement_properties():

@@ -1,5 +1,5 @@
 """-m gpu: every ViT operator of libdss_b200 against a plain PyTorch fp32 reference of the same op
-(and the tcgen05 GEMM against the in-GPU CUDA-core checker on identical fp16 operands)."""
+(and the wgmma GEMM against the in-GPU CUDA-core checker on identical fp16 operands)."""
 import math
 
 import pytest

@@ -20,7 +20,7 @@ pytestmark = pytest.mark.gpu
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("B,T,heads", [(1, 3601, 12), (1, 6401, 12), (2, 1601, 6)])
 def test_attention_config_scale_vs_fp32(cuda, B, T, heads):
-    """T = 3601 / 6401 are BASELINE configs C3 / C5 (29 / 51 key tiles: the lazy-rescale path and long TMEM
+    """T = 3601 / 6401 are BASELINE configs C3 / C5 (29 / 51 key tiles: the online-softmax rescaling and long register
     accumulation that T = 901 never reaches)."""
     _lib = load_pkg("_lib"); lib = _lib.load()
     g = torch.Generator(device="cuda").manual_seed(T)

@@ -1,4 +1,4 @@
-"""Tile-width / ring-depth sweep of the tcgen05 GEMM on the ViT-S shapes (tuning probe)."""
+"""Tile-width / ring-depth sweep of the wgmma GEMM on the ViT-S shapes (tuning probe)."""
 import importlib, sys
 from pathlib import Path
 import torch

@@ -42,7 +42,7 @@ def main():
     imgs = base
     feats8 = model.forward_k(imgs)
     N = feats8.shape[1]
-    for B in (8, 64, 148, 296, 592):
+    for B in (8, 64, 132, 264, 528):
         feats = feats8.repeat((B + 7) // 8, 1, 1)[:B].contiguous()
         deg = torch.empty(B, N, device=dev)
         Wm = spectral.affinity(feats, degree=deg)
