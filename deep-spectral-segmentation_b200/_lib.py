@@ -78,6 +78,13 @@ PROTOTYPES = {
     "dss_segment_kmeans": (c_int, [c_void_p, C.c_longlong, C.c_longlong, C.c_longlong, c_int, c_int, c_int, c_void_p,
                                    c_void_p, c_int, c_int, c_int, c_int, C.c_uint, c_int, c_float, c_void_p, c_void_p,
                                    c_void_p, c_void_p]),
+    "dss_segment_bboxes": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "dss_covariance_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "dss_covariance": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_size_t, c_void_p]),
+    "dss_pca_project": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p]),
+    "dss_kmeans_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "dss_kmeans": (c_int, [c_void_p, c_int, c_int, c_int, C.c_uint, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p,
+                           c_void_p, c_size_t, c_void_p]),
     "dss_upsample_bilinear": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "dss_normalize_rows": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
 }

@@ -14,7 +14,8 @@ from pathlib import Path
 HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 LIB = HERE / "libdss_b200.so"
-SOURCES = ["api.cu", "gemm.cu", "gemm_ln.cu", "vit_kernels.cu", "attention_tc.cu", "vit.cu", "affinity.cu", "eigsh.cu", "knn.cu", "segment.cu"]
+SOURCES = ["api.cu", "gemm.cu", "gemm_ln.cu", "vit_kernels.cu", "attention_tc.cu", "vit.cu", "affinity.cu", "eigsh.cu", "knn.cu", "segment.cu",
+           "cluster.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "-DDSS_BUILD", "-Xptxas", "-v", *os.environ.get("DSS_EXTRA_NVCC_FLAGS", "").split()]
 
@@ -30,7 +31,7 @@ def needs_build() -> bool:
     if not LIB.is_file():
         return True
     t = LIB.stat().st_mtime
-    deps = [CSRC / s for s in SOURCES] + [CSRC / "common.cuh", HERE.parent / "include" / "dss_b200.h", Path(__file__)]
+    deps = [CSRC / s for s in SOURCES] + [CSRC / "common.cuh", CSRC / "kmeans_common.cuh", HERE.parent / "include" / "dss_b200.h", Path(__file__)]
     return any(d.stat().st_mtime > t for d in deps)
 
 

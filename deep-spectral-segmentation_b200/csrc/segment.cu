@@ -12,6 +12,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "kmeans_common.cuh"
 
 namespace dss {
 
@@ -30,15 +31,6 @@ threshold_mask_kernel(const float* __restrict__ evecs, int K, int N, int which, 
 }
 
 __device__ __forceinline__ size_t align_up_dev(size_t x, size_t a) { return (x + a - 1) / a * a; }
-
-__device__ __forceinline__ uint32_t seg_hash(uint32_t a, uint32_t b, uint32_t c) {
-  uint32_t x = a * 0x9E3779B1u ^ (b + 0x7F4A7C15u) * 0x85EBCA77u ^ (c + 0x165667B1u) * 0xC2B2AE3Du;
-  x ^= x >> 16; x *= 0x7FEB352Du; x ^= x >> 15; x *= 0x846CA68Bu; x ^= x >> 16;
-  return x;
-}
-__device__ __forceinline__ double seg_uniform(uint32_t seed, uint32_t img, uint32_t ctr) {
-  return (double)(seg_hash(seed, img, ctr) >> 8) * (1.0 / 16777216.0);   // [0, 1)
-}
 
 struct KmeansParams {
   const float* pts;         // point n of image b, coordinate j: pts[b * img_stride + n * pt_stride + j * dim_stride]
@@ -131,7 +123,7 @@ kmeans_segment_kernel(KmeansParams p) {
       pot += d2;
     }
     pot = seg_block_sum(pot, red, tid);
-    const int trials = 2 + (int)log((double)k);
+    const int trials = kmeans_local_trials(k);
     for (int c = 1; c < k; ++c) {
       int best_cand = -1;
       double best_pot = 0.0;

@@ -5,7 +5,10 @@
     extract_eigs      (:247-280)  directory of features files -> eigs files (batched on the GPU)
     extract_all                   fused: images -> both file layouts (+ optional segmentations) without the disk round-trip
     extract_single_region_segmentations / extract_multi_region_segmentations  (:283-411)  eigs -> PNG masks (GPU kernels)
+    extract_bboxes        (:429-497)  segment bounding boxes after erosion / dilation (GPU kernel)
     extract_bbox_features (:500-544)  DINO CLS embedding of every bounding-box crop
+    extract_bbox_clusters (:547-599)  normalise, PCA, K-means of the box features (GPU kernels)
+    extract_semantic_segmentations (:602-647)  segment -> cluster lookup on every label map (host)
 
 Same argument names, defaults, file layouts and skip-if-exists behaviour; all arithmetic runs in libdss_b200. Host I/O
 (decode, pinned staging, .pth / PNG writers) is threaded, see io_pipeline.py."""
@@ -18,7 +21,7 @@ from typing import Dict, List, Optional, Tuple
 import numpy as np
 import torch
 
-from . import _lib, io_pipeline, segment, spectral
+from . import _lib, cluster, io_pipeline, segment, spectral
 from . import extract_utils as utils
 
 torch.set_grad_enabled(False)  # extract.py:838
@@ -501,6 +504,178 @@ def extract_bbox_features(images_root: str, bbox_file: str, model_name: str, out
         bbox_dict["features"] = torch.stack([feats[(bi, ji)] for ji in range(len(bbox_dict["bboxes"]))], dim=0)
     torch.save(bbox_list, output_file)
     print(f"Saved features to {output_file}")
+
+
+def _read_label_map(path) -> np.ndarray:
+    """np.array(Image.open(path)) as uint8 (a mode '1' PNG reads as bool)."""
+    from PIL import Image
+    segmap = np.array(Image.open(str(path)))
+    if segmap.dtype == bool:
+        segmap = segmap.astype(np.uint8)
+    if segmap.dtype != np.uint8 or segmap.ndim != 2:
+        raise ValueError(f"{path}: expected a single-channel 8-bit label map, got {segmap.dtype} {segmap.shape}")
+    return segmap
+
+
+def _bbox_dict(image_id, P: int, boxes: np.ndarray, present: np.ndarray, skip_bg_index: bool) -> dict:
+    """The dict _extract_bbox returns (extract.py:447-468): python int segment indices, numpy int64 coordinates."""
+    out = {"bboxes": [], "bboxes_original_resolution": [], "segment_indices": [], "id": image_id,
+           "format": "(xmin, ymin, xmax, ymax)"}
+    for v in np.flatnonzero(present).tolist():
+        if skip_bg_index and v == 0:
+            continue
+        bbox = [np.int64(c) for c in boxes[v]]
+        out["segment_indices"].append(v)
+        out["bboxes"].append(bbox)
+        out["bboxes_original_resolution"].append([c * P for c in bbox])
+    return out
+
+
+def extract_bboxes(features_dir: str, segmentations_dir: str, output_file: str, num_erode: int = 2, num_dilate: int = 3,
+                   skip_bg_index: bool = True, downsample_factor: Optional[int] = None, batch_size: int = 1024,
+                   num_workers: Optional[int] = None):
+    """
+    Bounding box of every segment of the multi-region segmentations after erosion and dilation (reference
+    extract/extract.py:429-497), same command / file contract: one list of dicts {'bboxes', 'bboxes_original_resolution',
+    'segment_indices', 'id', 'format'} saved to ``output_file``. The morphology and the boxes run on the GPU for batches
+    of label maps of equal size (csrc/cluster.cu); files are read on threads.
+
+    Example:
+    python extract.py extract_bboxes \
+        --features_dir "./data/VOC2012/features/dino_vits16" \
+        --segmentations_dir "./data/VOC2012/multi_region_segmentation/fixed" \
+        --num_erode 2 --num_dilate 5 \
+        --output_file "./data/VOC2012/multi_region_bboxes/fixed/bboxes_e2_d5.pth" \
+    """
+    utils.make_output_dir(str(Path(output_file).parent), check_if_empty=False)
+    inputs = utils.get_paired_input_files(features_dir, segmentations_dir)
+    dev = _device()
+    outputs: List[Optional[dict]] = [None] * len(inputs)
+
+    def load(i):
+        _, (feature_path, segmentation_path) = inputs[i]
+        data_dict = torch.load(str(feature_path), map_location="cpu")
+        P = utils.get_image_sizes(data_dict, downsample_factor)[4]
+        return i, data_dict["id"], P, _read_label_map(segmentation_path)
+
+    def flush(key, items):
+        maps = torch.from_numpy(np.stack([it[3] for it in items])).to(dev)
+        boxes, present = cluster.segment_bboxes(maps, num_erode, num_dilate)
+        boxes, present = boxes.cpu().numpy(), present.cpu().numpy()
+        for j, (i, image_id, P, _) in enumerate(items):
+            outputs[i] = _bbox_dict(image_id, P, boxes[j], present[j], skip_bg_index)
+
+    batcher = _Batcher(batch_size, flush)
+    for item in io_pipeline.ImagePrefetcher(load, range(len(inputs)), num_workers):
+        batcher.add(item[3].shape, item)
+    batcher.finish()
+    torch.save(outputs, output_file)
+    print("Done")
+
+
+def extract_bbox_clusters(bbox_features_file: str, output_file: str, num_clusters: int = 20, seed: int = 0,
+                          pca_dim: Optional[int] = 0, max_iter: int = 300, tol: float = 1e-4):
+    """
+    Clusters the CLS features of all boxes (reference extract/extract.py:547-599), same command / file contract: every
+    dict loses 'features' and gains 'clusters' (numpy int32, its slice of the labels). Runs on the GPU: row L2
+    normalisation, PCA by the covariance-eigh route (as scikit-learn's PCA does when there are many more rows than
+    columns), and K-means over the whole data set.
+
+    Deliberate deviations, both on the device's side of an ill-defined comparison:
+      - The reference runs MiniBatchKMeans(batch_size=4096, max_iter=5000, random_state=seed), a stochastic
+        approximation of the K-means objective whose label numbers are not reproducible across its own seeds. This
+        runs full-batch K-means (k-means++ seeding, Lloyd iterations, scikit-learn KMeans' stopping rules ``max_iter``
+        and ``tol``) seeded by ``seed``: the same objective, reproducible to the bit. Cluster ids compare up to
+        relabelling, which is what the Hungarian-matched evaluation uses.
+      - An all-zero feature row normalises to zeros here; the reference divides by its zero norm and gets NaN.
+
+    Example:
+        python extract.py extract_bbox_clusters \
+            --bbox_features_file "./data/VOC2012/multi_region_bboxes/fixed/bbox_features_e2_d5.pth" \
+            --pca_dim 32 --num_clusters 21 --seed 0 \
+            --output_file "./data/VOC2012/multi_region_bboxes/fixed/bbox_clusters_e2_d5_pca_32.pth" \
+    """
+    bbox_list = torch.load(bbox_features_file, weights_only=False)
+    total_num_boxes = sum(len(d["bboxes"]) for d in bbox_list)
+    print(f"Loaded bounding box list. There are {total_num_boxes} total bounding boxes with features.")
+    dev = _device()
+    print("Stacking and normalizing features")
+    feats = torch.cat([torch.as_tensor(d["features"]).to(torch.float32).reshape(-1, d["features"].shape[-1])
+                       for d in bbox_list], dim=0)
+    feats = spectral.normalize_rows(feats.to(dev))
+    if pca_dim:
+        print(f"Computing PCA with dimension {pca_dim}")
+        feats = cluster.pca(feats, int(pca_dim))
+    print(f"Computing K-Means clustering with {num_clusters} clusters")
+    labels, _, info, _ = cluster.kmeans(feats, int(num_clusters), seed=seed, max_iter=max_iter, tol=tol)
+    clusters = labels.cpu().numpy()
+    _indices, _counts = np.unique(clusters, return_counts=True)
+    print(f"Cluster indices: {_indices.tolist()}")
+    print(f"Cluster counts: {_counts.tolist()}")
+    idx = 0
+    for bbox_dict in bbox_list:
+        num_bboxes = len(bbox_dict["bboxes"])
+        del bbox_dict["features"]
+        bbox_dict["clusters"] = clusters[idx: idx + num_bboxes]
+        idx = idx + num_bboxes
+    torch.save(bbox_list, output_file)
+    print(f"Saved features to {output_file}")
+
+
+def semantic_map(segmap: np.ndarray, segment_indices, clusters) -> np.ndarray:
+    """extract.py:630-642 on one label map: a {0, 255} map becomes {0, 1}; each segment index maps to its cluster and 0
+    to 0 (so cluster 0 shares the background's value, as in the reference). The reference drops into pdb on a length
+    mismatch, asserts that 0 is not a segment index and raises KeyError on a label without an entry: ValueError here."""
+    segmap = np.array(segmap, dtype=np.uint8)
+    if set(np.unique(segmap).tolist()).issubset({0, 255}):
+        segmap[segmap == 255] = 1
+    clusters = np.asarray(clusters).reshape(-1).tolist()
+    if len(segment_indices) != len(clusters):
+        raise ValueError(f"{len(segment_indices)} segment indices but {len(clusters)} clusters")
+    lut = np.zeros(256, dtype=np.int64)
+    known = np.zeros(256, dtype=bool)
+    for s, c in zip(segment_indices, clusters):
+        if int(s) == 0:
+            raise ValueError("segment index 0 is the background and cannot carry a cluster")
+        lut[int(s)], known[int(s)] = c, True
+    known[0] = True
+    missing = sorted(set(np.unique(segmap).tolist()) - set(np.flatnonzero(known).tolist()))
+    if missing:
+        raise ValueError(f"labels {missing} of the segmentation have no cluster")
+    return lut[segmap].astype(np.uint8)
+
+
+def extract_semantic_segmentations(segmentations_dir: str, bbox_clusters_file: str, output_dir: str,
+                                   yes: Optional[bool] = None, num_workers: int = 4):
+    """
+    Pseudo-label maps: every segment of the multi-region segmentation takes the cluster of its box (reference
+    extract/extract.py:602-647), same command / file contract ({output_dir}/{id}.png, 8-bit 'L'). A 256-entry lookup
+    per image: PNG decode and encode dominate, so it runs on the host on the PNG writer threads.
+
+    Example:
+        python extract.py extract_semantic_segmentations \
+            --segmentations_dir "./data/VOC2012/multi_region_segmentation/fixed" \
+            --bbox_clusters_file "./data/VOC2012/multi_region_bboxes/fixed/bbox_clusters_e2_d5_pca_32.pth" \
+            --output_dir "./data/VOC2012/semantic_segmentations/patches/fixed/segmaps_e2_d5_pca_32" \
+    """
+    bbox_list = torch.load(bbox_clusters_file, weights_only=False)
+    total_num_boxes = sum(len(d["bboxes"]) for d in bbox_list)
+    print(f"Loaded bounding box list. There are {total_num_boxes} total bounding boxes with features and clusters.")
+    utils.make_output_dir(output_dir, assume_yes=yes)
+
+    def one(bbox_dict):
+        image_id = bbox_dict["id"]
+        segmap = _read_label_map(Path(segmentations_dir) / f"{image_id}.png")
+        try:
+            out = semantic_map(segmap, bbox_dict["segment_indices"], bbox_dict["clusters"])
+        except ValueError as e:
+            raise ValueError(f"{image_id}: {e}") from None
+        _save_png(out, str(Path(output_dir) / f"{image_id}.png"))
+
+    with _png_writer_pool(num_workers) as pool:
+        for f in [pool.submit(one, d) for d in bbox_list]:
+            f.result()
+    print(f"Saved features to {output_dir}")
 
 
 # ---------------------------------------------------------------------------------------------------------------

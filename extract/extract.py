@@ -25,6 +25,9 @@ if __name__ == "__main__":
         extract_eigs=_extract.extract_eigs,
         extract_single_region_segmentations=_extract.extract_single_region_segmentations,
         extract_multi_region_segmentations=_extract.extract_multi_region_segmentations,
+        extract_bboxes=_extract.extract_bboxes,
         extract_bbox_features=_extract.extract_bbox_features,
+        extract_bbox_clusters=_extract.extract_bbox_clusters,
+        extract_semantic_segmentations=_extract.extract_semantic_segmentations,
         extract_all=_extract.extract_all,
     ))

@@ -233,6 +233,43 @@ int dss_segment_kmeans(const float* points, long long image_stride, long long po
                        int grid_w, int infer_bg_index, unsigned int seed, int max_iter, float tol, uint8_t* labels,
                        int* info, float* inertia, dss_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Semantic segmentation: boxes, PCA and data-set k-means (replace extract/extract.py:429-599)
+ * ------------------------------------------------------------------------------------------------------------ */
+/* Bounding boxes of every segment of a batch of label maps (_extract_bbox, extract.py:429-470): for every label value v
+ * of segmaps [B, H, W] uint8, mask = (segmap == v) is eroded num_erode times and then dilated num_dilate times with the
+ * 3x3 cross footprint (skimage binary_erosion / binary_dilation: pixels outside the image count as set for erosion and
+ * unset for dilation); a step whose result is empty is discarded (extract_utils.py:115-121). boxes [B, 256, 4] int32 =
+ * {xmin, ymin, xmax + 1, ymax + 1} on the grid, present [B, 256] uint8 = 1 where v occurs (boxes of absent values are
+ * 0). H * W <= 16384 (DSS_ERR_UNSUPPORTED otherwise). One CTA per (image, value). */
+int dss_segment_bboxes(const uint8_t* segmaps, int B, int H, int W, int num_erode, int num_dilate, int* boxes,
+                       uint8_t* present, dss_stream_t stream);
+
+/* Column mean [d] fp32 and covariance cov [d, ldc] fp32 = (X - mean)^T (X - mean) / (M - 1) of X [M, d] fp32, both
+ * accumulated in fp64 through fixed per-CTA partials (bit-reproducible). M >= 2, d <= 1024. cov can be handed to
+ * dss_eigsh_topk (ldc % 4 == 0 there) for the covariance-eigh route of scikit-learn's PCA (extract.py:574-577). */
+size_t dss_covariance_workspace_bytes(int M, int d);
+int dss_covariance(const float* X, int M, int d, float* mean, float* cov, int ldc, void* ws, size_t ws_bytes,
+                   dss_stream_t stream);
+/* Y [M, p] = (X [M, d] - mean [d]) V^T, V [p, d] the principal axes (PCA.transform without whitening); p <= 64. */
+int dss_pca_project(const float* X, int M, int d, const float* mean, const float* V, int p, float* Y,
+                    dss_stream_t stream);
+
+/* K-means of all M points of X [M, dims] fp32 (extract_bbox_clusters, extract.py:579-582). Same algorithm and rules as
+ * dss_segment_kmeans -- greedy k-means++ seeding with 2 + ln k local trials drawn from the D^2 distribution
+ * (deterministic prefix sums), full-batch Lloyd iterations, scikit-learn's stopping rules (centre shift <= tol * mean
+ * column variance, strict label convergence, max_iter), empty clusters re-seeded with the farthest points -- with the
+ * counter-based generator keyed by `seed`. The reference runs MiniBatchKMeans, a stochastic approximation of the same
+ * objective; its label numbers are not reproducible, so results compare up to relabelling. Bit-reproducible: centre sums
+ * are 64-bit fixed point, every floating-point reduction has a fixed order. Nothing synchronises: max_iter iterations
+ * are enqueued and become no-ops once a device-side flag says the run stopped.
+ * centers [k, dims] fp32, labels [M] int32, info [2] int32 = {iterations, converged}, inertia [1] fp32 (may be NULL).
+ * Supported: k <= 64 at dims <= 768, k <= 256 at dims <= 64 (DSS_ERR_UNSUPPORTED otherwise); k <= M.
+ * max_iter <= 0 selects 300, tol < 0 selects 1e-4. The workspace query returns 0 for an unsupported shape. */
+size_t dss_kmeans_workspace_bytes(int M, int dims, int k);
+int dss_kmeans(const float* X, int M, int dims, int k, unsigned int seed, int max_iter, float tol, float* centers,
+               int* labels, int* info, float* inertia, void* ws, size_t ws_bytes, dss_stream_t stream);
+
 /* Bilinear up-sampling of patch features (align_corners=False, as F.interpolate at extract.py:185-188):
  * feats [B, Hp*Wp, d] fp32 -> out [B, Hl*Wl, d] fp32. Used when image_downsample_factor != patch size. */
 int dss_upsample_bilinear(const float* feats, int B, int Hp, int Wp, int d, int Hl, int Wl, float* out,
