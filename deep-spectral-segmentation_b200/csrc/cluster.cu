@@ -571,7 +571,7 @@ __global__ void __launch_bounds__(KM_FIN_THREADS) km_finish_kernel(KmParams p) {
       }
       p.cnt[old] -= 1;
       p.cnt[c] = 1;
-      p.labels[far] = c;
+      // the label stays the E step's (sklearn leaves it too): the next E step counts its changes against it
       p.mind2[far] = -1.f;   // not picked again for the next empty cluster
     }
     __syncthreads();

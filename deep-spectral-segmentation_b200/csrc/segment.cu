@@ -163,7 +163,7 @@ kmeans_segment_kernel(KmeansParams p) {
 
     // ---- Lloyd iterations
     for (int n = tid; n < N; n += SEG_THREADS) lab[n] = 255;
-    int iters = 0, converged = 0;
+    int iters = 0, converged = 0, strict = 0;
     double inertia = 0.0;
     for (int it = 0; it < p.max_iter; ++it) {
       // E step: nearest centre (ties -> lower index), label changes counted
@@ -193,7 +193,7 @@ kmeans_segment_kernel(KmeansParams p) {
       if (changed) atomicAdd(&s_changed, changed);
       __syncthreads();
       iters = it + 1;
-      if (s_changed == 0) { converged = 1; break; }   // strict convergence: labels did not change
+      if (s_changed == 0) { converged = strict = 1; break; }   // strict convergence: labels did not change
       // empty clusters take the point that is farthest from its centre (sklearn _relocate_empty_clusters)
       for (int c = 0; c < k; ++c) {
         if (counts[c] != 0) continue;   // block-uniform (shared memory, read after the barrier)
@@ -220,8 +220,7 @@ kmeans_segment_kernel(KmeansParams p) {
           }
           counts[old] -= 1;
           counts[c] = 1;
-          lab[far] = (uint8_t)c;
-          mind2[far] = 0.f;
+          mind2[far] = -1.f;   // not picked again; the label stays the E step's, as the next change count needs
         }
         __syncthreads();
       }
@@ -235,21 +234,24 @@ kmeans_segment_kernel(KmeansParams p) {
         cen[i] = nc;
       }
       shift = seg_block_sum(shift, red, tid);
-      if (shift <= tol_abs) {   // sklearn: centre shift below tol -> stop, then one more E step fixes the labels
-        for (int n = tid; n < N; n += SEG_THREADS) {
-          const float* pn = pts + (long long)n * p.pt_stride;
-          float bd = INFINITY;
-          int bc = 0;
-          for (int c = 0; c < k; ++c) {
-            const float d2 = seg_dist2(pn, p.dim_stride, cen + (size_t)c * dims, dims);
-            if (d2 < bd) { bd = d2; bc = c; }
-          }
-          lab[n] = (uint8_t)bc;
+      if (shift <= tol_abs) { converged = 1; break; }   // sklearn: centre shift within tol
+    }
+    // sklearn re-runs the E step unless the labels converged strictly (stop on tol or at max_iter), so that the labels
+    // and the inertia belong to the final centres
+    if (!strict) {
+      double in_part = 0.0;
+      for (int n = tid; n < N; n += SEG_THREADS) {
+        const float* pn = pts + (long long)n * p.pt_stride;
+        float bd = INFINITY;
+        int bc = 0;
+        for (int c = 0; c < k; ++c) {
+          const float d2 = seg_dist2(pn, p.dim_stride, cen + (size_t)c * dims, dims);
+          if (d2 < bd) { bd = d2; bc = c; }
         }
-        converged = 1;
-        __syncthreads();
-        break;
+        lab[n] = (uint8_t)bc;
+        in_part += bd;
       }
+      inertia = seg_block_sum(in_part, red, tid);
     }
 
     // ---- background rule (extract.py:337-345, extract_utils.py:124-135): the label with the largest share of the

@@ -225,7 +225,10 @@ int dss_segment_threshold(const float* evecs, int B, int K, int N, int which, fl
  * n_clusters [B] int32 (device) gives k per image (the reference's adaptive mode), capped by max_clusters <= 64.
  * If infer_bg_index, labels are taken on a grid_h x grid_w grid (grid_h * grid_w == N) and the label with the largest
  * border share is swapped with 0 (extract_utils.py:124-135). labels [B, N] uint8; info [B, 2] = {iterations,
- * converged}; inertia [B] (may be NULL). seed: counter-based generator keyed by (seed, image_keys[b]) -- image_keys [B]
+ * converged}; inertia [B] (may be NULL). As in scikit-learn's _kmeans_single_lloyd: a run that stops on tol or at
+ * max_iter re-runs the E step, so the labels and the inertia (sum of squared distances) belong to the final centres; an
+ * empty cluster takes the point farthest from its centre while the point keeps its E-step label, so the next iteration
+ * counts label changes against the E step. seed: counter-based generator keyed by (seed, image_keys[b]) -- image_keys [B]
  * int32 (device; e.g. the `indices` field of the feature files) makes an image's clustering independent of the batch it
  * is processed in; NULL uses the position in the batch. (The reference's clustering is unseeded.) */
 int dss_segment_kmeans(const float* points, long long image_stride, long long point_stride, long long dim_stride, int B,
@@ -263,7 +266,8 @@ int dss_pca_project(const float* X, int M, int d, const float* mean, const float
  * objective; its label numbers are not reproducible, so results compare up to relabelling. Bit-reproducible: centre sums
  * are 64-bit fixed point, every floating-point reduction has a fixed order. Nothing synchronises: max_iter iterations
  * are enqueued and become no-ops once a device-side flag says the run stopped.
- * centers [k, dims] fp32, labels [M] int32, info [2] int32 = {iterations, converged}, inertia [1] fp32 (may be NULL).
+ * centers [k, dims] fp32, labels [M] int32, info [2] int32 = {iterations, converged}, inertia [1] fp32 (may be NULL);
+ * labels and inertia belong to the final centres and relocated points keep their E-step labels, as in dss_segment_kmeans.
  * Supported: k <= 64 at dims <= 768, k <= 256 at dims <= 64 (DSS_ERR_UNSUPPORTED otherwise); k <= M.
  * max_iter <= 0 selects 300, tol < 0 selects 1e-4. The workspace query returns 0 for an unsupported shape. */
 size_t dss_kmeans_workspace_bytes(int M, int dims, int k);
