@@ -15,6 +15,9 @@
 // affinity kernel's epilogue (dss_affinity) when the caller passes it; otherwise one extra pass computes it.
 // The Lanczos basis lives in a per-CTA global scratch (L2), the working vectors in shared memory. Ritz values of the tridiagonal matrix come from a 32-way
 // Sturm multisection in fp64 (one warp per eigenvalue), Ritz vectors from a twisted factorisation.
+// One start vector sees a single direction of every eigenspace, so at an eigenvalue of multiplicity > 1 the Krylov space
+// becomes invariant (breakdown) before all copies are found. The iteration then restarts from a fresh vector orthogonal
+// to the basis: T becomes block diagonal, and Ritz vectors are taken per block, so each copy gets its own vector.
 #include <math.h>
 #include <stdlib.h>
 
@@ -95,6 +98,87 @@ __device__ __forceinline__ int sturm_count(const double* alpha, const double* be
   return cnt;
 }
 
+// Sturm multisection (one warp, 32 points per round) for the t-th smallest eigenvalue of the m x m tridiagonal: returns
+// the bracket [lo, hi) with count(lo) <= t < count(hi)
+__device__ __forceinline__ void tri_bracket(const double* alpha, const double* beta2, int m, int t, double gl, double gh,
+                                            int lane, double& lo_out, double& hi_out) {
+  double lo = gl, hi = gh;
+  for (int round = 0; round < 11; ++round) {
+    const double step = (hi - lo) / 33.0;
+    const double x = lo + step * (double)(lane + 1);
+    const int c = sturm_count(alpha, beta2, m, x);
+    const unsigned mask = __ballot_sync(0xffffffffu, c <= t);
+    const int np = __popc(mask);  // predicate is monotone: true for a prefix of lanes
+    const double nlo = (np > 0) ? lo + step * (double)np : lo;
+    const double nhi = (np < 32) ? lo + step * (double)(np + 1) : hi;
+    lo = nlo; hi = nhi;
+  }
+  lo_out = lo; hi_out = hi;
+}
+
+// Eigenvector (not normalised) of the m x m unreduced tridiagonal for its eigenvalue th by twisted factorisation
+// (one thread, sequential recurrences); tb: m doubles of scratch
+__device__ __forceinline__ void tri_twisted(const double* alpha, const double* beta, const double* beta2, int m, double th,
+                                            double* zs, double* tb) {
+  if (m == 1) {
+    zs[0] = 1.0;
+    return;
+  }
+  double dp = alpha[0] - th;
+  for (int i = 0; i < m - 1; ++i) {
+    if (dp == 0.0) dp = 1e-300;
+    zs[i] = dp;
+    dp = (alpha[i + 1] - th) - beta2[i] / dp;
+  }
+  if (dp == 0.0) dp = 1e-300;
+  zs[m - 1] = dp;
+  double dm = alpha[m - 1] - th;
+  double gmin = fabs(zs[m - 1] + dm - (alpha[m - 1] - th));
+  int r = m - 1;
+  if (dm == 0.0) dm = 1e-300;
+  tb[m - 1] = dm;
+  for (int i = m - 2; i >= 0; --i) {
+    dm = (alpha[i] - th) - beta2[i] / dm;
+    if (dm == 0.0) dm = 1e-300;
+    tb[i] = dm;
+    const double g = fabs(zs[i] + dm - (alpha[i] - th));
+    if (g < gmin) { gmin = g; r = i; }
+  }
+  // z_r = 1 ; upward z_i = -beta_i z_{i+1} / d+_i ; downward z_{i+1} = -beta_i z_i / d-_{i+1}
+  double z = 1.0;
+  zs[r] = 1.0;
+  // upward needs d+_i for i < r which are still stored in zs[i]
+  for (int i = r - 1; i >= 0; --i) {
+    z = -beta[i] * z / zs[i];
+    zs[i] = z;
+  }
+  z = 1.0;
+  for (int i = r; i < m - 1; ++i) {
+    z = -beta[i] * z / tb[i + 1];
+    zs[i + 1] = z;
+  }
+}
+
+// After a restart T is block diagonal (beta[i] == 0 between blocks). The block [b0, b1) that holds the t-th smallest
+// eigenvalue of the n x n T, bracketed by [lo, hi): the blocks take the eigenvalues inside the bracket in block order,
+// so a value repeated in several blocks is assigned to each of them once (one thread)
+__device__ __forceinline__ int tri_block_of(const double* alpha, const double* beta, const double* beta2, int n, int t,
+                                            double lo, double hi, int& b1) {
+  int m = t - sturm_count(alpha, beta2, n, lo);   // rank of the wanted eigenvalue among those in [lo, hi)
+  int b0 = 0;
+  for (;;) {
+    int e = b0 + 1;
+    while (e < n && beta[e - 1] != 0.0) ++e;
+    const int cnt = sturm_count(alpha + b0, beta2 + b0, e - b0, hi) - sturm_count(alpha + b0, beta2 + b0, e - b0, lo);
+    if (m < cnt || e >= n) {
+      b1 = e;
+      return b0;
+    }
+    m -= cnt;
+    b0 = e;
+  }
+}
+
 __host__ __device__ inline size_t eig_double_bytes(int mmax) {
   size_t nd = (size_t)3 * mmax + 2 * (EIG_MAX_K + 1) + EIG_WARPS;
   nd = (nd + 1) & ~(size_t)1;
@@ -131,6 +215,7 @@ lanczos_laplacian_kernel(EigParams p) {
   float* colbuf = ycol + Npad;                               // [NW][stripw] per-warp column accumulators
   float* coef = colbuf + (size_t)EIG_WARPS * stripw;         // [mmax + 2]
   __shared__ int s_flag;
+  __shared__ double s_top[2];   // top Ritz value of the newest block of T and its residual
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   float* basis = p.basis + (size_t)blockIdx.x * (size_t)(mmax + 1) * Npad;
@@ -192,6 +277,30 @@ lanczos_laplacian_kernel(EigParams p) {
     int n = 0;          // Lanczos steps done
     int converged = (Kw <= 0);
     bool have_theta = false;
+    int restarts = 0;   // breakdowns continued from a fresh start vector
+    int bs = 0;         // first step of the newest block of T
+    // two classical Gram-Schmidt passes of wv against u0, v_0 .. v_{j-1} (basis) and v_j (vcur); returns the sum of the
+    // v_j coefficients
+    auto cgs2 = [&](int j) -> double {
+      double aj = 0.0;
+      for (int pass = 0; pass < 2; ++pass) {
+        for (int i = warp; i < j + 2; i += NW) {
+          const float* a = (i == 0) ? u0 : ((i - 1 == j) ? vcur : basis + (size_t)(i - 1) * Npad);
+          const float c = warp_dot(a, wv, N, lane);
+          if (lane == 0) coef[i] = c;
+        }
+        __syncthreads();
+        aj += (double)coef[j + 1];
+        for (int i = tid; i < N; i += NT) {
+          float acc = coef[0] * u0[i];
+          for (int t = 0; t < j; ++t) acc = fmaf(coef[t + 1], basis[(size_t)t * Npad + i], acc);
+          acc = fmaf(coef[j + 1], vcur[i], acc);
+          wv[i] -= acc;
+        }
+        __syncthreads();
+      }
+      return aj;
+    };
     if (Kw > 0) {
       // ---- start vector: deterministic pseudo-random, orthogonal to u0
       for (int i = tid; i < Npad; i += NT) wv[i] = (i < N) ? hash_uniform((uint32_t)i, 0x1234567u) : 0.f;
@@ -336,23 +445,7 @@ lanczos_laplacian_kernel(EigParams p) {
         }
         __syncthreads();
         // ---- full re-orthogonalisation (CGS2) against u0, v_0..v_j ; alpha_j = sum of the v_j coefficients
-        double aj = 0.0;
-        for (int pass = 0; pass < 2; ++pass) {
-          for (int i = warp; i < j + 2; i += NW) {
-            const float* a = (i == 0) ? u0 : ((i - 1 == j) ? vcur : basis + (size_t)(i - 1) * Npad);
-            const float c = warp_dot(a, wv, N, lane);
-            if (lane == 0) coef[i] = c;
-          }
-          __syncthreads();
-          aj += (double)coef[j + 1];
-          for (int i = tid; i < N; i += NT) {
-            float acc = coef[0] * u0[i];
-            for (int t = 0; t < j; ++t) acc = fmaf(coef[t + 1], basis[(size_t)t * Npad + i], acc);
-            acc = fmaf(coef[j + 1], vcur[i], acc);
-            wv[i] -= acc;
-          }
-          __syncthreads();
-        }
+        const double aj = cgs2(j);
         double d = 0.0;
         for (int i = tid; i < N; i += NT) d += (double)wv[i] * (double)wv[i];
         const double bj = sqrt(block_sum<NW>(d, red, tid));
@@ -403,61 +496,23 @@ lanczos_laplacian_kernel(EigParams p) {
           for (int k = warp; k < kg; k += NW) {
             // k-th largest eigenvalue = ascending index t = n-1-k ; lambda_t >= x  <=>  count(x) <= t
             const int t = n - 1 - k;
-            double lo = gl, hi = gh;
-            for (int round = 0; round < 11; ++round) {
-              const double step = (hi - lo) / 33.0;
-              const double x = lo + step * (double)(lane + 1);
-              const int c = sturm_count(alpha, beta2, n, x);
-              const unsigned mask = __ballot_sync(0xffffffffu, c <= t);
-              const int np = __popc(mask);  // predicate is monotone: true for a prefix of lanes
-              const double nlo = (np > 0) ? lo + step * (double)np : lo;
-              const double nhi = (np < 32) ? lo + step * (double)(np + 1) : hi;
-              lo = nlo; hi = nhi;
-            }
+            double lo, hi;
+            tri_bracket(alpha, beta2, n, t, gl, gh, lane, lo, hi);
             const double th = 0.5 * (lo + hi);
-            // Ritz vector of T by twisted factorisation of T - th I (lane 0, sequential recurrences)
+            // unreduced block of T that holds this Ritz value (all of T unless a restart split it)
+            int b0 = 0, b1 = n;
+            if (restarts > 0) {
+              if (lane == 0) b0 = tri_block_of(alpha, beta, beta2, n, t, lo, hi, b1);
+              b0 = __shfl_sync(0xffffffffu, b0, 0);
+              b1 = __shfl_sync(0xffffffffu, b1, 0);
+            }
+            // Ritz vector of T by twisted factorisation of the block's T - th I, zero outside the block
             double* zs = triS + (size_t)k * mmax;
             double* tb = triB + (size_t)k * mmax;
             if (lane == 0) {
-              if (n == 1) {
-                zs[0] = 1.0;
-              } else {
-                double dp = alpha[0] - th;
-                for (int i = 0; i < n - 1; ++i) {
-                  if (dp == 0.0) dp = 1e-300;
-                  zs[i] = dp;
-                  dp = (alpha[i + 1] - th) - beta2[i] / dp;
-                }
-                if (dp == 0.0) dp = 1e-300;
-                zs[n - 1] = dp;
-                double dm = alpha[n - 1] - th;
-                double gmin = fabs(zs[n - 1] + dm - (alpha[n - 1] - th));
-                int r = n - 1;
-                if (dm == 0.0) dm = 1e-300;
-                tb[n - 1] = dm;
-                for (int i = n - 2; i >= 0; --i) {
-                  dm = (alpha[i] - th) - beta2[i] / dm;
-                  if (dm == 0.0) dm = 1e-300;
-                  tb[i] = dm;
-                  const double g = fabs(zs[i] + dm - (alpha[i] - th));
-                  if (g < gmin) { gmin = g; r = i; }
-                }
-                // z_r = 1 ; upward z_i = -beta_i z_{i+1} / d+_i ; downward z_{i+1} = -beta_i z_i / d-_{i+1}
-                double z = 1.0;
-                const double dpr = zs[r];
-                (void)dpr;
-                zs[r] = 1.0;
-                // upward needs d+_i for i < r which are still stored in zs[i]
-                for (int i = r - 1; i >= 0; --i) {
-                  z = -beta[i] * z / zs[i];
-                  zs[i] = z;
-                }
-                z = 1.0;
-                for (int i = r; i < n - 1; ++i) {
-                  z = -beta[i] * z / tb[i + 1];
-                  zs[i + 1] = z;
-                }
-              }
+              for (int i = 0; i < b0; ++i) zs[i] = 0.0;
+              for (int i = b1; i < n; ++i) zs[i] = 0.0;
+              tri_twisted(alpha + b0, beta + b0, beta2 + b0, b1 - b0, th, zs + b0, tb + b0);
             }
             __syncwarp();
             double nn = 0.0;
@@ -468,22 +523,84 @@ lanczos_laplacian_kernel(EigParams p) {
             __syncwarp();
             if (lane == 0) {
               theta[k] = th;
-              resid_s[k] = fabs(beta[n - 1] * zs[n - 1]);
+              resid_s[k] = fabs(beta[b1 - 1] * zs[b1 - 1]);   // beta is 0 at the end of a closed block
             }
           }
           __syncthreads();
+          // the newest block [bs, n) of T: its largest Ritz value and, while it is open, that value's residual
+          const bool exhausted = n + off >= N;   // the basis (with u0) spans the whole space
+          if (warp == 0 && (breakdown || restarts > 0) && !exhausted) {
+            const int m = n - bs;
+            double lo, hi;
+            tri_bracket(alpha + bs, beta2 + bs, m, m - 1, gl, gh, lane, lo, hi);
+            const double rho = 0.5 * (lo + hi);
+            double rr = 0.0;
+            if (!breakdown) {
+              double* zs = triB;          // the per-k temps are free again
+              if (lane == 0) tri_twisted(alpha + bs, beta + bs, beta2 + bs, m, rho, zs, triB + mmax);
+              __syncwarp();
+              double nn = 0.0;
+              for (int i = lane; i < m; i += 32) nn += zs[i] * zs[i];
+              nn = warp_sum(nn);
+              rr = fabs(beta[n - 1] * zs[m - 1]) / sqrt(nn);
+            }
+            if (lane == 0) { s_top[0] = rho; s_top[1] = rr; }
+          }
+          __syncthreads();
           if (tid == 0) {
+            const double tola = (double)p.tol * anorm;
             int ok = 1;
-            for (int k = 0; k < kk; ++k) ok &= (resid_s[k] <= (double)p.tol * anorm);
+            for (int k = 0; k < kk; ++k) ok &= (resid_s[k] <= tola);
             ok &= (kk == Kw);
-            if (kg > Kw && Kw > 0 && !breakdown && n < N - 1)   // guard: nothing hidden above the last wanted Ritz value
-              ok &= (theta[Kw] + resid_s[Kw] <= theta[Kw - 1] + (double)p.tol * anorm);
+            if (ok && !exhausted) {
+              if (breakdown) {
+                // the Krylov space of the block that just closed holds one vector per distinct eigenvalue of what was
+                // left of the space when the block started: whatever is still hidden is another copy of one of its Ritz
+                // values, so none may lie above the last wanted one
+                ok &= (s_top[0] <= theta[Kw - 1] + tola);
+              } else {
+                if (kg > Kw)   // guard: nothing hidden above the last wanted Ritz value
+                  ok &= (theta[Kw] + resid_s[Kw] <= theta[Kw - 1] + tola);
+                // after a restart the spectrum is known to repeat: a copy of any Ritz value of the open block may
+                // still be hidden outside the basis, so its largest one (with its residual) must not exceed the last
+                // wanted value; otherwise the block runs on to its breakdown and the next restart
+                if (restarts > 0) ok &= (s_top[0] + s_top[1] <= theta[Kw - 1] + tola);
+              }
+            }
             s_flag = ok;
           }
           __syncthreads();
           converged = s_flag;
           have_theta = true;
-          if (converged || breakdown) break;
+          if (converged) break;
+          if (breakdown) {
+            if (n == mmax || exhausted) break;   // no room for another block: not converged
+            // ---- restart: continue from a fresh pseudo-random vector orthogonal to u0 and the basis; T becomes block
+            // diagonal (beta_j = 0) and the next block finds the copies of repeated eigenvalues this one could not see
+            ++restarts;
+            double d0 = 0.0;
+            for (int i = tid; i < Npad; i += NT) {
+              const float v = (i < N) ? hash_uniform((uint32_t)i, 0x1234567u + (uint32_t)restarts) : 0.f;
+              wv[i] = v;
+              d0 += (double)v * (double)v;
+            }
+            const double n0s = sqrt(block_sum<NW>(d0, red, tid));   // (its barriers publish wv)
+            cgs2(j);
+            double d1 = 0.0;
+            for (int i = tid; i < N; i += NT) d1 += (double)wv[i] * (double)wv[i];
+            const double n1s = sqrt(block_sum<NW>(d1, red, tid));
+            if (!(n1s > 1e-3 * n0s)) break;   // nothing left outside the basis (rounding): not converged
+            const float inv = (float)(1.0 / n1s);
+            float* vn = basis + (size_t)(j + 1) * Npad;
+            for (int i = tid; i < Npad; i += NT) {
+              const float v = (i < N) ? wv[i] * inv : 0.f;
+              vcur[i] = v;
+              vn[i] = v;
+            }
+            if (tid == 0) { beta[j] = 0.0; beta2[j] = 0.0; }
+            bs = j + 1;
+            __syncthreads();
+          }
         }
       }
     }
@@ -509,7 +626,7 @@ lanczos_laplacian_kernel(EigParams p) {
         p.info[img * 4 + 0] = n;
         p.info[img * 4 + 1] = converged ? 1 : 0;
         p.info[img * 4 + 2] = lm_differs;
-        p.info[img * 4 + 3] = 0;
+        p.info[img * 4 + 3] = restarts;
       }
     }
     const int have = min(Kw, n);  // Ritz pairs available
@@ -554,9 +671,11 @@ static size_t eig_smem_bytes(int Npad, int mmax) {
          (size_t)(mmax + 2) * sizeof(float) + 16;
 }
 
-static int eig_resolve(int N, int K, int max_steps) {
+// Lanczos steps: the Laplacian modes work in the N - 1 dimensions orthogonal to the analytic null vector, the plain
+// mode in all N
+static int eig_resolve(int N, int K, int max_steps, bool plain) {
   int mmax = max_steps > 0 ? max_steps : 320;
-  if (mmax > N - 1) mmax = N - 1;
+  if (mmax > (plain ? N : N - 1)) mmax = plain ? N : N - 1;
   if (mmax < K) mmax = K;
   if (mmax < 1) mmax = 1;
   return mmax;
@@ -593,11 +712,15 @@ using namespace dss;
 extern "C" size_t dss_eigsh_workspace_bytes(int B, int N, int K, int max_steps) {
   if (B <= 0 || N <= 0 || K <= 0) return 0;
   const int Npad = (N + 3) & ~3;
-  const int mmax = eig_resolve(N, K, max_steps);
-  const int grid = eig_grid(B, Npad, mmax);
-  const size_t basis = align_up((size_t)grid * (mmax + 1) * Npad * sizeof(float), 256);
-  const size_t tri = align_up((size_t)grid * 2 * (K + 1) * mmax * sizeof(double), 256);
-  return basis + tri;
+  size_t bytes = 0;
+  for (const bool plain : {false, true}) {   // one size serves both entry points
+    const int mmax = eig_resolve(N, K, max_steps, plain);
+    const int grid = eig_grid(B, Npad, mmax);
+    const size_t basis = align_up((size_t)grid * (mmax + 1) * Npad * sizeof(float), 256);
+    const size_t tri = align_up((size_t)grid * 2 * (K + 1) * mmax * sizeof(double), 256);
+    bytes = basis + tri > bytes ? basis + tri : bytes;
+  }
+  return bytes;
 }
 
 static int eigsh_launch(const float* Wmat, const float* deg, int ldw, int B, int N, int K, int mode, float tol, int max_steps,
@@ -617,7 +740,7 @@ static int eigsh_launch(const float* Wmat, const float* deg, int ldw, int B, int
   EigParams p;
   p.W = Wmat; p.deg = deg; p.evals = evals; p.evecs = evecs; p.info = info; p.resid = resid;
   p.B = B; p.N = N; p.ldw = ldw; p.Npad = (N + 3) & ~3; p.K = K; p.mode = mode;
-  p.mmax = eig_resolve(N, K, max_steps);
+  p.mmax = eig_resolve(N, K, max_steps, mode == 2);
   p.tol = tol > 0.f ? tol : 1e-6f;
   const int grid = eig_grid(B, p.Npad, p.mmax);
   p.basis = reinterpret_cast<float*>(ws);

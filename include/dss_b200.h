@@ -188,9 +188,16 @@ int dss_knn_color_counts(const float* rgb, int B, int Hl, int Wl, uint8_t* count
  *                 extract_utils.py:217-218); eigenvectors D-orthonormal            extract.py:225-229
  *   lapnorm == 0: K smallest pairs of (D - W) v = lambda v, unit 2-norm vectors    extract.py:230-234
  * Outputs: evals [B, K] ascending, evecs [B, K, N] with the reference's sign rule applied (extract.py:237-240),
- * info [B, 4] int32 = {lanczos steps, converged(1/0), 0, 0}, resid [B, K] fp32 residual estimates (may be NULL).
+ * info [B, 4] int32, resid [B, K] fp32 residual estimates (may be NULL):
+ *   info[b,0] Lanczos steps taken, restarts included
+ *   info[b,1] 1 when the K pairs returned are eigenpairs to tol (repeated eigenvalues with all their copies, vectors
+ *             orthonormal), else 0: the step budget ran out first; pairs that do not exist yet are NaN
+ *   info[b,2] dss_eigsh_topk only: a negative eigenvalue is larger in magnitude than the K-th (see below); else 0
+ *   info[b,3] restarts: Lanczos breakdowns (an invariant Krylov subspace, e.g. at an eigenvalue of multiplicity > 1)
+ *             continued from a fresh start vector orthogonal to the basis; 0 on ordinary spectra
  * Method: Lanczos with full re-orthogonalisation on D^-1/2 W D^-1/2 (null vector deflated analytically), Ritz
- * values by Sturm bisection in fp64. tol <= 0 selects 1e-6; max_steps <= 0 selects min(N-1, 320). */
+ * values by Sturm bisection in fp64. tol <= 0 selects 1e-6; max_steps <= 0 selects min(N-1, 320) (min(N, 320) for
+ * dss_eigsh_topk). Restarts draw on the same budget. */
 size_t dss_eigsh_workspace_bytes(int B, int N, int K, int max_steps);
 int dss_eigsh_laplacian(const float* Wmat, const float* degree, int ldw, int B, int N, int K, int lapnorm, float tol,
                         int max_steps, float* evals, float* evecs, int* info, float* resid, void* ws, size_t ws_bytes,
