@@ -183,6 +183,17 @@ __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t rank)
       ::"r"(bar), "r"(rank)
       : "memory");
 }
+// The same arrive without release semantics, for a consumer handing back a ring slot it has only read through wgmma
+// (its reads have retired at wgmma.wait_group, so there is nothing to publish). The .release.cluster form above
+// compiles to MEMBAR.ALL.GPU before every arrive, which also waits for the thread's outstanding global writes.
+__device__ __forceinline__ void mbar_arrive_cluster_relaxed(uint32_t bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(bar), "r"(rank)
+      : "memory");
+}
 // 2D tiled load, multicast: the box lands at the same shared-memory offset in every CTA of `cta_mask`, and each
 // destination CTA's mbarrier (same offset) receives the complete_tx for the bytes written into that CTA
 __device__ __forceinline__ void tma_load_2d_mc(uint32_t smem_dst, const CUtensorMap* tm, uint32_t bar, int c0, int c1,

@@ -13,8 +13,15 @@
 // operand. A slab is free once the MMA groups of both CTAs have retired their wgmmas on it.
 // Both operands are K-major, which is the native layout of activations [rows, features] and of torch Linear
 // weights [out, in]; no transposes anywhere.
+//
+// Two schedules share the producer and the cluster / ring protocol:
+//   cooperative (gemm_f16_wgmma_kernel): both MMA groups work on the same 128 x BN tile, each on 64 of its rows, so the
+//     tensor cores idle while the tile's epilogue runs. Used by the row-remapping epilogues, the affinity GEMM (whose
+//     symmetric mode keeps the CTA pair in lock step) and dss_debug_gemm_cfg.
+//   ping-pong (gemm_f16_pingpong_kernel): each MMA group owns whole 128 x 128 tiles and the two groups take alternate
+//     work items; a pair of named barriers hands the "MMA turn" from one group to the other, so one group's epilogue
+//     runs under the other group's wgmmas. Used by the four ViT epilogues (qkv, proj, fc1, fc2).
 #include <math.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -38,19 +45,25 @@ __host__ __device__ constexpr bool epi_uses_tma_store(int epi) {
 }
 // Ring stage = one 64-deep K slab of A (128 rows) and B (BN rows); as many stages as the shared-memory budget leaves
 // next to the output staging (at most 6).
-template <int EPI, int BN> struct TileCfg {
+// Ping-pong (PP): 32 KB stages of 128 x 128 tiles next to two double-buffered 16 KB boxes per group = 5 stages
+// (6 * 32 + 4 * 16 KB would not fit). Double buffering keeps a group's store of one box under its writes of the next.
+template <int EPI, int BN, bool PP = false> struct TileCfg {
   static constexpr int B_ATOM_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_ATOM_BYTES + B_ATOM_BYTES;   // [A slab | B slab]
-  // TMA path: two swizzled output boxes (+ the affinity epilogue's row-major fp32 copy of one box); manual path: two
-  // fp32 chunks
-  static constexpr int STAGING_BYTES = epi_uses_tma_store(EPI) ? 2 * BOX_BYTES + (EPI == EPI_AFFINITY_F32 ? STG_BYTES : 0)
-                                                              : 2 * STG_BYTES;
+  // TMA path: two swizzled output boxes (+ the affinity epilogue's row-major fp32 copy of one box), two per consumer
+  // warp group for the ping-pong schedule; manual path: two fp32 chunks
+  static constexpr int STAGING_BYTES = PP ? CONSUMER_WGS * 2 * BOX_BYTES
+                                     : epi_uses_tma_store(EPI) ? 2 * BOX_BYTES + (EPI == EPI_AFFINITY_F32 ? STG_BYTES : 0)
+                                                               : 2 * STG_BYTES;
   static constexpr int MAX_STAGES = (SMEM_LIMIT - 1024 - 256 - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = MAX_STAGES > 6 ? 6 : MAX_STAGES;
   // ring | staging | barriers | alignment slack
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 256 + 1024;
   static_assert(STAGES >= 2, "shared memory budget");
 };
+// Ping-pong tile: 128 x 128 per consumer warp group, two m64n128k16 per k-step (128 accumulator registers per thread)
+constexpr int PP_BN = 128;
+static_assert(TileCfg<DSS_EPI_BIAS_F16, PP_BN, true>::STAGES == 5, "ping-pong ring depth");
 
 
 struct EpiParams {
@@ -73,7 +86,22 @@ struct EpiParams {
   int tri;
   float* deg_part;
   int ld_part;
+  // phase trace (dss_debug_gemm_trace only; read by the TRACE instantiations, layout at trace_stride)
+  unsigned long long* trace;
 };
+
+// Phase trace layout, per CTA (blockIdx.x): [0] ns the producer warp spent waiting on empty ring slots, [1..3] unused,
+// then for consumer warp group w and the j-th tile that group ran, four %globaltimer stamps at 4 + 4 * (w * tmax + j):
+// tile start (for the ping-pong schedule: once the group holds the MMA turn), first full-barrier wait satisfied, last
+// wgmma retired (wgmma_wait<0>), epilogue issued. tmax = cdiv(work items, clusters) bounds the tiles of one CTA.
+__host__ __device__ constexpr long long trace_stride(int total_items, int clusters) {
+  return 4 + 8ll * ((total_items + clusters - 1) / clusters);
+}
+__device__ __forceinline__ unsigned long long globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
+}
 
 // Row of the output buffer that GEMM row m maps to (or -1: skip).
 template <int EPI>
@@ -154,11 +182,58 @@ __device__ __forceinline__ TileCoord decode_tile(int t, int pairs_m, int tiles_n
 // same columns 8 rows further down.
 __device__ __forceinline__ int frag_row(int wg, int wi, int lane) { return 64 * wg + 16 * wi + (lane >> 2); }
 
-template <int EPI, int BN>
+// TMA producer (warp 0 of warp group 0) of both schedules: the CTA's work items in order, one ring slot per 64-deep K
+// slab, the ring position carried across tiles. The whole warp runs the loop with warp-uniform values; one elected
+// lane issues. The slab a slot held is free once one consumer group of EACH CTA has released it (empty barrier).
+template <int BN, int STAGES, int STAGE_BYTES, bool TRACE>
+__device__ __forceinline__ void produce(const CUtensorMap* tmA, const CUtensorMap* tmB, uint32_t base, uint32_t bar_base,
+                                        int num_kb, int cid, int ncl, int rank, int pairs_m, int tiles_n,
+                                        int total_items, const EpiParams& p) {
+  constexpr int B_ATOM_BYTES = BN * BK * 2;
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  const int lane = threadIdx.x & 31;
+  const uint32_t ubase = __shfl_sync(0xffffffffu, base, 0);
+  [[maybe_unused]] unsigned long long waited = 0;
+  int s = 0;
+  uint32_t ph = 0;   // ring position, carried across tiles
+  for (int t = cid; t < total_items; t += ncl) {
+    const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
+    const int row_base = tc.z * p.batch_rows;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      [[maybe_unused]] unsigned long long t0;
+      if constexpr (TRACE) t0 = globaltimer();
+      mbar_wait(empty_bar(s), ph ^ 1u);
+      if constexpr (TRACE) waited += globaltimer() - t0;
+      const uint32_t sa = ubase + s * STAGE_BYTES;
+      const uint32_t fb = full_bar(s);
+      // split-fp16 Gram product: A = [hi | hi/64 | 64 lo], B = [hi | 64 lo | hi/64] are the same array read with the
+      // last two groups of K slabs swapped
+      int kbB = kb;
+      if (p.perm_blocks > 0 && kb >= p.perm_blocks && kb < 3 * p.perm_blocks)
+        kbB = kb < 2 * p.perm_blocks ? kb + p.perm_blocks : kb - p.perm_blocks;
+      if (elect_one()) {
+        mbar_arrive_expect_tx(fb, STAGE_BYTES);
+        tma_load_2d(sa, tmA, fb, kb * BK, row_base + tc.m0);
+        // this CTA's half of the weight slab (box 64 x BN/2 rows), delivered to both CTAs of the pair
+        tma_load_2d_mc(sa + A_ATOM_BYTES + rank * (B_ATOM_BYTES / 2), tmB, fb, kbB * BK,
+                       row_base + tc.n0 + rank * (BN / 2), (uint16_t)0x3);
+      }
+      __syncwarp();
+      if (++s == STAGES) { s = 0; ph ^= 1u; }
+    }
+  }
+  if constexpr (TRACE) {
+    if (lane == 0) p.trace[blockIdx.x * trace_stride(total_items, ncl)] = waited;
+  }
+}
+
+template <int EPI, int BN, bool TRACE = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const __grid_constant__ CUtensorMap tmC, int M, int N, int K, int pairs_m, int tiles_n,
                       int total_items, EpiParams p) {
+  static_assert(!TRACE || (epi_uses_tma_store(EPI) && EPI != EPI_AFFINITY_F32), "traced: the four ViT epilogues only");
   using Cfg = TileCfg<EPI, BN>;
   constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
@@ -194,35 +269,9 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 
   if (warp < 4) {
     setmaxnreg_dec<40>();
-    if (warp == 0) {
-      // The whole warp runs the loop with warp-uniform values; one elected lane issues.
-      const uint32_t ubase = __shfl_sync(0xffffffffu, base, 0);
-      int s = 0;
-      uint32_t ph = 0;   // ring position, carried across tiles
-      for (int t = cid; t < total_items; t += ncl) {
-        const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
-        const int row_base = tc.z * p.batch_rows;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(empty_bar(s), ph ^ 1u);
-          const uint32_t sa = ubase + s * STAGE_BYTES;
-          const uint32_t fb = full_bar(s);
-          // split-fp16 Gram product: A = [hi | hi/64 | 64 lo], B = [hi | 64 lo | hi/64] are the same array read with the
-          // last two groups of K slabs swapped
-          int kbB = kb;
-          if (p.perm_blocks > 0 && kb >= p.perm_blocks && kb < 3 * p.perm_blocks)
-            kbB = kb < 2 * p.perm_blocks ? kb + p.perm_blocks : kb - p.perm_blocks;
-          if (elect_one()) {
-            mbar_arrive_expect_tx(fb, STAGE_BYTES);
-            tma_load_2d(sa, &tmA, fb, kb * BK, row_base + tc.m0);
-            // this CTA's half of the weight slab (box 64 x BN/2 rows), delivered to both CTAs of the pair
-            tma_load_2d_mc(sa + A_ATOM_BYTES + rank * (Cfg::B_ATOM_BYTES / 2), &tmB, fb, kbB * BK,
-                           row_base + tc.n0 + rank * (BN / 2), (uint16_t)0x3);
-          }
-          __syncwarp();
-          if (++s == STAGES) { s = 0; ph ^= 1u; }
-        }
-      }
-    }
+    if (warp == 0)
+      produce<BN, STAGES, STAGE_BYTES, TRACE>(&tmA, &tmB, base, bar_base, num_kb, cid, ncl, rank, pairs_m, tiles_n,
+                                              total_items, p);
   } else {
     setmaxnreg_inc<232>();
     const int ct = threadIdx.x - 128;               // consumer thread 0..255
@@ -236,13 +285,18 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     float acc[BN / 2];
     [[maybe_unused]] float aff_rowsum[2] = {0.f, 0.f};   // affinity: row sums of this thread's two column slices
     [[maybe_unused]] float aff_mx = 1.f, aff_rmx = 1.f, aff_unscale = 1.f;
+    [[maybe_unused]] unsigned long long* trec = nullptr;   // traced: this group's record of the current tile
+    if constexpr (TRACE) trec = p.trace + blockIdx.x * trace_stride(total_items, ncl) + 4 + 4 * wg * ((total_items + ncl - 1) / ncl);
+    const bool tracer = TRACE && (ct & 127) == 0;
     for (int t = cid; t < total_items; t += ncl) {
       const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
+      if (tracer) trec[0] = globaltimer();
       // ---- main loop: 4 wgmma k-steps per 64-deep slab; a slab is released (in both CTAs) once the wgmmas of the
       // NEXT slab have been issued and the older group has retired
       int prev = -1;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(full_bar(s), ph);
+        if (tracer && kb == 0) trec[1] = globaltimer();
         __syncwarp();   // wgmma is warp-aligned: reconverge after the per-thread barrier spin
         const uint32_t sa = base + s * STAGE_BYTES;
         const uint64_t adesc = wgmma_desc_sw128(sa + wg * 64 * 128);
@@ -262,6 +316,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       }
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
+      if (tracer) trec[2] = globaltimer();
       if ((ct & 127) == 0) {
         mbar_arrive_cluster(empty_bar(prev), 0);
         mbar_arrive_cluster(empty_bar(prev), 1);
@@ -480,6 +535,10 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
           }
           ++cc;   // (boxes that skip the staging buffers -- diagonal affinity tiles -- do not advance the buffer parity)
         }
+        if (tracer) {
+          trec[3] = globaltimer();
+          trec += 4;
+        }
       } else {
         // ---- row-remapping epilogues: 32-column chunks through a row-major fp32 staging buffer (double buffered),
         // then row-contiguous (coalesced) global reads of the aux rows and writes of the result
@@ -541,6 +600,186 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Ping-pong schedule for the TMA-store epilogues. Item i of the CTA (t = cid + i * ncl, the same sequence in both CTAs
+// of the pair) belongs to consumer group i % 2, so the ring holds the groups' slabs alternately, num_kb at a time, and
+// a slot is released by one group in each CTA. Named barriers (IDs 1 + g: group g may issue; 3 + g: group g's
+// epilogue) order the groups: item i > 0 waits (bar.sync, 256 threads) until the group of item i - 1 has issued its
+// last wgmma and arrived (bar.arrive) -- which that group does only when an item i exists, so every arrive has exactly
+// one matching sync, for any number of items per CTA (an idle group waits for nothing and is waited for by nothing).
+// The turn also keeps the parity waits on the full barriers sound: when a group starts item i, every slab of the items
+// before it has arrived, so the previous use of each slot it waits on has completed (a wait is never two phases ahead).
+// Each output element sums the same K slabs in the same order as under the cooperative schedule.
+constexpr int PP_TURN_BAR = 1, PP_EPI_BAR = 3;
+template <int EPI, bool TRACE = false>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                         const __grid_constant__ CUtensorMap tmC, int M, int N, int K, int pairs_m, int tiles_n,
+                         int total_items, EpiParams p) {
+  static_assert(epi_uses_tma_store(EPI) && EPI != EPI_AFFINITY_F32, "ping-pong: the four ViT epilogues only");
+  constexpr int BN = PP_BN;
+  using Cfg = TileCfg<EPI, BN, true>;
+  constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw = smem_u32(smem_raw);
+  const uint32_t base = (raw + 1023u) & ~1023u;   // SWIZZLE_128B alignment
+  const uint32_t bar_base = base + STAGES * STAGE_BYTES + Cfg::STAGING_BYTES;
+  auto full_bar = [&](int s) { return bar_base + 8u * s; };
+  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const int num_kb = (K + BK - 1) / BK;
+  const int rank = (int)cluster_ctarank();
+  const int cid = blockIdx.x >> 1, ncl = gridDim.x >> 1;
+
+  if (warp == 0 && lane == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    tma_prefetch_desc(&tmC);
+    for (int s = 0; s < STAGES; ++s) {
+      mbar_init(full_bar(s), 1);
+      mbar_init(empty_bar(s), 2);   // one consumer group of each CTA
+    }
+    mbar_fence_init();
+  }
+  __syncthreads();
+  cluster_sync_all();
+
+  if (warp < 4) {
+    setmaxnreg_dec<40>();
+    if (warp == 0)
+      produce<BN, STAGES, STAGE_BYTES, TRACE>(&tmA, &tmB, base, bar_base, num_kb, cid, ncl, rank, pairs_m, tiles_n,
+                                              total_items, p);
+  } else {
+    setmaxnreg_inc<232>();
+    const int ct = threadIdx.x - 128;
+    const int wg = ct >> 7, wi = (ct >> 5) & 3;
+    const int fc = 2 * (lane & 3);
+    const bool issuer = (ct & 127) == 0;   // issues this group's stores and releases its slabs
+    const uint32_t stage_u32 = base + STAGES * STAGE_BYTES + wg * 2 * BOX_BYTES;   // this group's two boxes
+    int s = 0, cc = 0;
+    uint32_t ph = 0;
+    if (wg == 1) {   // the ring position of item 1: item 0's slabs come first
+      s = num_kb % STAGES;
+      ph = (num_kb / STAGES) & 1;
+    }
+    float acc[2][64];   // rows 0-63 and 64-127 of the tile
+    [[maybe_unused]] unsigned long long* trec = nullptr;
+    if constexpr (TRACE) trec = p.trace + blockIdx.x * trace_stride(total_items, ncl) + 4 + 4 * wg * ((total_items + ncl - 1) / ncl);
+    const bool tracer = TRACE && issuer;
+    for (int t = cid + wg * ncl; t < total_items; t += 2 * ncl) {
+      if (t != cid) {   // wait for the MMA turn
+        __syncwarp();
+        asm volatile("bar.sync %0, 256;" ::"r"(PP_TURN_BAR + wg) : "memory");
+      }
+      const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank);
+      if (tracer) trec[0] = globaltimer();
+      int prev = -1;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(full_bar(s), ph);
+        if (tracer && kb == 0) trec[1] = globaltimer();
+        __syncwarp();   // wgmma is warp-aligned: reconverge after the per-thread barrier spin
+        const uint32_t sa = base + s * STAGE_BYTES;
+        const uint64_t adesc0 = wgmma_desc_sw128(sa), adesc1 = wgmma_desc_sw128(sa + 64 * 128);
+        const uint64_t bdesc = wgmma_desc_sw128(sa + A_ATOM_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < BK / MMA_K; ++k) {
+          Wgmma<BN>::ss(acc[0], adesc0 + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
+          Wgmma<BN>::ss(acc[1], adesc1 + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();
+        if (prev >= 0 && issuer) {
+          mbar_arrive_cluster_relaxed(empty_bar(prev), 0);
+          mbar_arrive_cluster_relaxed(empty_bar(prev), 1);
+        }
+        prev = s;
+        if (++s == STAGES) { s = 0; ph ^= 1u; }
+      }
+      // hand the MMA turn to the group of the next item (its wgmmas queue behind this tile's last ones)
+      if (t + ncl < total_items) {
+        __syncwarp();
+        asm volatile("bar.arrive %0, 256;" ::"r"(PP_TURN_BAR + (wg ^ 1)) : "memory");
+      }
+      wgmma_wait<0>();
+      wgmma_fence_acc(acc[0]);
+      wgmma_fence_acc(acc[1]);
+      if (tracer) trec[2] = globaltimer();
+      if (issuer) {
+        mbar_arrive_cluster_relaxed(empty_bar(prev), 0);
+        mbar_arrive_cluster_relaxed(empty_bar(prev), 1);
+      }
+      // skip the other group's item in the ring
+      s += num_kb % STAGES;
+      ph ^= (num_kb / STAGES) & 1;
+      if (s >= STAGES) { s -= STAGES; ph ^= 1u; }
+
+      // ---- epilogue, as in the cooperative kernel but on this group's 128 rows and boxes: +bias (-> GELU) -> 128 B-
+      // swizzled staging box -> TMA store / reduce-add
+      constexpr bool OUT16 = (EPI == DSS_EPI_BIAS_F16 || EPI == DSS_EPI_BIAS_GELU_F16);
+      constexpr int BOXC = OUT16 ? 64 : 32;
+      constexpr int NBOX = BN / BOXC;
+#pragma unroll
+      for (int b = 0; b < NBOX; ++b) {
+        const int nc = tc.n0 + b * BOXC;
+        // the box is free once the store this group issued two boxes ago has finished READING it
+        if (issuer) tma_store_wait_read<1>();
+        __syncwarp();
+        asm volatile("bar.sync %0, 128;" ::"r"(PP_EPI_BAR + wg) : "memory");
+        const uint32_t sbuf = stage_u32 + (cc & 1) * BOX_BYTES;
+#pragma unroll
+        for (int i = 0; i < BOXC / 8; ++i) {
+          const int ci = b * (BOXC / 8) + i;
+          const int col = nc + 8 * i + fc;
+          float2 bv = make_float2(0.f, 0.f);
+          if (p.bias != nullptr && col < N) bv = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+#pragma unroll
+          for (int hr = 0; hr < 4; ++hr) {   // row half hr / 2, fragment row + 8 (hr % 2)
+            const int h = hr >> 1, e = hr & 1;
+            const int row = frag_row(h, wi, lane) + 8 * e;
+            float x0 = acc[h][4 * ci + 2 * e] + bv.x, x1 = acc[h][4 * ci + 2 * e + 1] + bv.y;
+            // the next tile's first wgmma ignores the accumulators (scale-d 0), but its asm reads them: constants
+            // instead of values let the registers serve the rest of this epilogue
+            acc[h][4 * ci + 2 * e] = acc[h][4 * ci + 2 * e + 1] = 0.f;
+            if constexpr (EPI == DSS_EPI_BIAS_GELU_F16) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
+            if constexpr (OUT16) {
+              const uint32_t addr = sbuf + row * 128 + ((i ^ (row & 7)) << 4) + (lane & 3) * 4;
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_half2(x0, x1)) : "memory");
+            } else {
+              const int j = 2 * i + ((lane & 3) >> 1);
+              const uint32_t addr = sbuf + row * 128 + ((j ^ (row & 7)) << 4) + (lane & 1) * 8;
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x0), "f"(x1) : "memory");
+            }
+          }
+        }
+        fence_proxy_async_smem();   // generic-proxy smem writes -> visible to the TMA (async proxy)
+        __syncwarp();
+        asm volatile("bar.sync %0, 128;" ::"r"(PP_EPI_BAR + wg) : "memory");
+        if (issuer) {
+          if (nc < N) {
+            if constexpr (EPI == DSS_EPI_BIAS_RESID_F32)
+              tma_reduce_add_2d(&tmC, sbuf, nc, tc.m0);
+            else
+              tma_store_2d(&tmC, sbuf, nc, tc.m0);
+          }
+          tma_store_commit();
+        }
+        ++cc;
+      }
+      if (tracer) {
+        trec[3] = globaltimer();
+        trec += 4;
+      }
+    }
+    if (issuer) tma_store_wait_all<0>();
+  }
+  __syncwarp();
+  __syncthreads();
+  cluster_sync_all();   // the peer may still multicast / arrive into this CTA's shared memory until it is done too
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // CUDA-core checker with the same epilogues (tests only).
 template <int EPI>
 __global__ void gemm_f16_simt_kernel(const __half* __restrict__ A, const __half* __restrict__ Wt, int M, int N, int K,
@@ -582,13 +821,12 @@ static PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
-// Tile width used for an N-column GEMM (B operand = weights [N, K]): the widest of 256 / 192 / 128 that divides N.
-int gemm_tile_n(int N) {
-  static const char* force = getenv("DSS_GEMM_BN");  // tuning override (experiments only)
-  if (force) return atoi(force);
-  // operand bytes per FLOP fall with BN
-  return N % 256 == 0 ? 256 : (N % 192 == 0 ? 192 : 128);
-}
+// Tile width the weight tensor maps of the TMA-store epilogues (the ping-pong schedule) are built for.
+int gemm_tile_n() { return PP_BN; }
+
+// Tile width of the cooperative schedule for an N-column GEMM: the widest of 256 / 192 / 128 that divides N (operand
+// bytes per FLOP fall with BN).
+static int coop_tile_n(int N) { return N % 256 == 0 ? 256 : (N % 192 == 0 ? 192 : 128); }
 
 // 2D fp16 row-major [rows, cols] tensor, box = 64 columns x box_rows rows, 128 B swizzle, zero fill out of bounds.
 int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_rows) {
@@ -672,14 +910,26 @@ int make_tmap_out3d_f16(CUtensorMap* tm, const void* ptr, int images, int rows, 
   return DSS_OK;
 }
 
-template <int EPI, int BN>
+// CTA pairs of a persistent launch over `items` work items: one CTA per SM
+static int gemm_clusters(int items) {
+  int sms = device_sm_count();
+  if (sms <= 0) sms = 132;
+  return items < sms / 2 ? items : sms / 2;
+}
+
+// PP: ping-pong schedule (BN == PP_BN), else cooperative; TRACE: the phase-traced instantiation (p.trace)
+template <int EPI, int BN, bool PP = false, bool TRACE = false>
 static int launch_tc_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, int M, int N, int K,
                         const EpiParams& p, cudaStream_t st, int kclass, int batch) {
-  using Cfg = TileCfg<EPI, BN>;
+  static_assert(!PP || BN == PP_BN, "ping-pong tile width");
+  using Cfg = TileCfg<EPI, BN, PP>;
+  constexpr auto kernel = [] {
+    if constexpr (PP) return gemm_f16_pingpong_kernel<EPI, TRACE>;
+    else return gemm_f16_wgmma_kernel<EPI, BN, TRACE>;
+  }();
   static bool attr_set = false;
   if (!attr_set) {
-    DSS_CHECK_CUDA(cudaFuncSetAttribute(gemm_f16_wgmma_kernel<EPI, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg::SMEM_BYTES));
+    DSS_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     attr_set = true;
   }
   const int pairs_m = cdiv(cdiv(M, BM), 2), tiles_n = cdiv(N, BN);
@@ -689,9 +939,7 @@ static int launch_tc_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
     for (int q = 0; q < pairs_m; ++q) per_img += tiles_n - 2 * q > 0 ? tiles_n - 2 * q : 0;
   }
   const int total = per_img * batch;   // work items of a CTA pair
-  int sms = device_sm_count();
-  if (sms <= 0) sms = 132;
-  const int clusters = total < sms / 2 ? total : sms / 2;
+  const int clusters = gemm_clusters(total);
   if (epi_uses_tma_store(EPI) && tmC == nullptr) {
     set_error("gemm: this epilogue needs an output tensor map");
     return DSS_ERR_BAD_ARG;
@@ -709,29 +957,39 @@ static int launch_tc_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
   attr[0].val.clusterDim.z = 1;
   cfg.attrs = attr;
   cfg.numAttrs = 1;
-  DSS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_f16_wgmma_kernel<EPI, BN>, tmA, tmB, tmC ? *tmC : tmA, M, N, K,
-                                    pairs_m, tiles_n, total, p));
+  DSS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, tmC ? *tmC : tmA, M, N, K, pairs_m, tiles_n, total, p));
   DSS_CHECK_CUDA(cudaGetLastError());
   return DSS_OK;
 }
 
-// bn = tile width the B tensor map was built for (its TMA box has bn / 2 rows)
-template <int EPI>
+// Cooperative schedule; bn = tile width the B tensor map was built for (its TMA box has bn / 2 rows)
+template <int EPI, bool TRACE = false>
 static int launch_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, int M, int N, int K,
                      const EpiParams& p, cudaStream_t st, int kclass, int bn, int batch = 1) {
   switch (bn) {
-    case 128: return launch_tc_bn<EPI, 128>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
+    case 128: return launch_tc_bn<EPI, 128, false, TRACE>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
     case 192:
       if constexpr (epi_uses_tma_store(EPI) && EPI != EPI_AFFINITY_F32)
-        return launch_tc_bn<EPI, 192>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
+        return launch_tc_bn<EPI, 192, false, TRACE>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
       break;
     case 256:
       if constexpr (epi_uses_tma_store(EPI) && EPI != EPI_AFFINITY_F32)
-        return launch_tc_bn<EPI, 256>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
+        return launch_tc_bn<EPI, 256, false, TRACE>(tmA, tmB, tmC, M, N, K, p, st, kclass, batch);
       break;
   }
   set_error("gemm: unsupported tile width %d", bn);
   return DSS_ERR_BAD_ARG;
+}
+
+// Ping-pong schedule (the B tensor map's box has PP_BN / 2 rows)
+template <int EPI, bool TRACE = false>
+static int launch_pp(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, int M, int N, int K,
+                     const EpiParams& p, cudaStream_t st, int kclass, int bn) {
+  if (bn != PP_BN) {
+    set_error("gemm: the weight tensor map must be built for tile width %d (got %d)", PP_BN, bn);
+    return DSS_ERR_BAD_ARG;
+  }
+  return launch_tc_bn<EPI, PP_BN, true, TRACE>(tmA, tmB, tmC, M, N, K, p, st, kclass, 1);
 }
 
 static int check_gemm_args(int M, int N, int K, int epi, const float* bias, const void* out, const float* aux,
@@ -753,10 +1011,10 @@ int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
   if (rc) return rc;
   EpiParams p{out, bias, aux, N, rin, rout, 0, nullptr, nullptr, nullptr, 0.f, 0, 0, 0, nullptr, 0};
   switch (epi) {
-    case DSS_EPI_BIAS_F16: return launch_tc<DSS_EPI_BIAS_F16>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
-    case DSS_EPI_BIAS_GELU_F16: return launch_tc<DSS_EPI_BIAS_GELU_F16>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
-    case DSS_EPI_BIAS_RESID_F32: return launch_tc<DSS_EPI_BIAS_RESID_F32>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
-    case DSS_EPI_BIAS_F32: return launch_tc<DSS_EPI_BIAS_F32>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
+    case DSS_EPI_BIAS_F16: return launch_pp<DSS_EPI_BIAS_F16>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
+    case DSS_EPI_BIAS_GELU_F16: return launch_pp<DSS_EPI_BIAS_GELU_F16>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
+    case DSS_EPI_BIAS_RESID_F32: return launch_pp<DSS_EPI_BIAS_RESID_F32>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
+    case DSS_EPI_BIAS_F32: return launch_pp<DSS_EPI_BIAS_F32>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
     case DSS_EPI_PATCH_F32: return launch_tc<DSS_EPI_PATCH_F32>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
     case DSS_EPI_DROPCLS_F32: return launch_tc<DSS_EPI_DROPCLS_F32>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
   }
@@ -800,7 +1058,7 @@ extern "C" int dss_op_gemm_f16(const void* A, const void* Wt, const float* bias,
   if (rc) return rc;
   DSS_REQUIRE(A && Wt, "gemm: null operand");
   CUtensorMap tmA, tmB;
-  const int bn = epi_uses_tma_store(epilogue) ? gemm_tile_n(N) : 128;   // row-remapping epilogues: 128-wide only
+  const int bn = epi_uses_tma_store(epilogue) ? gemm_tile_n() : 128;   // row-remapping epilogues: 128-wide only
   if ((rc = make_tmap_f16(&tmA, A, M, K, BM))) return rc;
   if ((rc = make_tmap_f16(&tmB, Wt, N, K, bn / 2))) return rc;   // each CTA of a pair loads (and multicasts) half a tile
   CUtensorMap tmC;
@@ -851,4 +1109,60 @@ extern "C" int dss_debug_gemm_cfg(const void* A, const void* Wt, const float* bi
   }
   set_error("debug_gemm_cfg: unsupported (bn=%d, stages=%d)", bn, stages);
   return DSS_ERR_BAD_ARG;
+}
+
+namespace dss {
+template <int EPI, bool TRACE>
+static int launch_schedule(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap& tmC, int M, int N, int K,
+                           const EpiParams& p, cudaStream_t st, int schedule, int bn) {
+  return schedule ? launch_pp<EPI, TRACE>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, bn)
+                  : launch_tc<EPI, TRACE>(tmA, tmB, &tmC, M, N, K, p, st, KC_GEMM_OTHER, bn);
+}
+
+// One of the four TMA-store epilogues under either schedule (0 = cooperative at coop_tile_n(N), 1 = ping-pong), traced
+// when `trace` is not null (trace_bytes must hold trace_stride(items, clusters) words per CTA).
+template <bool TRACE>
+static int debug_gemm_schedule(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K,
+                               int epilogue, int schedule, unsigned long long* trace, size_t trace_bytes,
+                               cudaStream_t st) {
+  int rc = check_gemm_args(M, N, K, epilogue, bias, out, nullptr, 0, 0);
+  if (rc) return rc;
+  DSS_REQUIRE(A && Wt, "gemm: null operand");
+  DSS_REQUIRE(epi_uses_tma_store(epilogue), "debug_gemm_schedule: epilogue %d is not one of the four ViT epilogues", epilogue);
+  DSS_REQUIRE(schedule == 0 || schedule == 1, "debug_gemm_schedule: schedule must be 0 (cooperative) or 1 (ping-pong)");
+  const int bn = schedule ? PP_BN : coop_tile_n(N);
+  if (TRACE) {
+    const int items = cdiv(cdiv(M, BM), 2) * cdiv(N, bn), clusters = gemm_clusters(items);
+    const size_t need = (size_t)(2 * clusters) * trace_stride(items, clusters) * sizeof(unsigned long long);
+    DSS_REQUIRE(trace != nullptr && trace_bytes >= need, "debug_gemm_trace: the trace needs %zu bytes", need);
+    DSS_CHECK_CUDA(cudaMemsetAsync(trace, 0, need, st));
+  }
+  CUtensorMap tmA, tmB, tmC;
+  if ((rc = make_tmap_f16(&tmA, A, M, K, BM))) return rc;
+  if ((rc = make_tmap_f16(&tmB, Wt, N, K, bn / 2))) return rc;
+  const int f32 = (epilogue == DSS_EPI_BIAS_RESID_F32 || epilogue == DSS_EPI_BIAS_F32) ? 1 : 0;
+  if ((rc = make_tmap_out(&tmC, out, M, N, f32))) return rc;
+  EpiParams p{out, bias, nullptr, N, 0, 0, 0, nullptr, nullptr, nullptr, 0.f, 0, 0, 0, nullptr, 0, trace};
+  switch (epilogue) {
+    case DSS_EPI_BIAS_F16: return launch_schedule<DSS_EPI_BIAS_F16, TRACE>(tmA, tmB, tmC, M, N, K, p, st, schedule, bn);
+    case DSS_EPI_BIAS_GELU_F16: return launch_schedule<DSS_EPI_BIAS_GELU_F16, TRACE>(tmA, tmB, tmC, M, N, K, p, st, schedule, bn);
+    case DSS_EPI_BIAS_RESID_F32: return launch_schedule<DSS_EPI_BIAS_RESID_F32, TRACE>(tmA, tmB, tmC, M, N, K, p, st, schedule, bn);
+    case DSS_EPI_BIAS_F32: return launch_schedule<DSS_EPI_BIAS_F32, TRACE>(tmA, tmB, tmC, M, N, K, p, st, schedule, bn);
+  }
+  set_error("debug_gemm_schedule: unknown epilogue %d", epilogue);
+  return DSS_ERR_BAD_ARG;
+}
+}  // namespace dss
+
+extern "C" int dss_debug_gemm_schedule(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K,
+                                       int epilogue, int schedule, dss_stream_t stream) {
+  return debug_gemm_schedule<false>(A, Wt, bias, out, M, N, K, epilogue, schedule, nullptr, 0,
+                                    static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int dss_debug_gemm_trace(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K,
+                                    int epilogue, int schedule, unsigned long long* trace, size_t trace_bytes,
+                                    dss_stream_t stream) {
+  return debug_gemm_schedule<true>(A, Wt, bias, out, M, N, K, epilogue, schedule, trace, trace_bytes,
+                                   static_cast<cudaStream_t>(stream));
 }

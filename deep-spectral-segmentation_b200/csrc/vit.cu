@@ -20,7 +20,7 @@
 namespace dss {
 
 int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_rows);
-int gemm_tile_n(int N);
+int gemm_tile_n();
 int make_tmap_out(CUtensorMap* tm, const void* ptr, int rows, int cols, int is_f32);
 int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, const float* bias, void* out,
                 int M, int N, int K, int epi, const float* aux, int rin, int rout, cudaStream_t st, int kclass, int bn);
@@ -248,12 +248,12 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
     } else {
       if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
       if ((rc = gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, w.qkv, M, 3 * d, d, DSS_EPI_BIAS_F16, nullptr, 0, 0, st,
-                            KC_GEMM_QKV, gemm_tile_n(3 * d))))
+                            KC_GEMM_QKV, gemm_tile_n())))
         return rc;
     }
     if ((rc = launch_attention_tc(w.qkv, w.attn, B, T, c.heads, st))) return rc;
     if ((rc = gemm_f16_tc(tm_attn, bw.tm_proj, &tm_x_out, bw.proj_b, w.x, M, d, d, DSS_EPI_BIAS_RESID_F32, nullptr, 0, 0, st,
-                          KC_GEMM_PROJ, gemm_tile_n(d))))
+                          KC_GEMM_PROJ, gemm_tile_n())))
       return rc;
     if (fused_ln) {
       if ((rc = gemm_ln_f16_tc(bw.tm_fc1_ln, tm_hid_out, w.x, bw.ln2_w, bw.ln2_b, bw.fc1_b, M, c.mlp_ratio * d, c.ln_eps, true,
@@ -262,11 +262,11 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
     } else {
       if ((rc = launch_layernorm(w.x, bw.ln2_w, bw.ln2_b, w.xn, M, d, c.ln_eps, st))) return rc;
       if ((rc = gemm_f16_tc(tm_xn, bw.tm_fc1, &tm_hid_out, bw.fc1_b, w.hid, M, c.mlp_ratio * d, d, DSS_EPI_BIAS_GELU_F16,
-                            nullptr, 0, 0, st, KC_GEMM_FC1, gemm_tile_n(c.mlp_ratio * d))))
+                            nullptr, 0, 0, st, KC_GEMM_FC1, gemm_tile_n())))
         return rc;
     }
     if ((rc = gemm_f16_tc(tm_hid, bw.tm_fc2, &tm_x_out, bw.fc2_b, w.x, M, d, c.mlp_ratio * d, DSS_EPI_BIAS_RESID_F32, nullptr, 0,
-                          0, st, KC_GEMM_FC2, gemm_tile_n(d))))
+                          0, st, KC_GEMM_FC2, gemm_tile_n())))
       return rc;
   }
   if (k_proj) {
@@ -391,11 +391,11 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     b.ln2_w = reinterpret_cast<float*>(base + bo[l].ln2_w); b.ln2_b = reinterpret_cast<float*>(base + bo[l].ln2_b);
     b.qkv_b = reinterpret_cast<float*>(base + bo[l].qkv_b); b.proj_b = reinterpret_cast<float*>(base + bo[l].proj_b);
     b.fc1_b = reinterpret_cast<float*>(base + bo[l].fc1_b); b.fc2_b = reinterpret_cast<float*>(base + bo[l].fc2_b);
-    if ((rc = make_tmap_f16(&b.tm_qkv, b.qkv_w, (int)(3 * d), (int)d, gemm_tile_n((int)(3 * d)) / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_qkv, b.qkv_w, (int)(3 * d), (int)d, gemm_tile_n() / 2))) return rc;
     if ((rc = make_tmap_f16(&b.tm_k, b.qkv_w + d * d, (int)d, (int)d, 128 / 2))) return rc;
-    if ((rc = make_tmap_f16(&b.tm_proj, b.proj_w, (int)d, (int)d, gemm_tile_n((int)d) / 2))) return rc;
-    if ((rc = make_tmap_f16(&b.tm_fc1, b.fc1_w, (int)hid, (int)d, gemm_tile_n((int)hid) / 2))) return rc;
-    if ((rc = make_tmap_f16(&b.tm_fc2, b.fc2_w, (int)d, (int)hid, gemm_tile_n((int)d) / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_proj, b.proj_w, (int)d, (int)d, gemm_tile_n() / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_fc1, b.fc1_w, (int)hid, (int)d, gemm_tile_n() / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_fc2, b.fc2_w, (int)d, (int)hid, gemm_tile_n() / 2))) return rc;
     if (d == 384) {
       if ((rc = make_tmap_f16(&b.tm_qkv_ln, b.qkv_w, (int)(3 * d), (int)d, gemm_ln_tile_n((int)(3 * d)) / 2))) return rc;
       if ((rc = make_tmap_f16(&b.tm_fc1_ln, b.fc1_w, (int)hid, (int)d, gemm_ln_tile_n((int)hid) / 2))) return rc;

@@ -137,6 +137,20 @@ int dss_op_gemm_f16_simt(const void* A, const void* Wt, const float* bias, void*
  * (stages is ignored: the ring depth follows from the shared-memory budget of bn). Not used by the product path. */
 int dss_debug_gemm_cfg(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K, int bn,
                        int stages, dss_stream_t stream);
+/* Debug: dss_op_gemm_f16 with one of the four TMA-store epilogues (BIAS_F16, BIAS_GELU_F16, BIAS_RESID_F32, BIAS_F32)
+ * under either GEMM schedule, on the same inputs. schedule 0 = cooperative (both MMA warp groups on one 128 x BN tile,
+ * BN the widest of 256 / 192 / 128 dividing N); 1 = ping-pong (each MMA warp group owns 128 x 128 tiles, the groups
+ * alternate on the tensor cores; what dss_op_gemm_f16 runs for these epilogues). Not used by the product path. */
+int dss_debug_gemm_schedule(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K,
+                            int epilogue, int schedule, dss_stream_t stream);
+/* Same, with a phase trace (a separately compiled kernel variant): trace (device) receives, per CTA c of the
+ * persistent launch (2 * clusters CTAs, clusters = min(items, SMs / 2), items = ceil(ceil(M / 128) / 2) * ceil(N / BN)),
+ * S = 4 + 8 * ceil(items / clusters) words at c * S: [0] = ns the TMA producer waited on empty ring slots, then for
+ * consumer warp group w and its j-th tile, at 4 + 4 * (w * ceil(items / clusters) + j), the %globaltimer stamps
+ * {tile start, first operand slab arrived, last wgmma retired, epilogue issued}; records of tiles not run stay 0.
+ * trace_bytes smaller than needed is rejected (DSS_ERR_BAD_ARG, the message names the size). */
+int dss_debug_gemm_trace(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K, int epilogue,
+                         int schedule, unsigned long long* trace, size_t trace_bytes, dss_stream_t stream);
 /* LayerNorm fused into the GEMM's A-operand producer (the qkv / fc1 layers of ViT-S; K must be 384):
  * out f16 [M, N] = (gelu ? gelu_erf : id)(LayerNorm(x f32 [M, K]; gamma, beta, eps) @ Wt f16 [N, K]^T + bias); N % 128 == 0 */
 int dss_op_gemm_ln_f16(const float* x, const float* gamma, const float* beta, const void* Wt, const float* bias,
