@@ -5,8 +5,10 @@
 // feature x is split as x = hi + lo with hi = fp16(x), lo = x - hi (|lo| <= 2^-12 |x|) and
 //     x.y ~= hi.hi' + (hi/64).(64 lo') + (64 lo).(hi'/64)              (lo.lo' ~ 2^-24 is dropped)
 // i.e. ONE fp16 GEMM with K = 3d over S = [hi | hi/64 | 64 lo] against the same array with the last two groups of
-// K slabs swapped. The 2^+-6 factors keep every operand inside the fp16 normal range. Measured error of the split
-// against a float64 product: 7e-8, smaller than a plain fp32 product's 1e-6 (DESIGN.md section 3).
+// K slabs swapped. The 2^+-6 factors keep every operand inside the fp16 normal range. The split itself is exact to
+// ~2^-22 per product; the error that remains comes from the wgmma fp32 accumulation over 3 d / 16 k-steps. Measured
+// max |W - W_float64| on an H100 80GB HBM3 at 400 W (normalised rows, d = 384): 5e-6, three times a plain fp32 product's 1.6e-6
+// (d = 768: 9e-6 against 1e-6); DESIGN.md section 3, tests/test_affinity_exact_gpu.py.
 // The GEMM itself is gemm.cu's TMA/wgmma kernel in batched mode with the affinity epilogue (relu, /max,
 // + lambda*counts, zero padding of the row pitch) fused.
 #include "common.cuh"
@@ -15,8 +17,8 @@ namespace dss {
 
 int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_rows);
 int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int images, int Nimg, int d, float* Wout, int ldw,
-                     const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts, float lambda,
-                     int threshold, float* deg_part, int ld_part, cudaStream_t st);
+                     int ncols, const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts,
+                     float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st);
 
 // per-image max |f| (only needed when the features are NOT normalised: they are pre-scaled by a power of two so
 // that fp16 cannot overflow; the scale cancels in W / max(W))
@@ -177,8 +179,14 @@ extern "C" int dss_affinity(const float* feats, int B, int N, int d, int flags, 
   float* deg_out = degree ? degree
                           : reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(deg_part) + degpart_bytes(B, N));
   const int tiles = (N + 127) / 128, ld_part = tiles * 128;
-  if ((rc = affinity_gemm_tc(tmS, tmS_half, B, N, dpad, Wmat, ldw, img_max, normalize ? nullptr : img_absmax, color_counts,
-                             color_lambda,
+  // The GEMM covers the columns of the image's 128-wide tiles (fewer if the pitch ends sooner): the degree partial
+  // slots are laid out by those tiles in the epilogue and in degree_reduce_kernel alike. A wider pitch is zeroed here.
+  const int ncols = ldw < ld_part ? ldw : ld_part;
+  if (ldw > ncols)
+    DSS_CHECK_CUDA(cudaMemset2DAsync(Wmat + ncols, (size_t)ldw * sizeof(float), 0, (size_t)(ldw - ncols) * sizeof(float),
+                                     (size_t)B * N, st));
+  if ((rc = affinity_gemm_tc(tmS, tmS_half, B, N, dpad, Wmat, ldw, ncols, img_max, normalize ? nullptr : img_absmax,
+                             color_counts, color_lambda,
                              ((flags & DSS_AFF_THRESHOLD_AT_ZERO) ? 1 : 0) | ((flags & DSS_AFF_NO_MAX_SCALE) ? 2 : 0),
                              deg_part, ld_part, st)))
     return rc;

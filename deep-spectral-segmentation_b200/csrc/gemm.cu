@@ -1023,18 +1023,21 @@ int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
 }
 
 // Batched Gram product for the affinity build: per image z, W[z] = epilogue(S[z] S'[z]^T) with S = split-fp16 rows
-// [images*Nimg, 3d] (see affinity.cu). N output columns cover the padded pitch ldw.
+// [images*Nimg, 3d] (see affinity.cu). The GEMM's ncols output columns (Nimg <= ncols <= ldw) are the first ncols of
+// the row pitch ldw; they also set the column tiles, and with them the layout of the degree partial slots
+// [images, 8 * cdiv(ncols, 128), ld_part] that degree_reduce_kernel reads back.
 int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int images, int Nimg, int d, float* Wout, int ldw,
-                     const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts, float lambda,
-                     int threshold, float* deg_part, int ld_part, cudaStream_t st) {
+                     int ncols, const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts,
+                     float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st) {
   EpiParams p{Wout, nullptr, nullptr, ldw, 0, 0, Nimg, img_max, img_absmax, counts, lambda, threshold, d / BK,
               1, deg_part, ld_part};
   DSS_REQUIRE(d % BK == 0, "affinity: feature dim must be a multiple of %d for the tensor-core path (got %d)", BK, d);
-  DSS_REQUIRE(deg_part != nullptr && ld_part >= cdiv(ldw, 128) * 128, "affinity: bad degree partial buffer");
+  DSS_REQUIRE(ncols >= Nimg && ncols <= ldw, "affinity: bad GEMM column count %d (N=%d ldw=%d)", ncols, Nimg, ldw);
+  DSS_REQUIRE(deg_part != nullptr && ld_part >= cdiv(ncols, 128) * 128, "affinity: bad degree partial buffer");
   CUtensorMap tmW;
   int rc = make_tmap_out3d_f32(&tmW, Wout, images, Nimg, ldw);
   if (rc) return rc;
-  return launch_tc<EPI_AFFINITY_F32>(tmS, tmS_half, &tmW, Nimg, ldw, 3 * d, p, st, KC_AFFINITY, 128, images);
+  return launch_tc<EPI_AFFINITY_F32>(tmS, tmS_half, &tmW, Nimg, ncols, 3 * d, p, st, KC_AFFINITY, 128, images);
 }
 
 template <int EPI>

@@ -101,7 +101,9 @@ def test_affinity_matches_reference_arithmetic(cuda):
         W = spectral.affinity(feats[None].to(cuda))[0].cpu().numpy()
         W_ref, _ = eigs_ref.affinity_matrices(feats)
         assert W.shape == (N, spectral.pitch(N))
-        assert np.abs(W[:, :N] - W_ref).max() <= 1e-5   # tensor-core fp32 accumulation truncates: ~4e-6 at K=3d
+        # the wgmma fp32 accumulation over K = 3d: measured 5e-6 (d = 384, H100 at 400 W) against float64, where the
+        # fp32 product is off by 0.5e-6..1.6e-6 (DESIGN.md section 3)
+        assert np.abs(W[:, :N] - W_ref).max() <= 1e-5
         assert np.all(W[:, N:] == 0)
         assert W[:, :N].max() <= 1.0 + 1e-6 and W.min() >= 0.0
 
