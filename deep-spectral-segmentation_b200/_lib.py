@@ -96,12 +96,25 @@ PROTOTYPES = {
     "dss_lattice_filter_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "dss_op_lattice_filter": (c_int, [c_void_p, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                       c_size_t, c_void_p]),
+    "dss_eigseg_boxes_workspace_bytes": (c_size_t, [c_int]),
+    "dss_eigseg_boxes": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p, c_size_t,
+                                 c_void_p]),
+    "dss_lost_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "dss_lost_boxes": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
+                               c_void_p, c_void_p, c_size_t, c_void_p]),
+    "dss_dinoseg_boxes": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "dss_vit_forward_last_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int, c_int]),
+    "dss_vit_forward_last": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                     c_size_t, c_void_p]),
+    "dss_op_cls_attention": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "dss_op_im2col_pad_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "dss_upsample_bilinear": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "dss_normalize_rows": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
 }
 
 EPI_BIAS_F16, EPI_BIAS_GELU_F16, EPI_BIAS_RESID_F32, EPI_BIAS_F32, EPI_PATCH_F32, EPI_DROPCLS_F32 = range(6)
 AFF_NORMALIZE, AFF_THRESHOLD_AT_ZERO, AFF_NO_MAX_SCALE = 1, 2, 4
+LOC_OK, LOC_NO_GRID, LOC_SEED_IN_BACKGROUND, LOC_EMPTY_COMPONENT = range(4)
 
 _lib = None
 

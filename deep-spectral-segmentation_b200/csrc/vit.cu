@@ -25,6 +25,8 @@ int make_tmap_out(CUtensorMap* tm, const void* ptr, int rows, int cols, int is_f
 int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, const float* bias, void* out,
                 int M, int N, int K, int epi, const float* aux, int rin, int rout, cudaStream_t st, int kclass, int bn);
 int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
+int launch_im2col_pad(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
+int launch_cls_attention(const void* qkv, int B, int T, int heads, float* out, cudaStream_t st);
 int launch_cls_row(float* x, const float* cls, const float* pos, int B, int T, int d, cudaStream_t st);
 int launch_layernorm(const float* x, const float* g, const float* b, void* y, int M, int d, float eps, cudaStream_t st);
 int launch_attention_tc(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st);
@@ -57,6 +59,7 @@ struct BlockW {
   float *ln1_w, *ln1_b, *ln2_w, *ln2_b, *qkv_b, *proj_b, *fc1_b, *fc2_b;
   __half *qkv_w, *proj_w, *fc1_w, *fc2_w;
   CUtensorMap tm_qkv, tm_k, tm_proj, tm_fc1, tm_fc2;
+  CUtensorMap tm_q, tm_v;             // q and v thirds of the qkv weight (localization features)
   CUtensorMap tm_qkv_ln, tm_fc1_ln;   // weight maps of the LayerNorm-fused kernel (its own tile width)
 };
 
@@ -173,8 +176,8 @@ struct VitWs {
   size_t total;
 };
 
-static VitWs carve(const dss_vit_config& c, int B, int H, int W, void* base) {
-  const int Np = (H / c.patch) * (W / c.patch), T = Np + 1, d = c.dim;
+static VitWs carve(const dss_vit_config& c, int B, int Hp, int Wp, void* base) {
+  const int Np = Hp * Wp, T = Np + 1, d = c.dim;
   const size_t M = (size_t)B * T;
   uint8_t* p = reinterpret_cast<uint8_t*>(base);
   size_t off = 0;
@@ -194,19 +197,21 @@ static VitWs carve(const dss_vit_config& c, int B, int H, int W, void* base) {
   return w;
 }
 
-// mode 0: K projection of block n_full (features), 1: residual stream [B, T, d], 2: final-norm CLS token [B, d]
+// mode 0: K projection of block n_full (features), 1: residual stream [B, T, d], 2: final-norm CLS token [B, d],
+// 3: block n_full's `which` projection third (out, may be NULL) and CLS attention row (cls_attn, may be NULL).
+// pad: zero-padded ceil grid instead of the crop.
 static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_full, int mode, float* out, void* ws,
-                   size_t ws_bytes, cudaStream_t st) {
+                   size_t ws_bytes, cudaStream_t st, int pad = 0, int which = 1, float* cls_attn = nullptr) {
   const bool k_proj = mode == 0;
   DSS_REQUIRE(h && h->loaded, "vit: weights not loaded");
-  DSS_REQUIRE(img && out && ws, "vit: null pointer");
+  DSS_REQUIRE(img && (out || cls_attn) && ws, "vit: null pointer");
   const dss_vit_config& c = h->cfg;
   const int P = c.patch, d = c.dim;
-  const int Hp = H / P, Wp = W / P;
+  const int Hp = pad ? cdiv(H, P) : H / P, Wp = pad ? cdiv(W, P) : W / P;
   DSS_REQUIRE(B > 0 && Hp > 0 && Wp > 0, "vit: image %dx%d smaller than one %d-pixel patch", H, W, P);
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "vit: workspace must be 256-byte aligned");
   const int Np = Hp * Wp, T = Np + 1, M = B * T;
-  VitWs w = carve(c, B, H, W, ws);
+  VitWs w = carve(c, B, Hp, Wp, ws);
   if (ws_bytes < w.total) {
     set_error("vit: workspace too small (%zu < %zu)", ws_bytes, w.total);
     return DSS_ERR_WORKSPACE;
@@ -228,7 +233,8 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   if ((rc = make_tmap_out(&tm_hid_out, w.hid, M, c.mlp_ratio * d, 0))) return rc;
 
   // tokens: x[b, 1+n, :] = patch_embed + pos ; x[b, 0, :] = cls + pos[0]
-  if ((rc = launch_im2col(img, w.patches, B, H, W, P, st))) return rc;
+  if ((rc = pad ? launch_im2col_pad(img, w.patches, B, H, W, P, st) : launch_im2col(img, w.patches, B, H, W, P, st)))
+    return rc;
   if ((rc = gemm_f16_tc(tm_patches, h->tm_patch, nullptr, h->patch_b, w.x, B * Np, d, Kp, DSS_EPI_PATCH_F32, pos, Np, T, st,
                         KC_GEMM_PATCH, 128)))
     return rc;
@@ -276,6 +282,21 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
     if ((rc = gemm_f16_tc(tm_xn, bw.tm_k, nullptr, bw.qkv_b + d, out, M, d, d, DSS_EPI_DROPCLS_F32, nullptr, T, Np, st,
                           KC_GEMM_KPROJ, 128)))
       return rc;
+  } else if (mode == 3) {
+    const BlockW& bw = h->blocks[n_full];
+    if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
+    if (out) {   // qkv[b, 1+n, which*d : (which+1)*d] in fp32, as dss_vit_forward_k writes the K third
+      const CUtensorMap& tm = which == 0 ? bw.tm_q : (which == 1 ? bw.tm_k : bw.tm_v);
+      if ((rc = gemm_f16_tc(tm_xn, tm, nullptr, bw.qkv_b + (size_t)which * d, out, M, d, d, DSS_EPI_DROPCLS_F32, nullptr, T,
+                            Np, st, KC_GEMM_KPROJ, 128)))
+        return rc;
+    }
+    if (cls_attn) {   // the full qkv projection the attention kernels read, then the CLS row of the softmax
+      if ((rc = gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, w.qkv, M, 3 * d, d, DSS_EPI_BIAS_F16, nullptr, 0, 0, st,
+                            KC_GEMM_QKV, gemm_tile_n())))
+        return rc;
+      if ((rc = launch_cls_attention(w.qkv, B, T, c.heads, cls_attn, st))) return rc;
+    }
   } else if (mode == 2) {
     // upstream VisionTransformer.forward: x = norm(x); return x[:, 0]  (LayerNorm is row-wise: only the CLS rows)
     DSS_REQUIRE(h->norm_w && h->norm_b, "vit: the final LayerNorm weights (norm.weight / norm.bias) were not loaded");
@@ -393,6 +414,8 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     b.fc1_b = reinterpret_cast<float*>(base + bo[l].fc1_b); b.fc2_b = reinterpret_cast<float*>(base + bo[l].fc2_b);
     if ((rc = make_tmap_f16(&b.tm_qkv, b.qkv_w, (int)(3 * d), (int)d, gemm_tile_n() / 2))) return rc;
     if ((rc = make_tmap_f16(&b.tm_k, b.qkv_w + d * d, (int)d, (int)d, 128 / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_q, b.qkv_w, (int)d, (int)d, 128 / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_v, b.qkv_w + 2 * d * d, (int)d, (int)d, 128 / 2))) return rc;
     if ((rc = make_tmap_f16(&b.tm_proj, b.proj_w, (int)d, (int)d, gemm_tile_n() / 2))) return rc;
     if ((rc = make_tmap_f16(&b.tm_fc1, b.fc1_w, (int)hid, (int)d, gemm_tile_n() / 2))) return rc;
     if ((rc = make_tmap_f16(&b.tm_fc2, b.fc2_w, (int)d, (int)hid, gemm_tile_n() / 2))) return rc;
@@ -416,7 +439,25 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
 
 extern "C" size_t dss_vit_workspace_bytes(const dss_vit_t* h, int B, int H, int W) {
   if (!h || B <= 0 || H < h->cfg.patch || W < h->cfg.patch) return 0;
-  return carve(h->cfg, B, H, W, nullptr).total;
+  return carve(h->cfg, B, H / h->cfg.patch, W / h->cfg.patch, nullptr).total;
+}
+
+extern "C" size_t dss_vit_forward_last_workspace_bytes(const dss_vit_t* h, int B, int H, int W, int pad) {
+  if (!h || B <= 0 || H <= 0 || W <= 0) return 0;
+  const int P = h->cfg.patch;
+  if (!pad) return dss_vit_workspace_bytes(h, B, H, W);
+  return carve(h->cfg, B, cdiv(H, P), cdiv(W, P), nullptr).total;
+}
+
+extern "C" int dss_vit_forward_last(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, int pad, int which,
+                                    float* feats_out, float* cls_attn_out, void* ws, size_t ws_bytes,
+                                    dss_stream_t stream) {
+  DSS_REQUIRE(h, "vit_forward_last: null handle");
+  DSS_REQUIRE(which >= 0 && which <= 2, "vit_forward_last: which must be 0 (q), 1 (k) or 2 (v), got %d", which);
+  DSS_REQUIRE(feats_out || cls_attn_out, "vit_forward_last: null pointer (no output requested)");
+  DSS_REQUIRE(B > 0 && H > 0 && W > 0, "vit_forward_last: empty image batch");
+  return vit_run(h, images_u8, B, H, W, h->cfg.depth - 1, 3, feats_out, ws, ws_bytes, static_cast<cudaStream_t>(stream),
+                 pad, which, cls_attn_out);
 }
 
 extern "C" int dss_vit_forward_k(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, int which_block,

@@ -300,6 +300,102 @@ int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P,
   return DSS_OK;
 }
 
+// Zero-padded variant (object-localization/main.py:227-235 pads the normalised image with zeros up to multiples of
+// P): the grid is ceil(H/P) x ceil(W/P); a pixel outside the image is 0. One thread = 8 pixels of one patch row.
+__global__ void im2col_pad_f16_kernel(const uint8_t* __restrict__ img, __half* __restrict__ out, int B, int H, int W,
+                                      int P, int Hp, int Wp) {
+  const int groups_per_row = P / 8;
+  const long long total = (long long)B * Hp * Wp * P * groups_per_row;
+  const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (gid >= total) return;
+  const int g = (int)(gid % groups_per_row);
+  const int pw = (int)((gid / groups_per_row) % Wp);
+  const int py = (int)((gid / ((long long)groups_per_row * Wp)) % P);
+  const int ph = (int)((gid / ((long long)groups_per_row * Wp * P)) % Hp);
+  const int b = (int)(gid / ((long long)groups_per_row * Wp * P * Hp));
+  const int y = ph * P + py, x0 = pw * P + g * 8;
+  const long long patch = ((long long)b * Hp + ph) * Wp + pw;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    const float mean = c_mean[c], sd = c_std[c];
+    float v[8];
+#pragma unroll
+    for (int t = 0; t < 8; ++t) {
+      const int x = x0 + t;
+      v[t] = (y < H && x < W) ? (static_cast<float>(__ldg(img + (((long long)b * H + y) * W + x) * 3 + c)) / 255.0f - mean) / sd
+                              : 0.f;
+    }
+    uint4 q;
+    q.x = pack_half2(v[0], v[1]);
+    q.y = pack_half2(v[2], v[3]);
+    q.z = pack_half2(v[4], v[5]);
+    q.w = pack_half2(v[6], v[7]);
+    *reinterpret_cast<uint4*>(out + patch * (3LL * P * P) + (c * P + py) * P + g * 8) = q;
+  }
+}
+
+int launch_im2col_pad(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st) {
+  DSS_REQUIRE(P % 8 == 0 && P > 0, "im2col_pad: patch must be a multiple of 8 (got %d)", P);
+  DSS_REQUIRE(B > 0 && H > 0 && W > 0, "im2col_pad: empty image batch");
+  const int Hp = cdiv(H, P), Wp = cdiv(W, P);
+  const long long total = (long long)B * Hp * Wp * P * (P / 8);
+  const int threads = 256;
+  LaunchScope scope(st, KC_IM2COL);
+  im2col_pad_f16_kernel<<<(unsigned)((total + threads - 1) / threads), threads, 0, st>>>(
+      img, reinterpret_cast<__half*>(patches), B, H, W, P, Hp, Wp);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
+// CLS row of the last block's attention (get_last_selfattention(...)[:, :, 0, 1:], the input of dino_seg):
+// s_j = (q_0 . k_j) / 8 over all T tokens, softmax in fp32. One CTA per (head, image); the 64-term dot products are
+// recomputed in each of the three passes (max, sum, output) rather than kept in scratch memory.
+constexpr int CLSATT_THREADS = 256;
+__device__ __forceinline__ float cls_score(const float* q0, const __half* k) {
+  float acc = 0.f;
+#pragma unroll 8
+  for (int i = 0; i < 64; ++i) acc = fmaf(q0[i], __half2float(k[i]), acc);
+  return acc * 0.125f;
+}
+__device__ __forceinline__ float cls_block_reduce(float v, float* red, bool is_max) {
+  v = is_max ? warp_max(v) : warp_sum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x < 32) {
+    float t = threadIdx.x < CLSATT_THREADS / 32 ? red[threadIdx.x] : (is_max ? -INFINITY : 0.f);
+    t = is_max ? warp_max(t) : warp_sum(t);
+    if (threadIdx.x == 0) red[CLSATT_THREADS / 32] = t;
+  }
+  __syncthreads();
+  return red[CLSATT_THREADS / 32];
+}
+__global__ void __launch_bounds__(CLSATT_THREADS)
+cls_attention_kernel(const __half* __restrict__ qkv, int T, int heads, float* __restrict__ out) {
+  __shared__ float q0[64];
+  __shared__ float red[CLSATT_THREADS / 32 + 1];
+  const int h = blockIdx.x, b = blockIdx.y, d = heads * 64, tid = threadIdx.x;
+  const __half* base = qkv + (long long)b * T * 3 * d;
+  const __half* kbase = base + d + h * 64;
+  if (tid < 64) q0[tid] = __half2float(base[h * 64 + tid]);
+  __syncthreads();
+  float mx = -INFINITY;
+  for (int j = tid; j < T; j += CLSATT_THREADS) mx = fmaxf(mx, cls_score(q0, kbase + (long long)j * 3 * d));
+  mx = cls_block_reduce(mx, red, true);
+  float sum = 0.f;
+  for (int j = tid; j < T; j += CLSATT_THREADS) sum += expf(cls_score(q0, kbase + (long long)j * 3 * d) - mx);
+  sum = cls_block_reduce(sum, red, false);
+  float* o = out + ((long long)b * heads + h) * (T - 1);
+  for (int j = tid + 1; j < T; j += CLSATT_THREADS) o[j - 1] = expf(cls_score(q0, kbase + (long long)j * 3 * d) - mx) / sum;
+}
+
+int launch_cls_attention(const void* qkv, int B, int T, int heads, float* out, cudaStream_t st) {
+  DSS_REQUIRE(B > 0 && T >= 2 && heads > 0, "cls_attention: bad shape (B=%d T=%d heads=%d)", B, T, heads);
+  LaunchScope scope(st, KC_ATTENTION);
+  cls_attention_kernel<<<dim3(heads, B), CLSATT_THREADS, 0, st>>>(reinterpret_cast<const __half*>(qkv), T, heads, out);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
 int launch_cls_row(float* x, const float* cls, const float* pos, int B, int T, int d, cudaStream_t st) {
   LaunchScope scope(st, KC_CLS_ROW);
   cls_row_kernel<<<cdiv(B * d, 256), 256, 0, st>>>(x, cls, pos, B, T, d);
@@ -346,4 +442,14 @@ extern "C" int dss_op_attention_f16(const void* qkv, void* out, int B, int T, in
 extern "C" int dss_op_im2col_f16(const uint8_t* images_u8, void* patches, int B, int H, int W, int P,
                                  dss_stream_t stream) {
   return launch_im2col(images_u8, patches, B, H, W, P, static_cast<cudaStream_t>(stream));
+}
+extern "C" int dss_op_im2col_pad_f16(const uint8_t* images_u8, void* patches, int B, int H, int W, int P,
+                                     dss_stream_t stream) {
+  DSS_REQUIRE(images_u8 && patches, "im2col_pad: null pointer");
+  return launch_im2col_pad(images_u8, patches, B, H, W, P, static_cast<cudaStream_t>(stream));
+}
+extern "C" int dss_op_cls_attention(const void* qkv, int B, int T, int heads, float* cls_attn, dss_stream_t stream) {
+  DSS_REQUIRE(qkv && cls_attn, "cls_attention: null pointer");
+  DSS_REQUIRE(B > 0 && T >= 2 && heads > 0, "cls_attention: bad shape (B=%d T=%d heads=%d)", B, T, heads);
+  return launch_cls_attention(qkv, B, T, heads, cls_attn, static_cast<cudaStream_t>(stream));
 }

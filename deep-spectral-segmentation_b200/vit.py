@@ -171,6 +171,33 @@ class DinoViT:
 
     __call__ = forward_cls
 
+    @torch.no_grad()
+    def forward_last(self, images_u8: torch.Tensor, which: str = "k", pad: bool = True, feats: bool = True,
+                     cls_attn: bool = False):
+        """Last-block outputs for object localization (object-localization/main.py:219-322). pad=True zero-pads the
+        normalised image to multiples of the patch size (the grid is ceil(H/P) x ceil(W/P)); pad=False crops.
+        Returns (features [B, N, d] fp32 -- the q, k or v third of the last qkv projection, CLS row dropped -- or None,
+        CLS attention [B, heads, N] fp32 -- get_last_selfattention(...)[:, :, 0, 1:] -- or None)."""
+        img = self._check_images(images_u8)
+        B, H, W, _ = img.shape
+        P = self.patch_size
+        N = (-(-H // P)) * (-(-W // P)) if pad else (H // P) * (W // P)
+        w = {"q": 0, "k": 1, "v": 2}.get(which)
+        if w is None:
+            raise ValueError(f"which must be 'q', 'k' or 'v' (got {which!r})")
+        with torch.cuda.device(self.device):
+            need = int(self.lib.dss_vit_forward_last_workspace_bytes(self._h, B, H, W, 1 if pad else 0))
+            if need == 0:
+                raise _lib.DssError(f"image {H}x{W} is smaller than one patch")
+            if self._ws is None or self._ws.numel() < need:
+                self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+            f = torch.empty(B, N, self.dim, dtype=torch.float32, device=self.device) if feats else None
+            a = torch.empty(B, self.num_heads, N, dtype=torch.float32, device=self.device) if cls_attn else None
+            _lib.check(self.lib.dss_vit_forward_last(self._h, img.data_ptr(), B, H, W, 1 if pad else 0, w, _lib.ptr(f),
+                                                     _lib.ptr(a), self._ws.data_ptr(), self._ws.numel(),
+                                                     _lib.stream_ptr(self.device)), "dss_vit_forward_last")
+        return f, a
+
     def pos_embed(self, Hp: int, Wp: int) -> torch.Tensor:
         with torch.cuda.device(self.device):
             out = torch.empty(Hp * Wp + 1, self.dim, dtype=torch.float32, device=self.device)

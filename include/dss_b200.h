@@ -330,6 +330,63 @@ size_t dss_lattice_filter_workspace_bytes(int N, int d, int C);
 int dss_op_lattice_filter(const float* features, int N, int d, const float* values, int C, int normalize, float* out,
                           int* lattice_points, void* ws, size_t ws_bytes, dss_stream_t stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Object localization (replaces object-localization/object_discovery.py of the reference: get_bbox_from_patch_mask,
+ * lost / patch_scoring / detect_box, dino_seg, and the ViT hooks of object-localization/main.py:219-322)
+ * ------------------------------------------------------------------------------------------------------------ */
+/* Per-image outcomes written to status [B] int32 (device) by the box kernels; the box of a failed image is 0. */
+enum { DSS_LOC_OK = 0, DSS_LOC_NO_GRID = 1, DSS_LOC_SEED_IN_BACKGROUND = 2, DSS_LOC_EMPTY_COMPONENT = 3 };
+
+/* The box kernels hold one patch grid of at most 16384 cells (128 x 128) per CTA in shared memory and label it with
+ * one union-find whose component roots are their smallest raster index -- the numbering of scipy.ndimage.label and
+ * skimage.measure.label. Larger grids are rejected with DSS_ERR_UNSUPPORTED. Boxes [B, 4] int32 = {xmin, ymin, xmax,
+ * ymax} in pixels, the max exclusive.
+ *
+ * Eigen-segmentation (get_bbox_from_patch_mask + get_largest_cc_box): row `which` of evecs [B, K, N] fp32; dims_host
+ * [B, 2] = the un-cropped image size {H, W} (host). The grid is the first of (H/8, W/8) P 8, (H/16, W/16) P 16,
+ * (2 (H/16), 2 (W/16)) P 8, (4 (H/32), 4 (W/32)) P 8 with N cells (integer division), else status DSS_LOC_NO_GRID.
+ * mask = v > 0, complemented if 0.5 < mean < 1 or empty; the largest 8-connected component (ties: the first in
+ * label order); box {x0 P, y0 P, min((x1 + 1) P, W), min((y1 + 1) P, H)}. */
+size_t dss_eigseg_boxes_workspace_bytes(int B);
+int dss_eigseg_boxes(const float* evecs, int B, int K, int N, int which, const int* dims_host, int* boxes, int* status,
+                     void* ws, size_t ws_bytes, dss_stream_t stream);
+/* LOST on A [B, N, ldw] fp32 = F F^T (dss_affinity with DSS_AFF_NO_MAX_SCALE and no other flag), grid_h x grid_w == N
+ * cells of P pixels, un-padded image H x W (all images of the batch). degree_i = #{j != i : A_ij > 0}; patches in
+ * ascending degree, ties by index (the reference's unstable argsort leaves ties unspecified); seed = the first;
+ * similars = the first min(k_patches, N) with A[seed, p] > 0; M = sum of their rows in that order (fp32); the
+ * 4-connected component of M > 0 holding the seed gives {x0 P, y0 P, min((x1 + 1) P, W), min((y1 + 1) P, H)}.
+ * M[seed] <= 0: status DSS_LOC_SEED_IN_BACKGROUND. seeds [B] int32 (may be NULL) receives the seed patch. */
+size_t dss_lost_workspace_bytes(int B, int N);
+int dss_lost_boxes(const float* A, int B, int N, int ldw, int grid_h, int grid_w, int H, int W, int P, int k_patches,
+                   int* boxes, int* seeds, int* status, void* ws, size_t ws_bytes, dss_stream_t stream);
+/* DINO-seg on the CLS attention cls_attn [B, heads, N] fp32 (dss_vit_forward_last), head < heads: a patch is kept iff
+ * the running sum (fp64 accumulator, each prefix rounded to fp32, as torch's CPU cumsum) of the ascending-sorted
+ * values (ties by index), each divided by their fp32 total, exceeds float(1 - 0.6). 4-connected labels 1 .. n; as in
+ * the reference (which sizes labels 0 .. n-1 only), n >= 2 selects the largest of labels 1 .. n-1 and n <= 1 selects
+ * label 0, the cells not kept (status DSS_LOC_EMPTY_COMPONENT if there are none). Box {x0 P, y0 P, (x1+1) P, (y1+1) P},
+ * not clipped. */
+int dss_dinoseg_boxes(const float* cls_attn, int B, int heads, int N, int head, int grid_h, int grid_w, int P,
+                      int* boxes, int* status, dss_stream_t stream);
+
+/* Last-block ViT outputs for localization. pad != 0 zero-pads the NORMALISED image up to multiples of P
+ * (object-localization/main.py:227-235) and runs on the ceil(H/P) x ceil(W/P) grid; pad == 0 crops like
+ * dss_vit_forward_k. Blocks [0, depth-1) run fully, then the last block's LN1 and:
+ *   feats_out [B, N, d] fp32 (may be NULL): the `which` third of its qkv projection (0 = q, 1 = k, 2 = v), CLS row
+ *     dropped (the qkv hook of main.py:283-322);
+ *   cls_attn_out [B, heads, N] fp32 (may be NULL): softmax(q_0 k_j / 8) over all T = N + 1 tokens, patch entries
+ *     (get_last_selfattention(...)[:, :, 0, 1:]), from the fp16 qkv the attention kernels read.
+ * At least one output is required. Workspace: dss_vit_forward_last_workspace_bytes (0 if the image is smaller than a
+ * patch in crop mode). */
+size_t dss_vit_forward_last_workspace_bytes(const dss_vit_t* h, int B, int H, int W, int pad);
+int dss_vit_forward_last(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, int pad, int which,
+                         float* feats_out, float* cls_attn_out, void* ws, size_t ws_bytes, dss_stream_t stream);
+/* qkv f16 [B, T, 3*d] (heads of 64) -> cls_attn [B, heads, T - 1] fp32 = softmax_j(q_0 . k_j / 8)[1:], fp32
+ * arithmetic, one CTA per (image, head). T >= 2. */
+int dss_op_cls_attention(const void* qkv, int B, int T, int heads, float* cls_attn, dss_stream_t stream);
+/* images_u8 [B,H,W,3] -> patches f16 [B*N, 3*P*P] on the ceil(H/P) x ceil(W/P) grid, pixels outside the image 0
+ * (after normalisation) */
+int dss_op_im2col_pad_f16(const uint8_t* images_u8, void* patches, int B, int H, int W, int P, dss_stream_t stream);
+
 /* Bilinear up-sampling of patch features (align_corners=False, as F.interpolate at extract.py:185-188):
  * feats [B, Hp*Wp, d] fp32 -> out [B, Hl*Wl, d] fp32. Used when image_downsample_factor != patch size. */
 int dss_upsample_bilinear(const float* feats, int B, int Hp, int Wp, int d, int Hl, int Wl, float* out,
