@@ -24,6 +24,7 @@ import types
 import numpy as np
 
 UNARY_EPS = 1e-5
+U32 = 2.0 ** -24          # unit roundoff of fp32
 
 
 # ---------------------------------------------------------------------------------------------------- label upsampling
@@ -45,6 +46,48 @@ def upsample_labels(segmap: np.ndarray, H: int, W: int, P: int) -> np.ndarray:
 # ---------------------------------------------------------------------------------------------------- lattice
 def scales(d: int):
     return [math.sqrt(2.0 / 3.0) * (d + 1) / math.sqrt(float((i + 1) * (i + 2))) for i in range(d)]
+
+
+def key_bits(d: int, flo, fhi, B: int):
+    """Bits of a lattice key as csrc/crf.cu's key_layout sizes them for features f_k in [flo_k, fhi_k] and B images:
+    each coordinate field spans the interval bounds of its elevated coordinate widened by 3(d+1) + 1, the image index
+    takes ceil(log2 B) bits above them. None when one field alone needs more than 62 bits or the bounds are not finite;
+    the library accepts a layout iff this is <= 64. The double arithmetic repeats key_layout's order."""
+    sc = scales(d)
+    flo, fhi = [float(x) for x in flo], [float(x) for x in fhi]
+    if not all(math.isfinite(a) and math.isfinite(b) and a <= b for a, b in zip(flo, fhi)):
+        return None
+    clo = [flo[k] * sc[k] for k in range(d)]
+    chi = [fhi[k] * sc[k] for k in range(d)]
+    total = 0
+    while (1 << total) < B:
+        total += 1
+    for c in range(d):
+        lo = hi = 0.0
+        for k in range(c, d):
+            lo += clo[k]
+            hi += chi[k]
+        if c > 0:
+            lo -= c * chi[c - 1]
+            hi -= c * clo[c - 1]
+        margin = 3.0 * (d + 1) + 1.0
+        if not (abs(lo) < 1e15 and abs(hi) < 1e15):
+            return None
+        span = math.ceil(hi + margin) - math.floor(lo - margin)
+        w = 1
+        while w < 62 and (1 << w) <= span:
+            w += 1
+        if (1 << w) <= span:
+            return None
+        total += w
+    return total
+
+
+def crf_key_bits(H: int, W: int, B: int, alpha: float, beta: float, gamma: float):
+    """(bilateral, spatial) key bits of a dss_crf_segment call on B images of at most H x W pixels."""
+    bil = key_bits(5, [0.0] * 5, [(W - 1) / alpha, (H - 1) / alpha, 255.0 / beta, 255.0 / beta, 255.0 / beta], B)
+    sp = key_bits(2, [0.0] * 2, [(W - 1) / gamma, (H - 1) / gamma], B)
+    return bil, sp
 
 
 def embed(features: np.ndarray):
@@ -149,6 +192,71 @@ class Lattice:
             return self.apply(values)
         n = self.norm()[:, None]
         return n * self.apply(n * np.asarray(values, np.float64))
+
+    def contributions(self) -> np.ndarray:
+        """Number of (point, vertex) slots splatted into every lattice point."""
+        return np.bincount(self.inv.ravel(), minlength=self.points)
+
+    def _fp32_error(self, mag: np.ndarray, rel_in: np.ndarray, rel_out: np.ndarray):
+        """First-order error bound of csrc/crf.cu's fp32 L on splat inputs of magnitude ``mag`` [N, C] that carry a
+        relative error ``rel_in`` [N] (weights included) and an output scaling with relative error ``rel_out`` [N].
+        Returns (bound, magnitude) of alpha * slice(blur(splat)), both [N, C]."""
+        u, d = U32, self.d
+        C = mag.shape[1]
+        slots = self.inv.ravel()
+        order = np.argsort(slots, kind="stable")          # the kernel's contribution order: slot index within a point
+        grp = slots[order]
+        pix = order // (d + 1)
+        t = self.w.ravel()[order, None] * mag[pix]
+        # splat, one fmaf per contribution: every partial sum is rounded once, |error| <= u sum_k |s_k|
+        cum = np.cumsum(t, 0)
+        first = np.searchsorted(grp, np.arange(self.points))
+        base = np.vstack([np.zeros((1, C)), cum])[first][grp]
+        A = np.zeros((self.points, C))
+        E = np.zeros((self.points, C))
+        for c in range(C):
+            A[:, c] = np.bincount(grp, weights=t[:, c], minlength=self.points)
+            E[:, c] = np.bincount(grp, weights=u * (cum[:, c] - base[:, c]) + rel_in[pix] * t[:, c],
+                                  minlength=self.points)
+        # blur, v + 0.5 (a + b): the two roundings add at most u (|v| + |a| + |b|)
+        for n1, n2 in self.nbr:
+            Az, Ez = np.vstack([A, np.zeros((1, C))]), np.vstack([E, np.zeros((1, C))])
+            E = E + 0.5 * (Ez[n1] + Ez[n2]) + u * (A + Az[n1] + Az[n2])
+            A = A + 0.5 * (Az[n1] + Az[n2])
+        # slice, d + 1 fmaf with fp32 weights: (d + 2) u of the magnitude
+        Eo, Ao = np.zeros((self.N, C)), np.zeros((self.N, C))
+        for r in range(d + 1):
+            Eo += self.w[:, r, None] * E[self.inv[:, r]]
+            Ao += self.w[:, r, None] * A[self.inv[:, r]]
+        alpha = 1.0 / (1.0 + 2.0 ** (-d))
+        return alpha * (Eo + ((d + 2) * u + rel_out[:, None]) * Ao), alpha * Ao
+
+    def fp32_error_bound(self, values: np.ndarray, normalize: bool = False) -> np.ndarray:
+        """Componentwise bound on |dss_op_lattice_filter - filter| for fp32 ``values``, first order in u = 2^-24.
+
+        Every fp32 operation of the kernels rounds once to nearest (no fast math), so each adds at most u times the
+        magnitude of its result, and a magnitude is bounded by the same filter applied to |values|:
+          - slot weights are the float64 barycentric weights rounded to fp32: u;
+          - splat adds the n_j contributions of lattice point j one fmaf at a time in slot order: u sum_k |s_k| over
+            its partial sums, which is where the contribution counts enter (the busiest points of a VOC-size image
+            take 10^4 contributions);
+          - blur pass: u (|v| + |a| + |b|); slice: (d + 2) u of the magnitude; the alpha (fp32) and output scalings
+            add 2 u (3 u when normalised);
+          - normalised: n = 1 / sqrtf(alpha L(1) + 1e-20) inherits half the relative error of alpha L(1) + 1e-20 (its
+            alpha, product and sum roundings included) plus 2 u (sqrtf and the division), and the splat weights carry
+            n (one more product).
+        The neglected second-order terms are below (max_j n_j u)^2 of the bound; the float64 reference's own error is
+        some 10^9 times smaller than u."""
+        u = U32
+        mag = np.abs(np.asarray(values, np.float64))
+        one = np.full(self.N, u)
+        if not normalize:
+            return self._fp32_error(mag, one, 2 * one)[0] * (1 + 1e-3)
+        e1, s1 = self._fp32_error(np.ones((self.N, 1)), one, 3 * one)
+        en = 0.5 * (e1[:, 0] / s1[:, 0]) + 2 * u
+        n = self.norm()
+        e, _ = self._fp32_error(n[:, None] * mag, en + 2 * u, en + 3 * u)
+        return n[:, None] * e * (1 + 1e-3)
 
 
 def lattice_filter(features: np.ndarray, values: np.ndarray, normalize: bool = False) -> np.ndarray:

@@ -154,6 +154,50 @@ def test_stubbed_reference_command_equals_fixtures(name, tmp_path):
     assert np.array_equal(np.array(Image.open(tmp_path / "out" / f"{name}.png")), z["labels"])
 
 
+def test_key_layout_boundary_matches_restatement():
+    """dss_crf_segment accepts a batch iff oracle.crf_ref.key_bits puts both lattices' keys in at most 64 bits; at 65
+    and more it returns DSS_ERR_UNSUPPORTED before any device work. An accepted layout goes on to the workspace check,
+    which a 16-byte workspace fails, so the boundary is probed without a device."""
+    from oracle import crf_ref
+    _lib = load_pkg("_lib")
+    lib = _lib.load()
+    import torch
+    n0 = lib.dss_kernel_launch_count()
+    buf = torch.zeros(1 << 12, dtype=torch.uint8)
+    p = (buf.data_ptr() + 255) // 256 * 256
+    UNSUP, WS = -4, -3
+
+    def call(shapes, alpha, beta=13.0, gamma=3.0):
+        dims = np.array([[H, W, H // 16, W // 16] for H, W in shapes], np.int32)
+        return lib.dss_crf_segment(p, p, dims.ctypes.data, len(shapes), 16, 21, 10.0, alpha, beta, 3.0, gamma, 5, 1e-5,
+                                   p, None, p, p, 16, None)
+
+    def bits(shapes, alpha, beta=13.0, gamma=3.0):
+        H, W = max(h for h, _ in shapes), max(w for _, w in shapes)
+        return crf_ref.crf_key_bits(H, W, len(shapes), alpha, beta, gamma)
+
+    voc, big = (375, 500), (500, 500)
+    # the worked boundary cases: exactly 64 bits, then one image or one pixel of width more
+    assert bits([voc] * 2, 0.05) == (64, 19) and call([voc] * 2, 0.05) == WS
+    assert bits([voc] * 3, 0.05)[0] == 65 and call([voc] * 3, 0.05) == UNSUP
+    assert bits([voc] * 16, 0.1)[0] == 64 and call([voc] * 16, 0.1) == WS
+    assert bits([voc] * 15 + [big], 0.1)[0] == 65 and call([voc] * 15 + [big], 0.1) == UNSUP
+    assert bits([voc] * 16, 1.0, beta=0.5)[0] == 66 and call([voc] * 16, 1.0, beta=0.5) == UNSUP
+    assert bits([voc] * 16, 80.0) == (43, 22)              # the command's defaults leave 21 bits spare
+    # a sweep across the boundary, the spatial lattice's included
+    seen = set()
+    for shapes in ([voc], [voc] * 2, [voc, big, voc], [big] * 4, [voc] * 16, [voc] * 17, [(48, 64)] * 2):
+        for alpha in (0.004, 0.005, 0.008, 0.03, 0.05, 0.07, 0.08, 0.1, 0.13, 1.0):
+            for beta, gamma in ((13.0, 3.0), (0.5, 3.0), (13.0, 0.004), (13.0, 1e-3)):
+                b = bits(shapes, alpha, beta, gamma)
+                top = None if None in b else max(b)                # None: one field alone exceeds 62 bits
+                seen.add(top)
+                want = WS if top is not None and top <= 64 else UNSUP
+                assert call(shapes, alpha, beta, gamma) == want, (shapes, alpha, beta, gamma, b)
+    assert {62, 63, 64, 65, 66} <= seen
+    assert lib.dss_kernel_launch_count() == n0
+
+
 def test_crf_entry_points_reject_bad_arguments_before_any_device_work():
     _lib = load_pkg("_lib")
     lib = _lib.load()

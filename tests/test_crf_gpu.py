@@ -29,20 +29,33 @@ def _case(name):
     return z, image, seg, P, M, kw
 
 
+# "random" / "image": 1001 random points and a 37 x 45 image with 7 channels; "n<N>_c<C>": N random points with C
+# channels (every channel tail of the float4 class rows, up to 64; N around one 256-thread block); "image_c<C>"
+SOURCES = ["random", "image", "n1_c1", "n2_c3", "n7_c4", "n255_c5", "n256_c8", "n257_c16", "n1001_c17", "n1001_c33",
+           "image_c64"]
+
+
 @pytest.mark.parametrize("d", [2, 5])
-@pytest.mark.parametrize("source", ["random", "image"])
+@pytest.mark.parametrize("source", SOURCES)
 @pytest.mark.parametrize("normalize", [False, True])
 def test_lattice_filter_matches_float64_restatement(cuda, d, source, normalize):
     from oracle import crf_ref
     crf = load_pkg("crf")
-    rng = np.random.default_rng(d * 10 + (source == "image"))
-    if source == "random":
-        f = (rng.normal(size=(1001, d)) * 2.5).astype(np.float32)
+    rng = np.random.default_rng(d * 10 + (source == "image") if source in ("random", "image")
+                                else (d, SOURCES.index(source)))
+    kind, N, C = source, 1001, 7
+    if "_" in source:
+        kind, c = source.split("_")
+        C = int(c[1:])
+        if kind != "image":
+            kind, N = "random", int(kind[1:])
+    if kind == "random":
+        f = (rng.normal(size=(N, d)) * 2.5).astype(np.float32)
     else:
         img = load_pkg("synth").blobs_image(37, 45, 7).numpy()
         fb, fs = crf_ref.crf_features(img, 80, 13, 3)
         f = (fb if d == 5 else fs).astype(np.float32)
-    v = rng.random((f.shape[0], 7)).astype(np.float32)
+    v = rng.random((f.shape[0], C)).astype(np.float32)
     out, points = crf.lattice_filter(torch.from_numpy(f).to(cuda), torch.from_numpy(v).to(cuda), normalize)
     lat = crf_ref.Lattice(f.astype(np.float64))
     want = lat.filter(v.astype(np.float64), normalize)
