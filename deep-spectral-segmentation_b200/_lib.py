@@ -110,11 +110,16 @@ PROTOTYPES = {
     "dss_op_im2col_pad_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "dss_upsample_bilinear": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "dss_normalize_rows": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "dss_segeval_workspace_bytes": (c_size_t, [c_int, C.c_longlong]),
+    "dss_segeval_counts": (c_int, [c_void_p, C.c_longlong, c_void_p, C.c_longlong, c_void_p, c_int, c_void_p,
+                                   C.c_longlong, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
 }
 
 EPI_BIAS_F16, EPI_BIAS_GELU_F16, EPI_BIAS_RESID_F32, EPI_BIAS_F32, EPI_PATCH_F32, EPI_DROPCLS_F32 = range(6)
 AFF_NORMALIZE, AFF_THRESHOLD_AT_ZERO, AFF_NO_MAX_SCALE = 1, 2, 4
 LOC_OK, LOC_NO_GRID, LOC_SEED_IN_BACKGROUND, LOC_EMPTY_COMPONENT = range(4)
+SEGEVAL_SEMANTIC, SEGEVAL_BINARY, SEGEVAL_FIELDS = 0, 1, 13
+DSS_ERR_UNSUPPORTED = -4
 
 _lib = None
 

@@ -394,6 +394,27 @@ int dss_upsample_bilinear(const float* feats, int B, int Hp, int Wp, int d, int 
 /* Row-wise L2 normalisation x / max(||x||, 1e-12) (F.normalize, extract.py:148): feats [rows, d] -> out [rows, d]. */
 int dss_normalize_rows(const float* feats, int rows, int d, float* out, dss_stream_t stream);
 
+/* Segmentation evaluation counts of a ragged batch of (prediction, target) uint8 label maps (the pixel loops of the
+ * reference's semantic-segmentation/eval.py and object-segmentation/main.py). images_host [B, DSS_SEGEVAL_FIELDS] int64
+ * per image: {pred_offset, pred_h, pred_w, target_offset, target_h, target_w, top, left, h, w, block_h, block_w,
+ * table_offset}: maps are row-major at byte offsets of preds / targets (device); output pixel (y, x), 0 <= y < h,
+ * 0 <= x < w, reads target (top + y, left + x) and prediction (rows[y], cols[x]), where tables_host (int32, host) holds
+ * at table_offset rows_in[h], rows_out[h], cols_in[w], cols_out[w]: pixels with y < block_h and x < block_w use the
+ * _in halves, all others the _out halves.
+ *   DSS_SEGEVAL_SEMANTIC: target 255 is ignored; counts [256, num_classes + 1] int64 (device) += pixels per
+ *     (prediction value, target bin), bin = target if target < num_classes else num_classes. 2 <= num_classes + 1
+ *     <= 64, else DSS_ERR_UNSUPPORTED.
+ *   DSS_SEGEVAL_BINARY: prediction != 0 against target >= 128; counts [B, 4] int64 (device) = {TP, FP, FN, TN}.
+ * Integer arithmetic only: an image gets the same counts alone or in any batch. Table entries outside the prediction,
+ * crops outside the target, offsets outside the buffers, maps of 2^31 cells or rows wider than 2^24 pixels:
+ * DSS_ERR_UNSUPPORTED. Workspace: dss_segeval_workspace_bytes(B, table entries). */
+#define DSS_SEGEVAL_FIELDS 13
+enum { DSS_SEGEVAL_SEMANTIC = 0, DSS_SEGEVAL_BINARY = 1 };
+size_t dss_segeval_workspace_bytes(int B, long long table_entries);
+int dss_segeval_counts(const uint8_t* preds, long long preds_bytes, const uint8_t* targets, long long targets_bytes,
+                       const long long* images_host, int B, const int* tables_host, long long table_entries, int mode,
+                       int num_classes, long long* counts, void* ws, size_t ws_bytes, dss_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
