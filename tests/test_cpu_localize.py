@@ -7,6 +7,7 @@ from pathlib import Path
 
 import numpy as np
 import pytest
+import scipy.ndimage
 import torch
 
 from conftest import ROOT, load_pkg
@@ -57,6 +58,84 @@ def test_dinoseg_restatement_reproduces_reference():
                 localize_ref.dinoseg_box(a[head], grid, P)
         else:
             assert np.array_equal(localize_ref.dinoseg_box(a[head], grid, P), z["boxes"][i]), i
+
+
+GRIDS = [(1, 1), (1, 16384), (16384, 1), (2, 8192), (63, 63), (127, 129), (128, 128)]
+
+
+def test_cc_patterns_have_the_designed_components():
+    """The edge-case masks the GPU tests feed all three kernels: counted with scipy under both connectivities."""
+    def count(m, conn8):
+        return scipy.ndimage.label(m, structure=localize_ref.EIGHT if conn8 else None)[1]
+
+    for gh, gw in GRIDS:
+        p = localize_ref.cc_patterns(gh, gw)
+        N = gh * gw
+        assert p["all"].all() and not p["none"].any()
+        assert 2 * p["half"].sum() == 2 * (N // 2) and p["half_plus_one"].sum() == N // 2 + 1
+        if N > 1:
+            assert count(p["checkerboard"], True) == 1 or min(gh, gw) == 1
+            assert count(p["checkerboard"], False) == p["checkerboard"].sum()
+        if min(gh, gw) >= 3:
+            assert count(p["row_ends"], True) == p["row_ends"].sum()       # no wrap between the two ends of a row
+            assert count(p["row_wrap"], False) == p["row_wrap"].sum()      # nor from one row's end to the next's start
+            assert count(p["u"], False) == 1 and count(p["serpentine"], False) == 1
+            lab, n = scipy.ndimage.label(p["twin"])
+            assert n == 2 and (lab == 1).sum() == (lab == 2).sum()
+    assert localize_ref.cc_patterns(128, 128)["dots"].sum() == 4096
+    assert scipy.ndimage.label(localize_ref.cc_patterns(128, 128)["twin_then_small"])[1] == 3
+
+
+def test_dyadic_rows_give_designed_masks_under_torch():
+    """Every dyadic row the GPU tests use: exact in fp32 under torch's own CPU sort / sum / cumsum (dyadic_exact), and
+    the reference's ops keep exactly the designed cells, with either normalising sum. The last non-kept cell's
+    cumulative mass is fl32(0.4) = 0x3ECCCCCD itself, and torch compares with it in fp32 (it is not kept)."""
+    assert np.float32(localize_ref.THRESHOLD_UNITS * localize_ref.DYADIC_UNIT).view(np.uint32) == 0x3ECCCCCD
+    assert np.float32(1 - 0.6).view(np.uint32) == 0x3ECCCCCD
+    assert not (torch.tensor([np.float32(0.4)]) > (1 - 0.6)).item()
+    used = zeros = 0
+    for gh, gw in GRIDS + [(14, 14), (8, 12)]:
+        for name, m in localize_ref.cc_patterns(gh, gw).items():
+            try:
+                u = localize_ref.dyadic_row(m)
+            except ValueError:
+                continue
+            row = (u * localize_ref.DYADIC_UNIT).astype(np.float32)
+            srt = np.sort(u)
+            assert np.cumsum(srt)[(~m).sum() - 1] == localize_ref.THRESHOLD_UNITS
+            zeros += int((u == 0).sum())
+            for total in ("torch", "fp64"):
+                assert np.array_equal(localize_ref.dinoseg_kept(row, total), m.ravel()), (gh, gw, name, total)
+            used += 1
+    assert used >= 60 and zeros >= 100000                              # runs of exact zeros (underflowed softmax)
+    # equal values straddling the threshold: the smaller index is the last one not kept
+    m = np.zeros((8, 12), bool)
+    m[3:6, 4:8] = True
+    m[7, 11] = True
+    u = localize_ref.dyadic_row(m, tie_cell=2 * 12 + 4)
+    assert u[2 * 12 + 4] == u[3 * 12 + 4]
+    assert np.array_equal(localize_ref.dinoseg_kept((u * localize_ref.DYADIC_UNIT).astype(np.float32)), m.ravel())
+
+
+def test_lost_expand_in_chunks_and_sum_decidability():
+    """lost_expand reading A in row chunks gives lost_box's seed and M; where torch's CPU sum (the reference's
+    torch.sum(A[similars, :], dim=0)) and the sequential fp32 sum have different signs, sum_decided calls the cell
+    undecidable."""
+    rng = np.random.default_rng(5)
+    f = rng.normal(0, 1, (24 * 32, 64)).astype(np.float32)
+    A = f @ f.T
+    for k in (1, 33, 100, A.shape[0]):
+        seed, sim, M = localize_ref.lost_expand(lambda idx: A[idx], A.shape[0], k, chunk=100)
+        box, s2 = localize_ref.lost_box(A, (24, 32), (24 * 16, 32 * 16), 16, k)
+        assert seed == s2 and np.array_equal(localize_ref.detect_box(M, seed, (24, 32), (384, 512), 16)[0], box)
+        m64, decided = localize_ref.sum_decided(A[sim])
+        mt = torch.sum(torch.from_numpy(A[sim]), dim=0).numpy()
+        assert not ((M > 0) != (mt > 0))[decided].any()
+        assert ((M > 0) == (m64 > 0))[decided].all()
+    # integer rows: every order is exact, every nonzero cell is decided
+    a = rng.integers(-3, 4, (40, 50)).astype(np.float32)
+    m64, decided = localize_ref.sum_decided(a)
+    assert np.array_equal(decided, m64 != 0)
 
 
 def _tree(tmp_path):

@@ -104,11 +104,12 @@ def test_dinoseg_kernel_matches_fixtures_and_random_maps(cuda):
         boxes, status = loc.dinoseg_boxes(torch.from_numpy(a).to(cuda), (gh, gw), 16, 4)
         for b in range(4):
             row = a[b, 4]
-            srt = np.sort(row.astype(np.float64))
-            if (np.abs(np.cumsum(srt / srt.sum()) - 0.4) < 1e-6).any():
-                continue
-            assert status[b] == 0 and np.array_equal(boxes[b], localize_ref.dinoseg_box(row, (gh, gw), 16))
-            checked += 1
+            # the kernel normalises by the exactly rounded sum; torch's float sum may differ by an ulp and keep other cells
+            k64 = localize_ref.dinoseg_kept(row, "fp64")
+            assert status[b] == 0 and np.array_equal(boxes[b], localize_ref.dinoseg_select(k64, (gh, gw), 16)[0])
+            if np.array_equal(k64, localize_ref.dinoseg_kept(row)):
+                assert np.array_equal(boxes[b], localize_ref.dinoseg_box(row, (gh, gw), 16))
+                checked += 1
     assert checked >= 12
 
 
@@ -116,15 +117,18 @@ def test_cls_attention_kernel(cuda):
     """Against the float64 softmax of the same fp16 qkv, logits of standard deviation 1. (At a logit spread of 4 the
     fp32 rounding of the scores alone reaches 1.3e-6 relative.)"""
     _lib = load_pkg("_lib")
+    g = torch.Generator(device=cuda).manual_seed(197)   # its own stream: the draw must not depend on earlier tests
     for B, T, heads in [(2, 197, 6), (3, 1025, 12), (1, 2, 6)]:
-        qkv = torch.randn(B, T, 3 * heads * 64, device=cuda).half()   # q . k / 8 has standard deviation 1
+        qkv = torch.randn(B, T, 3 * heads * 64, generator=g, device=cuda).half()   # q . k / 8 has standard deviation 1
         out = torch.empty(B, heads, T - 1, device=cuda)
         _lib.check(_lib.load().dss_op_cls_attention(qkv.data_ptr(), B, T, heads, out.data_ptr(), _lib.stream_ptr(cuda)))
         want = localize_ref.cls_attention_from_qkv(qkv.cpu(), heads)
         err = out.cpu().double() - want
         rel = (err.norm(dim=-1) / want.norm(dim=-1)).max().item()          # per (image, head) row
         assert rel <= 1e-6, rel
-        assert (err.abs().amax(-1) <= 1e-6 * want.amax(-1)).all()
+        # per element, from the kernel's roundings (1e-6 of the row's max is not a bound: some draws exceed it)
+        _, bound = localize_ref.cls_attention_bound(qkv, heads)
+        assert (err.abs() <= bound).all(), float((err.abs() / bound).max())
 
 
 @pytest.mark.parametrize("name", ["dino_vits16", "dino_vits8"])
