@@ -76,6 +76,9 @@ PROTOTYPES = {
                                     c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "dss_eigsh_topk": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p,
                                c_void_p, c_void_p, c_size_t, c_void_p]),
+    "dss_debug_eigsh_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int, c_int]),
+    "dss_debug_eigsh": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_int, c_void_p,
+                                c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "dss_rw_affinity_add": (c_int, [c_void_p, c_int, c_int, c_int, c_float, C.c_double, c_void_p, c_int, c_void_p,
                                     c_void_p]),
     "dss_segment_threshold": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_float, c_void_p, c_void_p]),

@@ -343,6 +343,27 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
+// LayerNorm arithmetic of one row held as float4 chunks per lane, shared by layernorm_f16_kernel and the fused LayerNorm
+// GEMM (gemm_ln.cu) so that the fused GEMM's A operand is bit for bit the stand-alone kernel's output. Every rounding is
+// explicit (no contraction is left to the compiler, which chose differently in the two kernels): x - mean is one fused
+// multiply-add on the row sum S (the mean itself is never rounded), the squares pair as fma(a, a, b * b), the variance is
+// fma(Q, 1 / d, eps), and y = fma((x - mean) * rstd, gamma, beta).
+__device__ __forceinline__ float ln_sum4(float4 v) { return __fadd_rn(__fadd_rn(v.x, v.y), __fadd_rn(v.z, v.w)); }
+__device__ __forceinline__ float4 ln_center4(float4 v, float S, float inv_d) {
+  return make_float4(__fmaf_rn(S, -inv_d, v.x), __fmaf_rn(S, -inv_d, v.y), __fmaf_rn(S, -inv_d, v.z),
+                     __fmaf_rn(S, -inv_d, v.w));
+}
+__device__ __forceinline__ float ln_sq4(float4 a) {
+  return __fadd_rn(__fmaf_rn(a.x, a.x, __fmul_rn(a.y, a.y)), __fmaf_rn(a.z, a.z, __fmul_rn(a.w, a.w)));
+}
+__device__ __forceinline__ float ln_rstd(float Q, float inv_d, float eps) { return rsqrtf(__fmaf_rn(Q, inv_d, eps)); }
+// the four outputs of a centred chunk a, as two packed half2
+__device__ __forceinline__ uint2 ln_out4(float4 a, float rstd, float4 g, float4 b) {
+  uint2 o;
+  o.x = pack_half2(__fmaf_rn(__fmul_rn(a.x, rstd), g.x, b.x), __fmaf_rn(__fmul_rn(a.y, rstd), g.y, b.y));
+  o.y = pack_half2(__fmaf_rn(__fmul_rn(a.z, rstd), g.z, b.z), __fmaf_rn(__fmul_rn(a.w, rstd), g.w, b.w));
+  return o;
+}
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

@@ -18,6 +18,8 @@
 // One start vector sees a single direction of every eigenspace, so at an eigenvalue of multiplicity > 1 the Krylov space
 // becomes invariant (breakdown) before all copies are found. The iteration then restarts from a fresh vector orthogonal
 // to the basis: T becomes block diagonal, and Ritz vectors are taken per block, so each copy gets its own vector.
+// Three instantiations exist (<4, 1, 512> the default, <2, 2, 512> and <4, 2, 256> two CTAs per SM); dss_debug_eigsh
+// runs any of them on the same inputs, for the A/B of EIG_PAIR_DEFAULT and for the tests of the paired ones.
 #include <math.h>
 #include <stdlib.h>
 
@@ -689,33 +691,30 @@ static int eig_variant() {
   return variant;
 }
 
-static int eig_per_sm(int Npad, int mmax) {
+// variant: 1 = <2, 2, 512>, 2 = <4, 1, 512>, 3 = <4, 2, 256>, anything else = the default
+static int eig_per_sm(int Npad, int mmax, int variant) {
   const size_t smem = eig_smem_bytes(Npad, mmax);
   const int fit = (int)((size_t)(220 * 1024) / (smem + 1024));
-  const int v = eig_variant();
-  if (v == 2) return 1;
-  if (v == 1 || v == 3) return fit >= 2 ? 2 : 1;
+  if (variant == 2) return 1;
+  if (variant == 1 || variant == 3) return fit >= 2 ? 2 : 1;
   return (EIG_PAIR_DEFAULT && fit >= 2) ? 2 : 1;
 }
 
-static int eig_grid(int B, int Npad, int mmax) {
+static int eig_grid(int B, int Npad, int mmax, int variant) {
   int sms = device_sm_count();
   if (sms <= 0) sms = 132;
-  const int g = sms * eig_per_sm(Npad, mmax);
+  const int g = sms * eig_per_sm(Npad, mmax, variant);
   return B < g ? B : g;
 }
 
-}  // namespace dss
-
-using namespace dss;
-
-extern "C" size_t dss_eigsh_workspace_bytes(int B, int N, int K, int max_steps) {
+// every CTA owns a basis and a tridiagonal scratch slice: the size follows the grid of the variant
+static size_t eig_workspace_bytes(int B, int N, int K, int max_steps, int variant) {
   if (B <= 0 || N <= 0 || K <= 0) return 0;
   const int Npad = (N + 3) & ~3;
   size_t bytes = 0;
   for (const bool plain : {false, true}) {   // one size serves both entry points
     const int mmax = eig_resolve(N, K, max_steps, plain);
-    const int grid = eig_grid(B, Npad, mmax);
+    const int grid = eig_grid(B, Npad, mmax, variant);
     const size_t basis = align_up((size_t)grid * (mmax + 1) * Npad * sizeof(float), 256);
     const size_t tri = align_up((size_t)grid * 2 * (K + 1) * mmax * sizeof(double), 256);
     bytes = basis + tri > bytes ? basis + tri : bytes;
@@ -723,37 +722,52 @@ extern "C" size_t dss_eigsh_workspace_bytes(int B, int N, int K, int max_steps) 
   return bytes;
 }
 
+}  // namespace dss
+
+using namespace dss;
+
+extern "C" size_t dss_eigsh_workspace_bytes(int B, int N, int K, int max_steps) {
+  return eig_workspace_bytes(B, N, K, max_steps, eig_variant());
+}
+
+// forced: the variant was asked for explicitly (dss_debug_eigsh), so a pairing that does not fit is an error instead of
+// a fall-back to <4, 1, 512>
 static int eigsh_launch(const float* Wmat, const float* deg, int ldw, int B, int N, int K, int mode, float tol, int max_steps,
-                        float* evals, float* evecs, int* info, float* resid, void* ws, size_t ws_bytes,
-                        dss_stream_t stream) {
+                        int variant, bool forced, float* evals, float* evecs, int* info, float* resid, void* ws,
+                        size_t ws_bytes, dss_stream_t stream) {
   DSS_REQUIRE(Wmat && evals && evecs && info && ws, "eigsh: null pointer");
   DSS_REQUIRE(B > 0 && N > 1, "eigsh: empty problem B=%d N=%d", B, N);
   DSS_REQUIRE(K >= 1 && K <= EIG_MAX_K && K < N, "eigsh: need 1 <= K <= %d and K < N (K=%d N=%d)", EIG_MAX_K, K, N);
   DSS_REQUIRE(ldw >= N && ldw % 4 == 0, "eigsh: ldw must be >= N and a multiple of 4 (N=%d ldw=%d)", N, ldw);
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0 && (reinterpret_cast<uintptr_t>(Wmat) & 15) == 0,
               "eigsh: workspace must be 256-byte aligned and W 16-byte aligned");
-  const size_t need = dss_eigsh_workspace_bytes(B, N, K, max_steps);
-  if (ws_bytes < need) {
-    set_error("eigsh: workspace too small (%zu < %zu)", ws_bytes, need);
-    return DSS_ERR_WORKSPACE;
-  }
   EigParams p;
   p.W = Wmat; p.deg = deg; p.evals = evals; p.evecs = evecs; p.info = info; p.resid = resid;
   p.B = B; p.N = N; p.ldw = ldw; p.Npad = (N + 3) & ~3; p.K = K; p.mode = mode;
   p.mmax = eig_resolve(N, K, max_steps, mode == 2);
   p.tol = tol > 0.f ? tol : 1e-6f;
-  const int grid = eig_grid(B, p.Npad, p.mmax);
+  const size_t smem = eig_smem_bytes(p.Npad, p.mmax);
+  const int per_sm = eig_per_sm(p.Npad, p.mmax, variant);
+  if (forced && (variant == 1 || variant == 3) && per_sm != 2) {
+    set_error("eigsh: variant %d pairs two CTAs per SM, but N=%d with max_steps=%d needs %zu B of shared memory per CTA",
+              variant, N, p.mmax, smem);
+    return DSS_ERR_UNSUPPORTED;
+  }
+  const size_t need = eig_workspace_bytes(B, N, K, max_steps, variant);
+  if (ws_bytes < need) {
+    set_error("eigsh: workspace too small (%zu < %zu)", ws_bytes, need);
+    return DSS_ERR_WORKSPACE;
+  }
+  const int grid = eig_grid(B, p.Npad, p.mmax, variant);
   p.basis = reinterpret_cast<float*>(ws);
   p.tri = reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(ws) +
                                     align_up((size_t)grid * (p.mmax + 1) * p.Npad * sizeof(float), 256));
-  const size_t smem = eig_smem_bytes(p.Npad, p.mmax);
   if (smem > 227 * 1024) {
     set_error("eigsh: N=%d with max_steps=%d needs %zu B of shared memory (> 227 KB)", N, p.mmax, smem);
     return DSS_ERR_UNSUPPORTED;
   }
   LaunchScope scope(static_cast<cudaStream_t>(stream), KC_EIGSH);
-  const int per_sm = eig_per_sm(p.Npad, p.mmax);
-  if (per_sm == 2 && eig_variant() == 1) {
+  if (per_sm == 2 && variant == 1) {
     DSS_CHECK_CUDA(cudaFuncSetAttribute(lanczos_laplacian_kernel<2, 2, EIG_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     lanczos_laplacian_kernel<2, 2, EIG_THREADS><<<grid, EIG_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(p);
   } else if (per_sm == 2) {
@@ -770,11 +784,27 @@ static int eigsh_launch(const float* Wmat, const float* deg, int ldw, int B, int
 extern "C" int dss_eigsh_laplacian(const float* Wmat, const float* degree, int ldw, int B, int N, int K, int lapnorm,
                                    float tol, int max_steps, float* evals, float* evecs, int* info, float* resid,
                                    void* ws, size_t ws_bytes, dss_stream_t stream) {
-  return eigsh_launch(Wmat, degree, ldw, B, N, K, lapnorm ? 0 : 1, tol, max_steps, evals, evecs, info, resid, ws, ws_bytes,
-                      stream);
+  return eigsh_launch(Wmat, degree, ldw, B, N, K, lapnorm ? 0 : 1, tol, max_steps, eig_variant(), false, evals, evecs, info,
+                      resid, ws, ws_bytes, stream);
 }
 
 extern "C" int dss_eigsh_topk(const float* Amat, int lda, int B, int N, int K, float tol, int max_steps, float* evals,
                               float* evecs, int* info, float* resid, void* ws, size_t ws_bytes, dss_stream_t stream) {
-  return eigsh_launch(Amat, nullptr, lda, B, N, K, 2, tol, max_steps, evals, evecs, info, resid, ws, ws_bytes, stream);
+  return eigsh_launch(Amat, nullptr, lda, B, N, K, 2, tol, max_steps, eig_variant(), false, evals, evecs, info, resid, ws,
+                      ws_bytes, stream);
+}
+
+static bool eig_debug_variant(int variant) { return variant >= 1 && variant <= 3; }
+
+extern "C" size_t dss_debug_eigsh_workspace_bytes(int B, int N, int K, int max_steps, int variant) {
+  return eig_debug_variant(variant) ? eig_workspace_bytes(B, N, K, max_steps, variant) : 0;
+}
+
+extern "C" int dss_debug_eigsh(const float* Wmat, const float* degree, int ldw, int B, int N, int K, int mode, float tol,
+                               int max_steps, int variant, float* evals, float* evecs, int* info, float* resid, void* ws,
+                               size_t ws_bytes, dss_stream_t stream) {
+  DSS_REQUIRE(eig_debug_variant(variant), "eigsh: variant must be 1, 2 or 3 (got %d)", variant);
+  DSS_REQUIRE(mode >= 0 && mode <= 2, "eigsh: mode must be 0, 1 or 2 (got %d)", mode);
+  return eigsh_launch(Wmat, mode == 2 ? nullptr : degree, ldw, B, N, K, mode, tol, max_steps, variant, true, evals, evecs,
+                      info, resid, ws, ws_bytes, stream);
 }

@@ -13,7 +13,8 @@
 //                     groups have released the panel, the rows are re-read, normalised and written
 //   warp groups 1, 2  wgmma m64 x BN x 16 on 64 rows each, epilogue from the register accumulators (+bias -> GELU ->
 //                     fp16 -> swizzled staging box -> TMA store)
-// The arithmetic of the normalisation is that of layernorm_f16_kernel, so the A operand is the same fp16 values.
+// The normalisation is layernorm_f16_kernel's arithmetic (the ln_* helpers of common.cuh, every rounding explicit), so
+// the A operand is bit for bit the stand-alone kernel's output.
 #include <math.h>
 
 #include "common.cuh"
@@ -31,7 +32,7 @@ template <int BN> struct LnCfg {
   static constexpr int A_BYTES = LG_SLABS * LG_SLAB_BYTES;          // 96 KB
   static constexpr int B_STAGE = BN * 128;                          // BN rows x 64 f16
   static constexpr int STAGING = 2 * LG_BOX_BYTES;
-  static constexpr int VEC_BYTES = 2 * LG_BM * 4;                   // mean[128], rstd[128]
+  static constexpr int VEC_BYTES = 2 * LG_BM * 4;                   // row sum[128], rstd[128]
   static constexpr int FIXED = A_BYTES + STAGING + VEC_BYTES + 256 + 1024;
   static constexpr int STAGES = (232448 - FIXED) / B_STAGE > 6 ? 6 : (232448 - FIXED) / B_STAGE;
   static constexpr int SMEM = FIXED + STAGES * B_STAGE;
@@ -59,8 +60,8 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* gbase = smem_raw + (base - raw);
   const uint32_t sA = base, sB = base + Cfg::A_BYTES, sOut = sB + STAGES * Cfg::B_STAGE;
-  float* s_mean = reinterpret_cast<float*>(gbase + Cfg::A_BYTES + STAGES * Cfg::B_STAGE + Cfg::STAGING);
-  float* s_rstd = s_mean + LG_BM;
+  float* s_sum = reinterpret_cast<float*>(gbase + Cfg::A_BYTES + STAGES * Cfg::B_STAGE + Cfg::STAGING);
+  float* s_rstd = s_sum + LG_BM;
   const uint32_t bar_base = sOut + Cfg::STAGING + Cfg::VEC_BYTES;
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
@@ -110,7 +111,7 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
       auto stats = [&](int m0) {
         for (int r = lw; r < LG_BM; r += LG_LN_WARPS) {
           const int m = m0 + r;
-          float mean = 0.f, rstd = 0.f;
+          float S = 0.f, rstd = 0.f;
           if (m < p.M) {
             const float4* xr = reinterpret_cast<const float4*>(p.x + (long long)m * LG_K);
             float4 v[3];
@@ -118,18 +119,15 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
 #pragma unroll
             for (int i = 0; i < 3; ++i) {
               v[i] = xr[lane + 32 * i];
-              s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+              s = __fadd_rn(s, ln_sum4(v[i]));
             }
-            mean = warp_sum(s) * (1.0f / LG_K);
+            S = warp_sum(s);
             float q = 0.f;
 #pragma unroll
-            for (int i = 0; i < 3; ++i) {
-              const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, e = v[i].w - mean;
-              q += (a * a + b * b) + (c * c + e * e);
-            }
-            rstd = rsqrtf(warp_sum(q) * (1.0f / LG_K) + p.eps);
+            for (int i = 0; i < 3; ++i) q = __fadd_rn(q, ln_sq4(ln_center4(v[i], S, 1.0f / LG_K)));
+            rstd = ln_rstd(warp_sum(q), 1.0f / LG_K, p.eps);
           }
-          if (lane == 0) { s_mean[r] = mean; s_rstd[r] = rstd; }
+          if (lane == 0) { s_sum[r] = S; s_rstd[r] = rstd; }
         }
         __syncwarp();
       };
@@ -141,7 +139,7 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
         __syncwarp();
         for (int r = lw; r < LG_BM; r += LG_LN_WARPS) {
           const int m = m0 + r;
-          const float mean = s_mean[r], rstd = s_rstd[r];
+          const float S = s_sum[r], rstd = s_rstd[r];
 #pragma unroll
           for (int i = 0; i < 3; ++i) {
             const int c = 4 * (lane + 32 * i);   // first of this lane's 4 columns
@@ -150,8 +148,7 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
               const float4 v = reinterpret_cast<const float4*>(p.x + (long long)m * LG_K)[lane + 32 * i];
               const float4 g = __ldg(reinterpret_cast<const float4*>(p.gamma) + lane + 32 * i);
               const float4 bt = __ldg(reinterpret_cast<const float4*>(p.beta) + lane + 32 * i);
-              o.x = pack_half2((v.x - mean) * rstd * g.x + bt.x, (v.y - mean) * rstd * g.y + bt.y);
-              o.y = pack_half2((v.z - mean) * rstd * g.z + bt.z, (v.w - mean) * rstd * g.w + bt.w);
+              o = ln_out4(ln_center4(v, S, 1.0f / LG_K), rstd, g, bt);
             }
             const uint32_t addr = sA + (c >> 6) * LG_SLAB_BYTES + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2;
             asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(o.x), "r"(o.y) : "memory");

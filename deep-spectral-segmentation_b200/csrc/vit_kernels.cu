@@ -71,7 +71,8 @@ __global__ void cls_row_kernel(float* __restrict__ x, const float* __restrict__ 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// LayerNorm: one warp per row, row kept in registers, two-pass variance (mean, then E[(x-mean)^2]) like torch.
+// LayerNorm: one warp per row, row kept in registers, two-pass variance (mean, then E[(x-mean)^2]) like torch,
+// in the arithmetic of the ln_* helpers (common.cuh) that the fused LayerNorm GEMM shares.
 template <int D>
 __global__ void __launch_bounds__(256)
 layernorm_f16_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -86,24 +87,22 @@ layernorm_f16_kernel(const float* __restrict__ x, const float* __restrict__ gamm
 #pragma unroll
   for (int i = 0; i < V; ++i) {
     v[i] = xr[lane + 32 * i];
-    s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
+    s = __fadd_rn(s, ln_sum4(v[i]));
   }
-  const float mean = warp_sum(s) * (1.0f / D);
+  const float S = warp_sum(s);
   float q = 0.f;
 #pragma unroll
   for (int i = 0; i < V; ++i) {
-    const float a = v[i].x - mean, b = v[i].y - mean, c = v[i].z - mean, e = v[i].w - mean;
-    q += (a * a + b * b) + (c * c + e * e);
+    v[i] = ln_center4(v[i], S, 1.0f / D);
+    q = __fadd_rn(q, ln_sq4(v[i]));
   }
-  const float rstd = rsqrtf(warp_sum(q) * (1.0f / D) + eps);
+  const float rstd = ln_rstd(warp_sum(q), 1.0f / D, eps);
   uint2* yr = reinterpret_cast<uint2*>(y + (long long)warp * D);
 #pragma unroll
   for (int i = 0; i < V; ++i) {
     const float4 g = __ldg(reinterpret_cast<const float4*>(gamma) + lane + 32 * i);
     const float4 bt = __ldg(reinterpret_cast<const float4*>(beta) + lane + 32 * i);
-    uint2 o;
-    o.x = pack_half2((v[i].x - mean) * rstd * g.x + bt.x, (v[i].y - mean) * rstd * g.y + bt.y);
-    o.y = pack_half2((v[i].z - mean) * rstd * g.z + bt.z, (v[i].w - mean) * rstd * g.w + bt.w);
+    const uint2 o = ln_out4(v[i], rstd, g, bt);
     yr[lane + 32 * i] = o;
   }
 }

@@ -225,6 +225,15 @@ int dss_eigsh_laplacian(const float* Wmat, const float* degree, int ldw, int B, 
  * F^ F^T, extract.py:160-163). Same workspace / info / resid conventions as dss_eigsh_laplacian. */
 int dss_eigsh_topk(const float* Amat, int lda, int B, int N, int K, float tol, int max_steps, float* evals,
                    float* evecs, int* info, float* resid, void* ws, size_t ws_bytes, dss_stream_t stream);
+/* Debug: dss_eigsh_laplacian (mode 0 = lapnorm, 1 = unnormalised) or dss_eigsh_topk (mode 2, degree ignored) with the
+ * instantiation forced: variant 1 = <2, 2, 512>, 2 = <4, 1, 512> (the default), 3 = <4, 2, 256>. The paired variants 1
+ * and 3 run two CTAs per SM, each with its own scratch slice, so they need up to twice the workspace of
+ * dss_eigsh_workspace_bytes; a paired variant whose two CTAs do not fit in shared memory is DSS_ERR_UNSUPPORTED (no
+ * fall-back). A bad variant or mode is DSS_ERR_BAD_ARG (the workspace query returns 0). Not used by the product path. */
+size_t dss_debug_eigsh_workspace_bytes(int B, int N, int K, int max_steps, int variant);
+int dss_debug_eigsh(const float* Wmat, const float* degree, int ldw, int B, int N, int K, int mode, float tol,
+                    int max_steps, int variant, float* evals, float* evecs, int* info, float* resid, void* ws,
+                    size_t ws_bytes, dss_stream_t stream);
 
 /* Random-walk colour affinity (which_color_matrix='rw', extract_utils.py:191-204 -> pymatting _rw_laplacian with
  * radius 1): Wmat[b, i, j] += float32(sum over the 3x3 clamped neighbourhood offsets that land on j of

@@ -40,6 +40,18 @@ def test_bad_arguments_are_rejected_before_any_device_work():
     assert lib.dss_affinity(p, 1, 10, 8, 3, None, 0.0, p, 12, None, p, 16, None) == -3         # workspace too small
     assert lib.dss_eigsh_laplacian(p, None, 12, 1, 10, 10, 1, 0.0, 0, p, p, p, None, p, 1 << 15, None) == -1   # K >= N
     assert lib.dss_eigsh_laplacian(p, None, 12, 1, 10, 0, 1, 0.0, 0, p, p, p, None, p, 1 << 15, None) == -1    # K < 1
+    for variant, mode in ((0, 0), (4, 0), (-1, 2), (3, 3), (1, -1)):                     # forced instantiation
+        assert lib.dss_debug_eigsh(p, None, 12, 1, 10, 5, mode, 0.0, 0, variant, p, p, p, None, p, 1 << 15, None) == -1
+    assert lib.dss_debug_eigsh_workspace_bytes(1, 10, 5, 0, 0) == 0
+    assert lib.dss_debug_eigsh_workspace_bytes(1, 10, 5, 0, 4) == 0
+    assert lib.dss_debug_eigsh(p, None, 12, 1, 10, 10, 0, 0.0, 0, 3, p, p, p, None, p, 1 << 15, None) == -1  # K >= N
+    for variant in (1, 2, 3):
+        need = lib.dss_debug_eigsh_workspace_bytes(300, 700, 5, 0, variant)
+        assert need >= lib.dss_eigsh_workspace_bytes(300, 700, 5, 0) > 0
+        assert lib.dss_debug_eigsh(p, None, 700, 300, 700, 5, 0, 0.0, 0, variant, p, p, p, None, p, need - 1,
+                                   None) == -3                                              # one byte short
+    assert lib.dss_debug_eigsh(p, None, 4000, 1, 4000, 5, 0, 0.0, 0, 3, p, p, p, None, p, 1 << 30, None) == -4
+    assert b"N=4000" in lib.dss_last_error()                                                # two CTAs do not fit
     assert lib.dss_op_gemm_f16(p, p, p, p, 16, 30, 64, 0, None, 0, 0, None) == -1           # N % 32
     assert lib.dss_op_layernorm_f16(p, p, p, p, 4, 100, 1e-6, None) == -1                   # unsupported width
     cfg = _lib.VitConfig(16, 384, 12, 5, 4, 14, 1e-6)                                       # 384 / 5 != 64

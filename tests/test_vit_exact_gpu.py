@@ -416,6 +416,34 @@ def test_im2col_layout(cuda, B, H, W, P):
         assert torch.equal(got, want), f"images {b0}..{b0 + nb - 1}: {_diff(got != want)}"
 
 
+def _ln_inputs(M, d, g, dev):
+    """LayerNorm rows in repeating groups of 1024: N(0.5, 3^2) in [0, 256), a common offset of 1e3 in [256, 512) and
+    of -2e3 in [512, 640), one outlier channel (x 50) per row in [640, 896), tiny rows (x 1e-3) in [896, 1024)."""
+    x = torch.randn(M, d, generator=g, device=dev) * 3 + 0.5
+    i = torch.arange(M, device=dev) % 1024
+    up = ((i >= 256) & (i < 512)).nonzero()[:, 0]
+    x[up] = 1e3 + torch.randn(up.numel(), d, generator=g, device=dev)
+    down = ((i >= 512) & (i < 640)).nonzero()[:, 0]
+    x[down] = -2e3 + torch.randn(down.numel(), d, generator=g, device=dev)
+    r = ((i >= 640) & (i < 896)).nonzero()[:, 0]
+    x[r, (r * 7) % d] *= 50.0                                    # one outlier channel per row
+    x[i >= 896] *= 1e-3
+    return x
+
+
+def _ln_bound(x, gamma, beta, eps):
+    """float64 LayerNorm y of fp32 rows x and the bound on |y_kernel - y| (see test_layernorm_float64_bound):
+    (y, fp32 allowance pre, bound = pre + half an fp16 ulp)."""
+    x64, g64, b64 = x.double(), gamma.double(), beta.double()
+    mu = x64.mean(-1, keepdim=True)
+    xc = x64 - mu
+    sig = torch.sqrt((xc * xc).mean(-1, keepdim=True) + eps)
+    y = xc / sig * g64 + b64
+    pre = (g64.abs() * (16 * 2.0 ** -23 * xc.abs() + 16 * 2.0 ** -24 * x64.abs().mean(-1, keepdim=True)) / sig
+           + 2.0 ** -23 * ((xc / sig * g64).abs() + b64.abs()))
+    return y, pre, pre + 0.5 * _ulp16(y.abs() + pre)
+
+
 @pytest.mark.parametrize("d", [384, 768])
 def test_layernorm_float64_bound(cuda, d):
     """Bound per element: half an fp16 ulp of y, plus |gamma| / sigma times (16 2^-23 |x - mu| for the variance,
@@ -424,12 +452,7 @@ def test_layernorm_float64_bound(cuda, d):
     _l, lib = _lib()
     M = 1024
     g = torch.Generator(device=cuda).manual_seed(d)
-    x = torch.randn(M, d, generator=g, device=cuda) * 3 + 0.5
-    x[256:512] = 1e3 + torch.randn(256, d, generator=g, device=cuda)
-    x[512:640] = -2e3 + torch.randn(128, d, generator=g, device=cuda)
-    r = torch.arange(640, 896, device=cuda)
-    x[r, (r * 7) % d] *= 50.0                                    # one outlier channel per row
-    x[896:] *= 1e-3
+    x = _ln_inputs(M, d, g, cuda)
     gamma = torch.randn(d, generator=g, device=cuda)
     beta = torch.randn(d, generator=g, device=cuda)
     eps = 1e-6
@@ -438,14 +461,7 @@ def test_layernorm_float64_bound(cuda, d):
                                       _l.stream_ptr()), "layernorm")
     torch.cuda.synchronize()
     _assert_guard(buf, M)
-    x64, g64, b64 = x.double(), gamma.double(), beta.double()
-    mu = x64.mean(-1, keepdim=True)
-    xc = x64 - mu
-    sig = torch.sqrt((xc * xc).mean(-1, keepdim=True) + eps)
-    y = xc / sig * g64 + b64
-    pre = (g64.abs() * (16 * 2.0 ** -23 * xc.abs() + 16 * 2.0 ** -24 * x64.abs().mean(-1, keepdim=True)) / sig
-           + 2.0 ** -23 * ((xc / sig * g64).abs() + b64.abs()))
-    bound = pre + 0.5 * _ulp16(y.abs() + pre)
+    y, pre, bound = _ln_bound(x, gamma, beta, eps)
     err = (buf[:M].double() - y).abs()
     ok = err <= bound
     # half an ulp is the rounding of a correct value: report the share of the fp32 allowance used beyond it
