@@ -31,7 +31,7 @@ def needs_build() -> bool:
     if not LIB.is_file():
         return True
     t = LIB.stat().st_mtime
-    deps = [CSRC / s for s in SOURCES] + [CSRC / "common.cuh", CSRC / "kmeans_common.cuh", HERE.parent / "include" / "dss_b200.h", Path(__file__)]
+    deps = [CSRC / s for s in SOURCES] + [CSRC / "common.cuh", CSRC / "gemm_pipeline.cuh", CSRC / "kmeans_common.cuh", HERE.parent / "include" / "dss_b200.h", Path(__file__)]
     return any(d.stat().st_mtime > t for d in deps)
 
 

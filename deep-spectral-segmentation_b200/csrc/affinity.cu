@@ -15,11 +15,6 @@
 
 namespace dss {
 
-int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_rows);
-int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int images, int Nimg, int d, float* Wout, int ldw,
-                     int ncols, const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts,
-                     float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st);
-
 // per-image max |f| (only needed when the features are NOT normalised: they are pre-scaled by a power of two so
 // that fp16 cannot overflow; the scale cancels in W / max(W))
 __global__ void __launch_bounds__(256)

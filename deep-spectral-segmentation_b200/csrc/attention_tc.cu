@@ -15,9 +15,6 @@
 
 namespace dss {
 
-int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_rows);
-int make_tmap_out3d_f16(CUtensorMap* tm, const void* ptr, int images, int rows, int cols);
-
 // one MUFU.EX2 (2 ulp), flushes denormal results to zero; exp2f would add range checks and fix-ups per element
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
@@ -174,7 +171,7 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
     for (int hh = 0; hh < 2; ++hh) {
       const int row = r0 + 8 * hh;
       const float inv = hh ? inv1 : inv0;
-      const uint32_t addr = sQ + row * 128 + ((i ^ (row & 7)) << 4) + (lane & 3) * 4;
+      const uint32_t addr = sw128_addr(sQ, row, i) + (lane & 3) * 4;
       asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_half2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv))
                    : "memory");
     }

@@ -40,6 +40,30 @@ static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; 
 
 int device_sm_count();
 
+// ---------------------------------------------------------------- host functions shared between files
+// TMA tensor maps (gemm.cu): 128 B swizzle, 128-byte-wide boxes
+int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_rows);
+int make_tmap_out(CUtensorMap* tm, const void* ptr, int rows, int cols, int is_f32);
+int make_tmap_out3d_f32(CUtensorMap* tm, const void* ptr, int images, int rows, int ld);
+int make_tmap_out3d_f16(CUtensorMap* tm, const void* ptr, int images, int rows, int cols);
+// persistent wgmma GEMMs (gemm.cu, gemm_ln.cu)
+int gemm_tile_n();
+int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, const float* bias, void* out,
+                int M, int N, int K, int epi, const float* aux, int rin, int rout, cudaStream_t st, int kclass, int bn);
+int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int images, int Nimg, int d, float* Wout, int ldw,
+                     int ncols, const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts,
+                     float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st);
+int gemm_ln_tile_n(int N);
+int gemm_ln_f16_tc(const CUtensorMap& tmB, const CUtensorMap& tmC, const float* x, const float* gamma, const float* beta,
+                   const float* bias, int M, int N, float eps, bool gelu, cudaStream_t st, int kclass);
+// ViT kernels (vit_kernels.cu, attention_tc.cu)
+int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
+int launch_im2col_pad(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
+int launch_cls_attention(const void* qkv, int B, int T, int heads, float* out, cudaStream_t st);
+int launch_cls_row(float* x, const float* cls, const float* pos, int B, int T, int d, cudaStream_t st);
+int launch_layernorm(const float* x, const float* g, const float* b, void* y, int M, int d, float eps, cudaStream_t st);
+int launch_attention_tc(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st);
+
 // ---------------------------------------------------------------- launch accounting / per-class device timing
 enum KernelClass {
   KC_IM2COL = 0, KC_GEMM_PATCH, KC_CLS_ROW, KC_LAYERNORM, KC_GEMM_QKV, KC_ATTENTION, KC_GEMM_PROJ, KC_GEMM_FC1,
@@ -228,6 +252,10 @@ __device__ __forceinline__ void wgmma_fence_acc(float (&d)[R]) {
 // wide) advances K by 16 rows as +2048 B.
 __device__ __forceinline__ uint64_t wgmma_desc_sw128(uint32_t smem_addr) {
   return (static_cast<uint64_t>((smem_addr & 0x3FFFFu) >> 4)) | (1ull << 16) | (64ull << 32) | (1ull << 62);
+}
+// Address of 16-byte chunk `chunk` (0..7) of row `row` of such a tile at `base`: the chunk index is XORed with row % 8.
+__device__ __forceinline__ uint32_t sw128_addr(uint32_t base, int row, int chunk) {
+  return base + row * 128 + ((chunk ^ (row & 7)) << 4);
 }
 // d[i .. i+7] as read-write asm operands
 #define DSS_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \

@@ -23,11 +23,11 @@
 //     runs under the other group's wgmmas. Used by the four ViT epilogues (qkv, proj, fc1, fc2).
 #include <math.h>
 
-#include "common.cuh"
+#include "gemm_pipeline.cuh"
 
 namespace dss {
 
-constexpr int BM = 128, BK = 64, MMA_K = 16;   // BK: one 128-byte swizzle atom of fp16 (one TMA box / 4 wgmma k-steps)
+constexpr int BM = 128;
 constexpr int A_ATOM_BYTES = BM * BK * 2;
 constexpr int CONSUMER_WGS = 2;                 // MMA + epilogue warp groups, each owns 64 rows of the 128-row tile
 constexpr int EPI_THREADS = CONSUMER_WGS * 128;
@@ -35,7 +35,6 @@ constexpr int GEMM_THREADS = 128 + EPI_THREADS; // warp group 0: TMA producer (o
 constexpr int STG_LD = 36;               // manual path staging chunk: 128 rows x 32 cols fp32, row pitch 36
 constexpr int STG_BYTES = BM * STG_LD * 4;
 constexpr int BOX_BYTES = BM * 128;      // TMA-store path staging box: 128 rows x 128 bytes (swizzled)
-constexpr int SMEM_LIMIT = 232448;       // 227 KB of dynamic shared memory per block (sm_90)
 
 // epilogues whose output rows are the GEMM rows: written with TMA (the row-remapping ones keep the manual path)
 constexpr int EPI_AFFINITY_F32 = 100;    // internal epilogue id (not in the public enum): batched patch-affinity tile
@@ -55,7 +54,7 @@ template <int EPI, int BN, bool PP = false> struct TileCfg {
   static constexpr int STAGING_BYTES = PP ? CONSUMER_WGS * 2 * BOX_BYTES
                                      : epi_uses_tma_store(EPI) ? 2 * BOX_BYTES + (EPI == EPI_AFFINITY_F32 ? STG_BYTES : 0)
                                                                : 2 * STG_BYTES;
-  static constexpr int MAX_STAGES = (SMEM_LIMIT - 1024 - 256 - STAGING_BYTES) / STAGE_BYTES;
+  static constexpr int MAX_STAGES = (SMEM_BUDGET - 1024 - 256 - STAGING_BYTES) / STAGE_BYTES;
   static constexpr int STAGES = MAX_STAGES > 6 ? 6 : MAX_STAGES;
   // ring | staging | barriers | alignment slack
   static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + STAGING_BYTES + 256 + 1024;
@@ -96,11 +95,6 @@ struct EpiParams {
 // wgmma retired (wgmma_wait<0>), epilogue issued. tmax = cdiv(work items, clusters) bounds the tiles of one CTA.
 __host__ __device__ constexpr long long trace_stride(int total_items, int clusters) {
   return 4 + 8ll * ((total_items + clusters - 1) / clusters);
-}
-__device__ __forceinline__ unsigned long long globaltimer() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-  return t;
 }
 
 // Row of the output buffer that GEMM row m maps to (or -1: skip).
@@ -186,27 +180,24 @@ __device__ __forceinline__ int frag_row(int wg, int wi, int lane) { return 64 * 
 // slab, the ring position carried across tiles. The whole warp runs the loop with warp-uniform values; one elected
 // lane issues. The slab a slot held is free once one consumer group of EACH CTA has released it (empty barrier).
 template <int BN, int STAGES, int STAGE_BYTES, bool TRACE>
-__device__ __forceinline__ void produce(const CUtensorMap* tmA, const CUtensorMap* tmB, uint32_t base, uint32_t bar_base,
-                                        int num_kb, int cid, int ncl, int rank, int pairs_m, int tiles_n,
-                                        int total_items, const EpiParams& p) {
+__device__ __forceinline__ void produce(const CUtensorMap* tmA, const CUtensorMap* tmB, uint32_t base,
+                                        const RingBars<STAGES>& bars, int num_kb, int cid, int ncl, int rank,
+                                        int pairs_m, int tiles_n, int total_items, const EpiParams& p) {
   constexpr int B_ATOM_BYTES = BN * BK * 2;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
   const int lane = threadIdx.x & 31;
   const uint32_t ubase = __shfl_sync(0xffffffffu, base, 0);
   [[maybe_unused]] unsigned long long waited = 0;
-  int s = 0;
-  uint32_t ph = 0;   // ring position, carried across tiles
+  RingPos<STAGES> pos;   // carried across tiles
   for (int t = cid; t < total_items; t += ncl) {
     const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
     const int row_base = tc.z * p.batch_rows;
     for (int kb = 0; kb < num_kb; ++kb) {
       [[maybe_unused]] unsigned long long t0;
       if constexpr (TRACE) t0 = globaltimer();
-      mbar_wait(empty_bar(s), ph ^ 1u);
+      mbar_wait(bars.empty(pos.slot), pos.phase ^ 1u);
       if constexpr (TRACE) waited += globaltimer() - t0;
-      const uint32_t sa = ubase + s * STAGE_BYTES;
-      const uint32_t fb = full_bar(s);
+      const uint32_t sa = ubase + pos.slot * STAGE_BYTES;
+      const uint32_t fb = bars.full(pos.slot);
       // split-fp16 Gram product: A = [hi | hi/64 | 64 lo], B = [hi | 64 lo | hi/64] are the same array read with the
       // last two groups of K slabs swapped
       int kbB = kb;
@@ -220,7 +211,7 @@ __device__ __forceinline__ void produce(const CUtensorMap* tmA, const CUtensorMa
                        row_base + tc.n0 + rank * (BN / 2), (uint16_t)0x3);
       }
       __syncwarp();
-      if (++s == STAGES) { s = 0; ph ^= 1u; }
+      pos.advance();
     }
   }
   if constexpr (TRACE) {
@@ -242,10 +233,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   const uint32_t base = (raw + 1023u) & ~1023u;
   uint8_t* gbase = smem_raw + (base - raw);
   float* stage_base = reinterpret_cast<float*>(gbase + STAGES * STAGE_BYTES);
-  const uint32_t bar_base = base + STAGES * STAGE_BYTES + Cfg::STAGING_BYTES;
-  // barrier block: full[STAGES] | empty[STAGES]
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  const RingBars<STAGES> bars{base + STAGES * STAGE_BYTES + Cfg::STAGING_BYTES};
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -257,11 +245,8 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     if constexpr (epi_uses_tma_store(EPI)) tma_prefetch_desc(&tmC);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      // released by the MMA warp groups of BOTH CTAs (each CTA's producer writes half of the B slab into the other)
-      mbar_init(empty_bar(s), 2 * CONSUMER_WGS);
-    }
+    // released by the MMA warp groups of BOTH CTAs (each CTA's producer writes half of the B slab into the other)
+    bars.init(2 * CONSUMER_WGS);
     mbar_fence_init();
   }
   __syncthreads();
@@ -270,7 +255,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
   if (warp < 4) {
     setmaxnreg_dec<40>();
     if (warp == 0)
-      produce<BN, STAGES, STAGE_BYTES, TRACE>(&tmA, &tmB, base, bar_base, num_kb, cid, ncl, rank, pairs_m, tiles_n,
+      produce<BN, STAGES, STAGE_BYTES, TRACE>(&tmA, &tmB, base, bars, num_kb, cid, ncl, rank, pairs_m, tiles_n,
                                               total_items, p);
   } else {
     setmaxnreg_inc<232>();
@@ -280,47 +265,34 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     const int fc = 2 * (lane & 3);                  // column of this thread inside an 8-column block
     const uint32_t stage_u32 = base + STAGES * STAGE_BYTES;
     const bool issuer = ct == 0;
-    int s = 0, cc = 0;
-    uint32_t ph = 0;
+    RingPos<STAGES> pos;
+    int cc = 0;
     float acc[BN / 2];
     [[maybe_unused]] float aff_rowsum[2] = {0.f, 0.f};   // affinity: row sums of this thread's two column slices
     [[maybe_unused]] float aff_mx = 1.f, aff_rmx = 1.f, aff_unscale = 1.f;
     [[maybe_unused]] unsigned long long* trec = nullptr;   // traced: this group's record of the current tile
     if constexpr (TRACE) trec = p.trace + blockIdx.x * trace_stride(total_items, ncl) + 4 + 4 * wg * ((total_items + ncl - 1) / ncl);
     const bool tracer = TRACE && (ct & 127) == 0;
+    const NamedBar<1, EPI_THREADS> epi_bar;
+    // each group computes 64 rows of the tile against the whole B slab
+    auto mma = [&](int s, int kb) {
+      const uint32_t sa = base + s * STAGE_BYTES;
+      mma_slab<BN>(acc, wgmma_desc_sw128(sa + wg * 64 * 128), wgmma_desc_sw128(sa + A_ATOM_BYTES), kb == 0);
+    };
+    auto release = [&](int s) {
+      if ((ct & 127) == 0) {
+        mbar_arrive_cluster(bars.empty(s), 0);
+        mbar_arrive_cluster(bars.empty(s), 1);
+      }
+    };
     for (int t = cid; t < total_items; t += ncl) {
       const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
       if (tracer) trec[0] = globaltimer();
-      // ---- main loop: 4 wgmma k-steps per 64-deep slab; a slab is released (in both CTAs) once the wgmmas of the
-      // NEXT slab have been issued and the older group has retired
-      int prev = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(full_bar(s), ph);
-        if (tracer && kb == 0) trec[1] = globaltimer();
-        __syncwarp();   // wgmma is warp-aligned: reconverge after the per-thread barrier spin
-        const uint32_t sa = base + s * STAGE_BYTES;
-        const uint64_t adesc = wgmma_desc_sw128(sa + wg * 64 * 128);
-        const uint64_t bdesc = wgmma_desc_sw128(sa + A_ATOM_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / MMA_K; ++k)
-          Wgmma<BN>::ss(acc, adesc + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (prev >= 0 && (ct & 127) == 0) {
-          mbar_arrive_cluster(empty_bar(prev), 0);
-          mbar_arrive_cluster(empty_bar(prev), 1);
-        }
-        prev = s;
-        if (++s == STAGES) { s = 0; ph ^= 1u; }
-      }
+      const int last = consume_slabs(pos, bars, num_kb, tracer ? trec + 1 : nullptr, mma, release);
       wgmma_wait<0>();
       wgmma_fence_acc(acc);
       if (tracer) trec[2] = globaltimer();
-      if ((ct & 127) == 0) {
-        mbar_arrive_cluster(empty_bar(prev), 0);
-        mbar_arrive_cluster(empty_bar(prev), 1);
-      }
+      release(last);
 
       if constexpr (epi_uses_tma_store(EPI)) {
         // ---- 128-byte-wide output boxes (32 fp32 or 64 fp16 columns): fragments -> +bias (-> GELU) -> 128 B-swizzled
@@ -337,10 +309,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         for (int b = 0; b < NBOX; ++b) {
           const int nc = tc.n0 + b * BOXC;           // first global column of the box
           const bool live = nc < N;
-          // the staging box is free once the store issued two boxes ago has finished READING it
-          if (issuer) tma_store_wait_read<1>();
-          __syncwarp();
-          asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+          box_acquire(epi_bar, issuer);
           const uint32_t sbuf = stage_u32 + (cc & 1) * BOX_BYTES;
           if constexpr (EPI != EPI_AFFINITY_F32) {
 #pragma unroll
@@ -351,17 +320,9 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
               if (p.bias != nullptr && col < N) bv = __ldg(reinterpret_cast<const float2*>(p.bias + col));
 #pragma unroll
               for (int h = 0; h < 2; ++h) {
-                const int row = fr + 8 * h;
                 float x0 = acc[4 * ci + 2 * h] + bv.x, x1 = acc[4 * ci + 2 * h + 1] + bv.y;
                 if constexpr (EPI == DSS_EPI_BIAS_GELU_F16) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
-                if constexpr (OUT16) {
-                  const uint32_t addr = sbuf + row * 128 + ((i ^ (row & 7)) << 4) + (lane & 3) * 4;
-                  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_half2(x0, x1)) : "memory");
-                } else {
-                  const int j = 2 * i + ((lane & 3) >> 1);
-                  const uint32_t addr = sbuf + row * 128 + ((j ^ (row & 7)) << 4) + (lane & 1) * 8;
-                  asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x0), "f"(x1) : "memory");
-                }
+                box_put_pair<OUT16>(sbuf, fr + 8 * h, i, lane, x0, x1);
               }
             }
           } else {
@@ -377,8 +338,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                 *reinterpret_cast<float2*>(rowbuf + (fr + 8 * h) * STG_LD + 8 * i + fc) =
                     make_float2(acc[4 * ci + 2 * h], acc[4 * ci + 2 * h + 1]);
             }
-            __syncwarp();
-            asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+            epi_bar.sync();
             const int q = (ct >> 5) & 3, sp = ct >> 7;
             const int row = q * 32 + lane;
             const int m = tc.m0 + row;
@@ -503,26 +463,21 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
                   part[(long long)(4 * tiles_n + (tc.m0 / BM) * 4 + q) * p.ld_part + n + e] = c1;
                 }
               }
-              const uint32_t srow = sbuf + row * 128;
 #pragma unroll
               for (int h = 0; h < 2; ++h) {   // two 16-byte chunks per slice
                 const int j = sl * 2 + h;
-                asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(srow + ((j ^ (row & 7)) << 4)),
+                asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(sw128_addr(sbuf, row, j)),
                              "f"(x[h * 4 + 0]), "f"(x[h * 4 + 1]), "f"(x[h * 4 + 2]), "f"(x[h * 4 + 3])
                              : "memory");
               }
             }
             // diagonal tiles of the symmetric mode store directly (above) and skip the staging box
             if (p.tri && !upper) {
-              __syncwarp();
-              asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");   // row-major copy reused by the next box
+              epi_bar.sync();   // row-major copy reused by the next box
               continue;
             }
           }
-          fence_proxy_async_smem();   // generic-proxy smem writes -> visible to the TMA (async proxy)
-          __syncwarp();
-          asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
-          if (issuer) {
+          box_issue(epi_bar, issuer, [&, tc] {
             if (live) {
               if constexpr (EPI == DSS_EPI_BIAS_RESID_F32)
                 tma_reduce_add_2d(&tmC, sbuf, nc, tc.m0);
@@ -531,8 +486,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
               else
                 tma_store_2d(&tmC, sbuf, nc, tc.m0);
             }
-            tma_store_commit();
-          }
+          });
           ++cc;   // (boxes that skip the staging buffers -- diagonal affinity tiles -- do not advance the buffer parity)
         }
         if (tracer) {
@@ -559,8 +513,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
           }
           // Double-buffered staging: one barrier per chunk is enough, because a thread reaches the barrier of chunk c
           // only after finishing phase 2 of the previous user of buffer c^1.
-          __syncwarp();
-          asm volatile("bar.sync 1, %0;" ::"n"(EPI_THREADS) : "memory");
+          epi_bar.sync();
           // Phase 2: 8 lanes x 16 B cover the 128 B of one row of the chunk, 4 rows per warp instruction
           if (nc < N) {
             const int cw = ct >> 5;
@@ -594,9 +547,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
       if (issuer) tma_store_wait_all<0>();
     }
   }
-  __syncwarp();
-  __syncthreads();
-  cluster_sync_all();   // the peer may still multicast / arrive into this CTA's shared memory until it is done too
+  cluster_pair_exit();
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -622,9 +573,7 @@ gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw = smem_u32(smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;   // SWIZZLE_128B alignment
-  const uint32_t bar_base = base + STAGES * STAGE_BYTES + Cfg::STAGING_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
+  const RingBars<STAGES> bars{base + STAGES * STAGE_BYTES + Cfg::STAGING_BYTES};
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -636,10 +585,7 @@ gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     tma_prefetch_desc(&tmC);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 2);   // one consumer group of each CTA
-    }
+    bars.init(2);   // one consumer group of each CTA
     mbar_fence_init();
   }
   __syncthreads();
@@ -648,7 +594,7 @@ gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
   if (warp < 4) {
     setmaxnreg_dec<40>();
     if (warp == 0)
-      produce<BN, STAGES, STAGE_BYTES, TRACE>(&tmA, &tmB, base, bar_base, num_kb, cid, ncl, rank, pairs_m, tiles_n,
+      produce<BN, STAGES, STAGE_BYTES, TRACE>(&tmA, &tmB, base, bars, num_kb, cid, ncl, rank, pairs_m, tiles_n,
                                               total_items, p);
   } else {
     setmaxnreg_inc<232>();
@@ -657,16 +603,25 @@ gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
     const int fc = 2 * (lane & 3);
     const bool issuer = (ct & 127) == 0;   // issues this group's stores and releases its slabs
     const uint32_t stage_u32 = base + STAGES * STAGE_BYTES + wg * 2 * BOX_BYTES;   // this group's two boxes
-    int s = 0, cc = 0;
-    uint32_t ph = 0;
-    if (wg == 1) {   // the ring position of item 1: item 0's slabs come first
-      s = num_kb % STAGES;
-      ph = (num_kb / STAGES) & 1;
-    }
+    RingPos<STAGES> pos;
+    int cc = 0;
+    if (wg == 1) pos.skip(num_kb);   // the ring position of item 1: item 0's slabs come first
     float acc[2][64];   // rows 0-63 and 64-127 of the tile
     [[maybe_unused]] unsigned long long* trec = nullptr;
     if constexpr (TRACE) trec = p.trace + blockIdx.x * trace_stride(total_items, ncl) + 4 + 4 * wg * ((total_items + ncl - 1) / ncl);
     const bool tracer = TRACE && issuer;
+    const GroupBar<128> epi_bar{PP_EPI_BAR + wg};
+    auto mma = [&](int s, int kb) {
+      const uint32_t sa = base + s * STAGE_BYTES;
+      mma_slab<BN, 2>(acc, {wgmma_desc_sw128(sa), wgmma_desc_sw128(sa + 64 * 128)}, wgmma_desc_sw128(sa + A_ATOM_BYTES),
+                      kb == 0);
+    };
+    auto release = [&](int s) {
+      if ((ct & 127) == 0) {
+        mbar_arrive_cluster_relaxed(bars.empty(s), 0);
+        mbar_arrive_cluster_relaxed(bars.empty(s), 1);
+      }
+    };
     for (int t = cid + wg * ncl; t < total_items; t += 2 * ncl) {
       if (t != cid) {   // wait for the MMA turn
         __syncwarp();
@@ -674,29 +629,7 @@ gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
       }
       const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank);
       if (tracer) trec[0] = globaltimer();
-      int prev = -1;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(full_bar(s), ph);
-        if (tracer && kb == 0) trec[1] = globaltimer();
-        __syncwarp();   // wgmma is warp-aligned: reconverge after the per-thread barrier spin
-        const uint32_t sa = base + s * STAGE_BYTES;
-        const uint64_t adesc0 = wgmma_desc_sw128(sa), adesc1 = wgmma_desc_sw128(sa + 64 * 128);
-        const uint64_t bdesc = wgmma_desc_sw128(sa + A_ATOM_BYTES);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < BK / MMA_K; ++k) {
-          Wgmma<BN>::ss(acc[0], adesc0 + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
-          Wgmma<BN>::ss(acc[1], adesc1 + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
-        }
-        wgmma_commit();
-        wgmma_wait<1>();
-        if (prev >= 0 && issuer) {
-          mbar_arrive_cluster_relaxed(empty_bar(prev), 0);
-          mbar_arrive_cluster_relaxed(empty_bar(prev), 1);
-        }
-        prev = s;
-        if (++s == STAGES) { s = 0; ph ^= 1u; }
-      }
+      const int last = consume_slabs(pos, bars, num_kb, tracer ? trec + 1 : nullptr, mma, release);
       // hand the MMA turn to the group of the next item (its wgmmas queue behind this tile's last ones)
       if (t + ncl < total_items) {
         __syncwarp();
@@ -706,14 +639,8 @@ gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
       wgmma_fence_acc(acc[0]);
       wgmma_fence_acc(acc[1]);
       if (tracer) trec[2] = globaltimer();
-      if (issuer) {
-        mbar_arrive_cluster_relaxed(empty_bar(prev), 0);
-        mbar_arrive_cluster_relaxed(empty_bar(prev), 1);
-      }
-      // skip the other group's item in the ring
-      s += num_kb % STAGES;
-      ph ^= (num_kb / STAGES) & 1;
-      if (s >= STAGES) { s -= STAGES; ph ^= 1u; }
+      release(last);
+      pos.skip(num_kb);   // the other group's item
 
       // ---- epilogue, as in the cooperative kernel but on this group's 128 rows and boxes: +bias (-> GELU) -> 128 B-
       // swizzled staging box -> TMA store / reduce-add
@@ -723,10 +650,7 @@ gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
 #pragma unroll
       for (int b = 0; b < NBOX; ++b) {
         const int nc = tc.n0 + b * BOXC;
-        // the box is free once the store this group issued two boxes ago has finished READING it
-        if (issuer) tma_store_wait_read<1>();
-        __syncwarp();
-        asm volatile("bar.sync %0, 128;" ::"r"(PP_EPI_BAR + wg) : "memory");
+        box_acquire(epi_bar, issuer);
         const uint32_t sbuf = stage_u32 + (cc & 1) * BOX_BYTES;
 #pragma unroll
         for (int i = 0; i < BOXC / 8; ++i) {
@@ -743,28 +667,17 @@ gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
             // instead of values let the registers serve the rest of this epilogue
             acc[h][4 * ci + 2 * e] = acc[h][4 * ci + 2 * e + 1] = 0.f;
             if constexpr (EPI == DSS_EPI_BIAS_GELU_F16) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
-            if constexpr (OUT16) {
-              const uint32_t addr = sbuf + row * 128 + ((i ^ (row & 7)) << 4) + (lane & 3) * 4;
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_half2(x0, x1)) : "memory");
-            } else {
-              const int j = 2 * i + ((lane & 3) >> 1);
-              const uint32_t addr = sbuf + row * 128 + ((j ^ (row & 7)) << 4) + (lane & 1) * 8;
-              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(addr), "f"(x0), "f"(x1) : "memory");
-            }
+            box_put_pair<OUT16>(sbuf, row, i, lane, x0, x1);
           }
         }
-        fence_proxy_async_smem();   // generic-proxy smem writes -> visible to the TMA (async proxy)
-        __syncwarp();
-        asm volatile("bar.sync %0, 128;" ::"r"(PP_EPI_BAR + wg) : "memory");
-        if (issuer) {
+        box_issue(epi_bar, issuer, [&] {
           if (nc < N) {
             if constexpr (EPI == DSS_EPI_BIAS_RESID_F32)
               tma_reduce_add_2d(&tmC, sbuf, nc, tc.m0);
             else
               tma_store_2d(&tmC, sbuf, nc, tc.m0);
           }
-          tma_store_commit();
-        }
+        });
         ++cc;
       }
       if (tracer) {
@@ -774,9 +687,7 @@ gemm_f16_pingpong_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
     }
     if (issuer) tma_store_wait_all<0>();
   }
-  __syncwarp();
-  __syncthreads();
-  cluster_sync_all();   // the peer may still multicast / arrive into this CTA's shared memory until it is done too
+  cluster_pair_exit();
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -821,6 +732,27 @@ static PFN_encodeTiled get_encode_fn() {
   return fn;
 }
 
+// Tiled tensor map of `rank` dimensions (innermost first) with the settings all of them share: dense, 128 B swizzle,
+// 256 B L2 promotion, zero fill out of bounds. `what` names the map in the error message; a 2D map's message also
+// gives its rows and columns.
+static int encode_tmap(CUtensorMap* tm, CUtensorMapDataType dtype, cuuint32_t rank, const void* ptr,
+                       const cuuint64_t* gdim, const cuuint64_t* gstride, const cuuint32_t* box, const char* what) {
+  PFN_encodeTiled enc = get_encode_fn();
+  if (!enc) return DSS_ERR_CUDA;
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = enc(tm, dtype, rank, const_cast<void*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    if (rank == 2)
+      set_error("cuTensorMapEncodeTiled%s failed with CUresult %d (rows=%d cols=%d)", what, (int)r, (int)gdim[1],
+                (int)gdim[0]);
+    else
+      set_error("cuTensorMapEncodeTiled%s failed with CUresult %d", what, (int)r);
+    return DSS_ERR_CUDA;
+  }
+  return DSS_OK;
+}
+
 // Tile width the weight tensor maps of the TMA-store epilogues (the ping-pong schedule) are built for.
 int gemm_tile_n() { return PP_BN; }
 
@@ -830,91 +762,49 @@ static int coop_tile_n(int N) { return N % 256 == 0 ? 256 : (N % 192 == 0 ? 192 
 
 // 2D fp16 row-major [rows, cols] tensor, box = 64 columns x box_rows rows, 128 B swizzle, zero fill out of bounds.
 int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_rows) {
-  PFN_encodeTiled enc = get_encode_fn();
-  if (!enc) return DSS_ERR_CUDA;
+  if (!get_encode_fn()) return DSS_ERR_CUDA;
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "TMA operand must be 16-byte aligned");
   DSS_REQUIRE(cols % 8 == 0, "TMA operand row pitch must be a multiple of 16 bytes (cols=%d)", cols);
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t gstride[1] = {(cuuint64_t)cols * 2};
   DSS_REQUIRE(box_rows > 0 && box_rows <= 256, "TMA box rows must be in [1, 256]");
   cuuint32_t box[2] = {(cuuint32_t)BK, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed with CUresult %d (rows=%d cols=%d)", (int)r, rows, cols);
-    return DSS_ERR_CUDA;
-  }
-  return DSS_OK;
+  return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, gdim, gstride, box, "");
 }
 
 // Output tensor map for the TMA-store epilogues: row-major [rows, cols] of fp16 (box 64 x 128) or fp32 (box 32 x 128),
 // i.e. 128-byte-wide boxes with the 128 B swizzle.
 int make_tmap_out(CUtensorMap* tm, const void* ptr, int rows, int cols, int is_f32) {
-  PFN_encodeTiled enc = get_encode_fn();
-  if (!enc) return DSS_ERR_CUDA;
+  if (!get_encode_fn()) return DSS_ERR_CUDA;
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0, "TMA output must be 16-byte aligned");
   const int esz = is_f32 ? 4 : 2;
   DSS_REQUIRE((cols * esz) % 16 == 0, "TMA output row pitch must be a multiple of 16 bytes (cols=%d)", cols);
   cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   cuuint64_t gstride[1] = {(cuuint64_t)cols * esz};
   cuuint32_t box[2] = {(cuuint32_t)(is_f32 ? 32 : 64), (cuuint32_t)BM};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = enc(tm, is_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
-                   const_cast<void*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled (output) failed with CUresult %d (rows=%d cols=%d)", (int)r, rows, cols);
-    return DSS_ERR_CUDA;
-  }
-  return DSS_OK;
+  return encode_tmap(tm, is_f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, ptr, gdim,
+                     gstride, box, " (output)");
 }
 
 // Per-image fp32 output [images, rows, ld] for the affinity epilogue: 3D map, box 32 columns x 128 rows x 1 image
 int make_tmap_out3d_f32(CUtensorMap* tm, const void* ptr, int images, int rows, int ld) {
-  PFN_encodeTiled enc = get_encode_fn();
-  if (!enc) return DSS_ERR_CUDA;
+  if (!get_encode_fn()) return DSS_ERR_CUDA;
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && ld % 4 == 0, "affinity output must be 16-byte aligned / pitched");
   cuuint64_t gdim[3] = {(cuuint64_t)ld, (cuuint64_t)rows, (cuuint64_t)images};
   cuuint64_t gstride[2] = {(cuuint64_t)ld * 4, (cuuint64_t)rows * ld * 4};
   cuuint32_t box[3] = {32, (cuuint32_t)BM, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled (3D output) failed with CUresult %d", (int)r);
-    return DSS_ERR_CUDA;
-  }
-  return DSS_OK;
+  return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, ptr, gdim, gstride, box, " (3D output)");
 }
 
 // 3D fp16 output [images, rows, cols] written in 128-row x 64-column boxes (128 B swizzle); rows past `rows` of an image
 // are clipped by the TMA unit, so a partial last tile never spills into the next image.
 int make_tmap_out3d_f16(CUtensorMap* tm, const void* ptr, int images, int rows, int cols) {
-  PFN_encodeTiled enc = get_encode_fn();
-  if (!enc) return DSS_ERR_CUDA;
+  if (!get_encode_fn()) return DSS_ERR_CUDA;
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ptr) & 15) == 0 && cols % 64 == 0, "fp16 tile output must be 16-byte aligned, cols %% 64 == 0");
   cuuint64_t gdim[3] = {(cuuint64_t)cols, (cuuint64_t)rows, (cuuint64_t)images};
   cuuint64_t gstride[2] = {(cuuint64_t)cols * 2, (cuuint64_t)rows * cols * 2};
   cuuint32_t box[3] = {64, (cuuint32_t)BM, 1};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(ptr), gdim, gstride, box, estr,
-                   CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                   CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled (3D fp16 output) failed with CUresult %d", (int)r);
-    return DSS_ERR_CUDA;
-  }
-  return DSS_OK;
-}
-
-// CTA pairs of a persistent launch over `items` work items: one CTA per SM
-static int gemm_clusters(int items) {
-  int sms = device_sm_count();
-  if (sms <= 0) sms = 132;
-  return items < sms / 2 ? items : sms / 2;
+  return encode_tmap(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, ptr, gdim, gstride, box, " (3D fp16 output)");
 }
 
 // PP: ping-pong schedule (BN == PP_BN), else cooperative; TRACE: the phase-traced instantiation (p.trace)
@@ -922,16 +812,10 @@ template <int EPI, int BN, bool PP = false, bool TRACE = false>
 static int launch_tc_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, int M, int N, int K,
                         const EpiParams& p, cudaStream_t st, int kclass, int batch) {
   static_assert(!PP || BN == PP_BN, "ping-pong tile width");
-  using Cfg = TileCfg<EPI, BN, PP>;
   constexpr auto kernel = [] {
     if constexpr (PP) return gemm_f16_pingpong_kernel<EPI, TRACE>;
     else return gemm_f16_wgmma_kernel<EPI, BN, TRACE>;
   }();
-  static bool attr_set = false;
-  if (!attr_set) {
-    DSS_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    attr_set = true;
-  }
   const int pairs_m = cdiv(cdiv(M, BM), 2), tiles_n = cdiv(N, BN);
   int per_img = pairs_m * tiles_n;
   if (p.tri) {   // symmetric output: row pair p visits the n-tiles j >= 2p only (see decode_tile)
@@ -939,27 +823,13 @@ static int launch_tc_bn(const CUtensorMap& tmA, const CUtensorMap& tmB, const CU
     for (int q = 0; q < pairs_m; ++q) per_img += tiles_n - 2 * q > 0 ? tiles_n - 2 * q : 0;
   }
   const int total = per_img * batch;   // work items of a CTA pair
-  const int clusters = gemm_clusters(total);
   if (epi_uses_tma_store(EPI) && tmC == nullptr) {
     set_error("gemm: this epilogue needs an output tensor map");
     return DSS_ERR_BAD_ARG;
   }
-  LaunchScope scope(st, kclass);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  DSS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kernel, tmA, tmB, tmC ? *tmC : tmA, M, N, K, pairs_m, tiles_n, total, p));
-  DSS_CHECK_CUDA(cudaGetLastError());
-  return DSS_OK;
+  return launch_cluster_pairs<kernel, TileCfg<EPI, BN, PP>::SMEM_BYTES>(gemm_clusters(total), GEMM_THREADS, st, kclass,
+                                                                        tmA, tmB, tmC ? *tmC : tmA, M, N, K, pairs_m,
+                                                                        tiles_n, total, p);
 }
 
 // Cooperative schedule; bn = tile width the B tensor map was built for (its TMA box has bn / 2 rows)

@@ -17,14 +17,11 @@
 // the A operand is bit for bit the stand-alone kernel's output.
 #include <math.h>
 
-#include "common.cuh"
+#include "gemm_pipeline.cuh"
 
 namespace dss {
 
-int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_rows);
-int make_tmap_out(CUtensorMap* tm, const void* ptr, int rows, int cols, int is_f32);
-
-constexpr int LG_BM = 128, LG_K = 384, LG_SLABS = LG_K / 64, LG_SLAB_BYTES = LG_BM * 128;
+constexpr int LG_BM = 128, LG_K = 384, LG_SLABS = LG_K / BK, LG_SLAB_BYTES = LG_BM * 128;
 constexpr int LG_THREADS = 384, LG_LN_WARPS = 3;
 constexpr int LG_BOX_BYTES = LG_BM * 128;
 
@@ -34,9 +31,9 @@ template <int BN> struct LnCfg {
   static constexpr int STAGING = 2 * LG_BOX_BYTES;
   static constexpr int VEC_BYTES = 2 * LG_BM * 4;                   // row sum[128], rstd[128]
   static constexpr int FIXED = A_BYTES + STAGING + VEC_BYTES + 256 + 1024;
-  static constexpr int STAGES = (232448 - FIXED) / B_STAGE > 6 ? 6 : (232448 - FIXED) / B_STAGE;
+  static constexpr int STAGES = (SMEM_BUDGET - FIXED) / B_STAGE > 6 ? 6 : (SMEM_BUDGET - FIXED) / B_STAGE;
   static constexpr int SMEM = FIXED + STAGES * B_STAGE;
-  static_assert(STAGES >= 2 && SMEM <= 232448, "shared memory budget");
+  static_assert(STAGES >= 2 && SMEM <= SMEM_BUDGET, "shared memory budget");
   static_assert((B_STAGE / 2) % 1024 == 0, "half tiles must keep the 1024 B swizzle-atom alignment");
 };
 
@@ -62,10 +59,8 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
   const uint32_t sA = base, sB = base + Cfg::A_BYTES, sOut = sB + STAGES * Cfg::B_STAGE;
   float* s_sum = reinterpret_cast<float*>(gbase + Cfg::A_BYTES + STAGES * Cfg::B_STAGE + Cfg::STAGING);
   float* s_rstd = s_sum + LG_BM;
-  const uint32_t bar_base = sOut + Cfg::STAGING + Cfg::VEC_BYTES;
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t a_full = bar_base + 8u * (2 * STAGES), a_empty = a_full + 8u;
+  const RingBars<STAGES> bars{sOut + Cfg::STAGING + Cfg::VEC_BYTES};
+  const uint32_t a_full = bars.base + 8u * (2 * STAGES), a_empty = a_full + 8u;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int rank = (int)cluster_ctarank();
@@ -75,10 +70,7 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmB);
     tma_prefetch_desc(&tmC);
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 4);   // the two MMA warp groups of both CTAs
-    }
+    bars.init(4);   // the two MMA warp groups of both CTAs
     mbar_init(a_full, LG_LN_WARPS);
     mbar_init(a_empty, 2);
     mbar_fence_init();
@@ -90,19 +82,19 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
     setmaxnreg_dec<56>();
     if (warp == 0) {
       const uint32_t ub = __shfl_sync(0xffffffffu, sB, 0);
-      int s = 0;
-      uint32_t ph = 0;
+      RingPos<STAGES> pos;
       for (int u = cid; u < units; u += ncl)
         for (int nt = 0; nt < tiles_n; ++nt)
           for (int kb = 0; kb < LG_SLABS; ++kb) {
-            mbar_wait(empty_bar(s), ph ^ 1u);
+            const int s = pos.slot;
+            mbar_wait(bars.empty(s), pos.phase ^ 1u);
             if (elect_one()) {
-              mbar_arrive_expect_tx(full_bar(s), Cfg::B_STAGE);
-              tma_load_2d_mc(ub + s * Cfg::B_STAGE + rank * (Cfg::B_STAGE / 2), &tmB, full_bar(s), kb * 64,
+              mbar_arrive_expect_tx(bars.full(s), Cfg::B_STAGE);
+              tma_load_2d_mc(ub + s * Cfg::B_STAGE + rank * (Cfg::B_STAGE / 2), &tmB, bars.full(s), kb * BK,
                              nt * BN + rank * (BN / 2), (uint16_t)0x3);
             }
             __syncwarp();
-            if (++s == STAGES) { s = 0; ph ^= 1u; }
+            pos.advance();
           }
     } else {
       // ---- LayerNorm producers: warp w handles rows w-1, w+2, ... of the block
@@ -150,7 +142,7 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
               const float4 bt = __ldg(reinterpret_cast<const float4*>(p.beta) + lane + 32 * i);
               o = ln_out4(ln_center4(v, S, 1.0f / LG_K), rstd, g, bt);
             }
-            const uint32_t addr = sA + (c >> 6) * LG_SLAB_BYTES + r * 128 + ((((c & 63) >> 3) ^ (r & 7)) << 4) + (c & 7) * 2;
+            const uint32_t addr = sw128_addr(sA + (c >> 6) * LG_SLAB_BYTES, r, (c & 63) >> 3) + (c & 7) * 2;
             asm volatile("st.shared.v2.b32 [%0], {%1, %2};" ::"r"(addr), "r"(o.x), "r"(o.y) : "memory");
           }
         }
@@ -166,45 +158,36 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
     const int wg = ct >> 7, wi = (ct >> 5) & 3;
     const int fr = 64 * wg + 16 * wi + (lane >> 2), fc = 2 * (lane & 3);
     const bool issuer = ct == 0;
-    int s = 0, cc = 0, lu = 0;
-    uint32_t ph = 0;
+    const NamedBar<1, 256> epi_bar;
+    RingPos<STAGES> pos;
+    int cc = 0, lu = 0;
     float acc[BN / 2];
+    auto mma = [&](int s, int kb) {
+      mma_slab<BN>(acc, wgmma_desc_sw128(sA + kb * LG_SLAB_BYTES + wg * 64 * 128), wgmma_desc_sw128(sB + s * Cfg::B_STAGE),
+                   kb == 0);
+    };
+    auto release = [&](int s) {
+      mbar_arrive_cluster(bars.empty(s), 0);
+      mbar_arrive_cluster(bars.empty(s), 1);
+    };
     for (int u = cid; u < units; u += ncl, ++lu) {
       const int m0 = (2 * u + rank) * LG_BM;
       mbar_wait(a_full, lu & 1);
       for (int nt = 0; nt < tiles_n; ++nt) {
-        int prev = -1;
-        for (int kb = 0; kb < LG_SLABS; ++kb) {
-          mbar_wait(full_bar(s), ph);
-          __syncwarp();   // wgmma is warp-aligned: reconverge after the per-thread barrier spin
-          const uint64_t adesc = wgmma_desc_sw128(sA + kb * LG_SLAB_BYTES + wg * 64 * 128);
-          const uint64_t bdesc = wgmma_desc_sw128(sB + s * Cfg::B_STAGE);
-          wgmma_fence();
-#pragma unroll
-          for (int k = 0; k < 4; ++k) Wgmma<BN>::ss(acc, adesc + 2u * k, bdesc + 2u * k, (kb | k) != 0 ? 1u : 0u);
-          wgmma_commit();
-          wgmma_wait<1>();
-          if (prev >= 0 && (ct & 127) == 0) {
-            mbar_arrive_cluster(empty_bar(prev), 0);
-            mbar_arrive_cluster(empty_bar(prev), 1);
-          }
-          prev = s;
-          if (++s == STAGES) { s = 0; ph ^= 1u; }
-        }
+        const int last = consume_slabs(pos, bars, LG_SLABS, nullptr, mma, [&](int s) {
+          if ((ct & 127) == 0) release(s);
+        });
         wgmma_wait<0>();
         wgmma_fence_acc(acc);
         if ((ct & 127) == 0) {
-          mbar_arrive_cluster(empty_bar(prev), 0);
-          mbar_arrive_cluster(empty_bar(prev), 1);
+          release(last);
           if (nt == tiles_n - 1) mbar_arrive(a_empty);   // last reader of the panel: the next block may overwrite it
         }
         // ---- epilogue: 64-column boxes, fragments -> +bias (-> GELU) -> fp16 -> swizzled staging box -> TMA store
 #pragma unroll
         for (int b = 0; b < BN / 64; ++b) {
           const int nc = nt * BN + b * 64;
-          if (issuer) tma_store_wait_read<1>();
-          __syncwarp();
-          asm volatile("bar.sync 1, %0;" ::"n"(256) : "memory");
+          box_acquire(epi_bar, issuer);
           const uint32_t sbuf = sOut + (cc & 1) * LG_BOX_BYTES;
 #pragma unroll
           for (int i = 0; i < 8; ++i) {
@@ -212,60 +195,26 @@ gemm_ln_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_c
             const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + nc + 8 * i + fc));
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              const int row = fr + 8 * h;
               float x0 = acc[4 * ci + 2 * h] + bv.x, x1 = acc[4 * ci + 2 * h + 1] + bv.y;
               if constexpr (GELU) { x0 = gelu_erf(x0); x1 = gelu_erf(x1); }
-              const uint32_t addr = sbuf + row * 128 + ((i ^ (row & 7)) << 4) + (lane & 3) * 4;
-              asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(pack_half2(x0, x1)) : "memory");
+              box_put_pair<true>(sbuf, fr + 8 * h, i, lane, x0, x1);
             }
           }
-          fence_proxy_async_smem();
-          __syncwarp();
-          asm volatile("bar.sync 1, %0;" ::"n"(256) : "memory");
-          if (issuer) {
-            tma_store_2d(&tmC, sbuf, nc, m0);
-            tma_store_commit();
-          }
+          box_issue(epi_bar, issuer, [&] { tma_store_2d(&tmC, sbuf, nc, m0); });
           ++cc;
         }
       }
     }
     if (issuer) tma_store_wait_all<0>();
   }
-  __syncwarp();
-  __syncthreads();
-  cluster_sync_all();   // the peer may still multicast / arrive into this CTA's shared memory until it is done too
+  cluster_pair_exit();
 }
 
 template <bool GELU, int BN>
 static int launch_ln(const CUtensorMap& tmB, const CUtensorMap& tmC, const LnParams& p, cudaStream_t st, int kclass) {
-  using Cfg = LnCfg<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    DSS_CHECK_CUDA(cudaFuncSetAttribute(gemm_ln_f16_wgmma_kernel<GELU, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                        Cfg::SMEM));
-    attr_set = true;
-  }
   const int units = cdiv(cdiv(p.M, LG_BM), 2);   // pairs of row blocks
-  int sms = device_sm_count();
-  if (sms <= 0) sms = 132;
-  const int clusters = units < sms / 2 ? units : sms / 2;
-  LaunchScope scope(st, kclass);
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(2 * clusters);
-  cfg.blockDim = dim3(LG_THREADS);
-  cfg.dynamicSmemBytes = Cfg::SMEM;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 2;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  DSS_CHECK_CUDA(cudaLaunchKernelEx(&cfg, gemm_ln_f16_wgmma_kernel<GELU, BN>, tmB, tmC, units, p));
-  DSS_CHECK_CUDA(cudaGetLastError());
-  return DSS_OK;
+  return launch_cluster_pairs<gemm_ln_f16_wgmma_kernel<GELU, BN>, LnCfg<BN>::SMEM>(gemm_clusters(units), LG_THREADS, st,
+                                                                                  kclass, tmB, tmC, units, p);
 }
 
 // tile width of the fused kernel for an N-column layer (0: not supported)

@@ -19,21 +19,6 @@
 
 namespace dss {
 
-int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_rows);
-int gemm_tile_n();
-int make_tmap_out(CUtensorMap* tm, const void* ptr, int rows, int cols, int is_f32);
-int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, const float* bias, void* out,
-                int M, int N, int K, int epi, const float* aux, int rin, int rout, cudaStream_t st, int kclass, int bn);
-int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
-int launch_im2col_pad(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
-int launch_cls_attention(const void* qkv, int B, int T, int heads, float* out, cudaStream_t st);
-int launch_cls_row(float* x, const float* cls, const float* pos, int B, int T, int d, cudaStream_t st);
-int launch_layernorm(const float* x, const float* g, const float* b, void* y, int M, int d, float eps, cudaStream_t st);
-int launch_attention_tc(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st);
-int gemm_ln_tile_n(int N);
-int gemm_ln_f16_tc(const CUtensorMap& tmB, const CUtensorMap& tmC, const float* x, const float* gamma, const float* beta,
-                   const float* bias, int M, int N, float eps, bool gelu, cudaStream_t st, int kclass);
-
 // y[b, :] = LayerNorm(x[b * row_stride, :]) * gamma + beta in fp32 (one warp per row): the final norm of the CLS token
 __global__ void __launch_bounds__(128)
 layernorm_rows_f32_kernel(const float* __restrict__ x, long long row_stride, const float* __restrict__ gamma,

@@ -114,10 +114,6 @@ layernorm_f16_kernel(const float* __restrict__ x, const float* __restrict__ gamm
 // Shared tiles are [64 rows][64 halves] = 128 B rows with the 16 B chunk index XOR-swizzled by (row & 7).
 constexpr int ATT_BM = 64, ATT_BN = 64, ATT_D = 64, ATT_THREADS = 128;
 
-__device__ __forceinline__ uint32_t att_sw(uint32_t tile_base, int row, int chunk) {
-  return tile_base + row * 128 + ((chunk ^ (row & 7)) << 4);
-}
-
 // loads a [64 x 64] half tile (rows row0.. of a [T, ld] matrix slice starting at column col0) with zero fill
 __device__ __forceinline__ void att_load_tile(uint32_t tile_base, const __half* g, int row0, int T, long long ld,
                                               int tid) {
@@ -127,7 +123,7 @@ __device__ __forceinline__ void att_load_tile(uint32_t tile_base, const __half* 
     const int r = idx >> 3, ch = idx & 7;
     const bool ok = (row0 + r) < T;
     const __half* src = g + (long long)(ok ? row0 + r : 0) * ld + ch * 8;
-    cp_async_16(att_sw(tile_base, r, ch), src, ok);
+    cp_async_16(sw128_addr(tile_base, r, ch), src, ok);
   }
 }
 
@@ -178,7 +174,7 @@ attention_f16_kernel(const __half* __restrict__ qkv, __half* __restrict__ out, i
       for (int ks = 0; ks < 4; ++ks) {
         const int r = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
         const int ch = ks * 2 + (lane >> 4);
-        ldmatrix_x4(att_sw(sQ, r, ch), qf[ks][0], qf[ks][1], qf[ks][2], qf[ks][3]);
+        ldmatrix_x4(sw128_addr(sQ, r, ch), qf[ks][0], qf[ks][1], qf[ks][2], qf[ks][3]);
       }
     }
     const uint32_t kt = sK + st * ATT_BN * ATT_D * 2;
@@ -195,7 +191,7 @@ attention_f16_kernel(const __half* __restrict__ qkv, __half* __restrict__ out, i
         uint32_t b0, b1, b2, b3;
         const int r = np * 16 + (lane & 7) + (lane >> 4) * 8;  // key row
         const int ch = ks * 2 + ((lane >> 3) & 1);
-        ldmatrix_x4(att_sw(kt, r, ch), b0, b1, b2, b3);
+        ldmatrix_x4(sw128_addr(kt, r, ch), b0, b1, b2, b3);
         mma_m16n8k16_f16(s[np * 2], qf[ks], b0, b1);
         mma_m16n8k16_f16(s[np * 2 + 1], qf[ks], b2, b3);
       }
@@ -259,7 +255,7 @@ attention_f16_kernel(const __half* __restrict__ qkv, __half* __restrict__ out, i
         uint32_t b0, b1, b2, b3;
         const int r = ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;  // key row
         const int ch = np * 2 + (lane >> 4);                          // head-dim chunk
-        ldmatrix_x4_trans(att_sw(vt, r, ch), b0, b1, b2, b3);
+        ldmatrix_x4_trans(sw128_addr(vt, r, ch), b0, b1, b2, b3);
         mma_m16n8k16_f16(o[np * 2], pf[ks], b0, b1);
         mma_m16n8k16_f16(o[np * 2 + 1], pf[ks], b2, b3);
       }
