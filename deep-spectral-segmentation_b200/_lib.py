@@ -72,6 +72,7 @@ PROTOTYPES = {
     "dss_knn_workspace_bytes": (c_size_t, [c_int, c_int]),
     "dss_knn_color_counts": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "dss_eigsh_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "dss_eigsh_max_steps": (c_int, [c_int, c_int]),
     "dss_eigsh_laplacian": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p,
                                     c_void_p, c_void_p, c_void_p, c_void_p, c_size_t, c_void_p]),
     "dss_eigsh_topk": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_float, c_int, c_void_p, c_void_p, c_void_p,

@@ -216,7 +216,7 @@ lanczos_laplacian_kernel(EigParams p) {
   const int stripw = Npad < EIG_STRIP ? Npad : EIG_STRIP;
   float* colbuf = ycol + Npad;                               // [NW][stripw] per-warp column accumulators
   float* coef = colbuf + (size_t)EIG_WARPS * stripw;         // [mmax + 2]
-  __shared__ int s_flag;
+  __shared__ int s_flag;        // static: EIG_STATIC_SMEM counts these two
   __shared__ double s_top[2];   // top Ritz value of the newest block of T and its residual
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -673,6 +673,25 @@ static size_t eig_smem_bytes(int Npad, int mmax) {
          (size_t)(mmax + 2) * sizeof(float) + 16;
 }
 
+// A CTA may opt in to 227 KB of shared memory on sm_90, static and dynamic together: the kernel's static s_flag and
+// s_top take 32 B (ptxas -v, every instantiation), so a dynamic size above 227 KB - 32 B fails cudaFuncSetAttribute
+constexpr size_t EIG_STATIC_SMEM = 32;
+constexpr size_t EIG_SMEM_MAX = 227 * 1024 - EIG_STATIC_SMEM;   // the dynamic shared memory a launch may ask for
+
+// Checked before every launch (a host-side query, like the cudaFuncSetAttribute next to it): a __shared__ variable
+// added to the kernel must raise EIG_STATIC_SMEM, or the size checks and dss_eigsh_max_steps would pass budgets that
+// cannot launch.
+static int eig_check_static_smem(void (*kernel)(EigParams)) {
+  cudaFuncAttributes attr{};
+  DSS_CHECK_CUDA(cudaFuncGetAttributes(&attr, kernel));
+  if (attr.sharedSizeBytes > EIG_STATIC_SMEM) {
+    set_error("eigsh: the kernel has %zu B of static shared memory, EIG_STATIC_SMEM allows for %zu B",
+              attr.sharedSizeBytes, EIG_STATIC_SMEM);
+    return DSS_ERR_UNSUPPORTED;
+  }
+  return DSS_OK;
+}
+
 // Lanczos steps: the Laplacian modes work in the N - 1 dimensions orthogonal to the analytic null vector, the plain
 // mode in all N
 static int eig_resolve(int N, int K, int max_steps, bool plain) {
@@ -753,6 +772,12 @@ static int eigsh_launch(const float* Wmat, const float* deg, int ldw, int B, int
               variant, N, p.mmax, smem);
     return DSS_ERR_UNSUPPORTED;
   }
+  // before the workspace check: a budget that can never run is reported as such (see dss_eigsh_max_steps)
+  if (smem > EIG_SMEM_MAX) {
+    set_error("eigsh: N=%d with max_steps=%d needs %zu B of shared memory (> %zu B: 227 KB less %zu B static)", N,
+              p.mmax, smem, EIG_SMEM_MAX, EIG_STATIC_SMEM);
+    return DSS_ERR_UNSUPPORTED;
+  }
   const size_t need = eig_workspace_bytes(B, N, K, max_steps, variant);
   if (ws_bytes < need) {
     set_error("eigsh: workspace too small (%zu < %zu)", ws_bytes, need);
@@ -762,23 +787,25 @@ static int eigsh_launch(const float* Wmat, const float* deg, int ldw, int B, int
   p.basis = reinterpret_cast<float*>(ws);
   p.tri = reinterpret_cast<double*>(reinterpret_cast<uint8_t*>(ws) +
                                     align_up((size_t)grid * (p.mmax + 1) * p.Npad * sizeof(float), 256));
-  if (smem > 227 * 1024) {
-    set_error("eigsh: N=%d with max_steps=%d needs %zu B of shared memory (> 227 KB)", N, p.mmax, smem);
-    return DSS_ERR_UNSUPPORTED;
-  }
+  void (*kernel)(EigParams) = per_sm == 2 && variant == 1 ? lanczos_laplacian_kernel<2, 2, EIG_THREADS>
+                              : per_sm == 2                ? lanczos_laplacian_kernel<4, 2, 256>
+                                                           : lanczos_laplacian_kernel<4, 1, EIG_THREADS>;
+  const int threads = per_sm == 2 && variant != 1 ? 256 : EIG_THREADS;
+  if (const int rc = eig_check_static_smem(kernel)) return rc;
   LaunchScope scope(static_cast<cudaStream_t>(stream), KC_EIGSH);
-  if (per_sm == 2 && variant == 1) {
-    DSS_CHECK_CUDA(cudaFuncSetAttribute(lanczos_laplacian_kernel<2, 2, EIG_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    lanczos_laplacian_kernel<2, 2, EIG_THREADS><<<grid, EIG_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(p);
-  } else if (per_sm == 2) {
-    DSS_CHECK_CUDA(cudaFuncSetAttribute(lanczos_laplacian_kernel<4, 2, 256>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    lanczos_laplacian_kernel<4, 2, 256><<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(p);
-  } else {
-    DSS_CHECK_CUDA(cudaFuncSetAttribute(lanczos_laplacian_kernel<4, 1, EIG_THREADS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    lanczos_laplacian_kernel<4, 1, EIG_THREADS><<<grid, EIG_THREADS, smem, static_cast<cudaStream_t>(stream)>>>(p);
-  }
+  DSS_CHECK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  kernel<<<grid, threads, smem, static_cast<cudaStream_t>(stream)>>>(p);
   DSS_CHECK_CUDA(cudaGetLastError());
   return DSS_OK;
+}
+
+// the tridiagonal grows by 3 doubles per step, so above N ~ 3800 a budget of N - 1 steps no longer fits
+extern "C" int dss_eigsh_max_steps(int N, int mode) {
+  if (N < 2 || mode < 0 || mode > 2) return 0;
+  const int Npad = (N + 3) & ~3;
+  for (int m = mode == 2 ? N : N - 1; m >= 1; --m)
+    if (eig_smem_bytes(Npad, m) <= EIG_SMEM_MAX) return m;
+  return 0;
 }
 
 extern "C" int dss_eigsh_laplacian(const float* Wmat, const float* degree, int ldw, int B, int N, int K, int lapnorm,

@@ -200,22 +200,35 @@ def _bad_rows(evals: torch.Tensor, evecs: torch.Tensor, info: torch.Tensor) -> L
     return (~ok).nonzero().flatten().tolist()
 
 
-def _solve_with_retry(solve, n_images: int, N: int):
-    """Runs ``solve(sel, max_steps)`` (sel = None for the whole batch, else a list of batch rows) and retries the images
-    whose Lanczos run did not reach its tolerance or came back non-finite with the largest possible Krylov space
-    (max_steps = N - 1). The reference's own safety net is a second eigsh call (which='SM', extract.py:226-234).
-    Returns (eigenvalues, eigenvectors, info, failed rows) on the CPU."""
-    evals, evecs, info = (t.cpu() for t in solve(None, 0))
+def _retry_bad_rows(solve, evals: torch.Tensor, evecs: torch.Tensor, info: torch.Tensor, N: int) -> List[int]:
+    """Second half of the solve of a batch whose default-budget results (CPU tensors) are given: re-solves the rows whose
+    Lanczos run did not reach its tolerance or came back non-finite through ``solve(rows, max_steps)`` with the largest
+    Krylov space the solver fits -- N - 1 steps up to N = 3816, fewer above (spectral.max_steps; 1602 at N = 6400) --
+    and writes the converged ones into evals / evecs / info. Where that budget is no larger than the default (N <= 321,
+    or N >= 7893) a retry would only repeat the first run, so nothing is re-solved. The reference's own safety net is
+    a second eigsh call (which='SM', extract.py:226-234). Returns the rows that still failed."""
     bad = _bad_rows(evals, evecs, info)
+    if not bad:
+        return []
+    steps = spectral.max_steps(N)
+    if steps <= spectral.DEFAULT_MAX_STEPS:
+        return bad
     failed = []
-    if bad:
-        ev2, vec2, info2 = (t.cpu() for t in solve(bad, max(N - 1, 1)))
-        for j, i in enumerate(bad):
-            ok = int(info2[j, 1]) == 1 and bool(torch.isfinite(vec2[j]).all() and torch.isfinite(ev2[j]).all())
-            if ok:
-                evals[i], evecs[i], info[i] = ev2[j], vec2[j], info2[j]
-            else:
-                failed.append(i)
+    ev2, vec2, info2 = (t.cpu() for t in solve(bad, steps))
+    for j, i in enumerate(bad):
+        ok = int(info2[j, 1]) == 1 and bool(torch.isfinite(vec2[j]).all() and torch.isfinite(ev2[j]).all())
+        if ok:
+            evals[i], evecs[i], info[i] = ev2[j], vec2[j], info2[j]
+        else:
+            failed.append(i)
+    return failed
+
+
+def _solve_with_retry(solve, n_images: int, N: int):
+    """Runs ``solve(sel, max_steps)`` (sel = None for the whole batch, else a list of batch rows) with the default
+    budget, then _retry_bad_rows. Returns (eigenvalues, eigenvectors, info, failed rows) on the CPU."""
+    evals, evecs, info = (t.cpu() for t in solve(None, 0))
+    failed = _retry_bad_rows(solve, evals, evecs, info, N)
     return evals, evecs, info, failed
 
 
@@ -793,15 +806,8 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
             items, H, W, Hp, Wp = h["items"], h["H"], h["W"], h["Hp"], h["Wp"]
             evals, evecs, info = h["evals"], h["evecs"], h["info"]
             n_img = len(items)
-            bad = _bad_rows(evals, evecs, info)
-            failed = []
-            if bad:   # rare: largest possible Krylov space for the images that did not reach the tolerance
-                ev2, vec2, info2 = (t.cpu() for t in h["solve"](bad, max(Hp * Wp - 1, 1)))
-                for j, i in enumerate(bad):
-                    if int(info2[j, 1]) == 1 and bool(torch.isfinite(vec2[j]).all()):
-                        evals[i], evecs[i] = ev2[j], vec2[j]
-                    else:
-                        failed.append(i)
+            # rare: the largest Krylov space that fits for the images that did not reach the tolerance
+            failed = _retry_bad_rows(h["solve"], evals, evecs, info, Hp * Wp)
             all_failed.extend(items[j][1] for j in failed)
             if features_dir:
                 wr.submit_batch({"k": h["k"].numpy()}, [it_ for j, it_ in enumerate(_feature_items(

@@ -77,6 +77,15 @@ def affinity(feats: torch.Tensor, normalize=True, threshold_at_zero=True, color_
     return out
 
 
+DEFAULT_MAX_STEPS = 320   # the solver's step budget for max_steps <= 0 (at most N - 1, N for eigsh_topk)
+
+
+def max_steps(N: int, mode: int = 0) -> int:
+    """Largest step budget the solver accepts at N: its Lanczos tridiagonal (3 doubles per step) lives in shared memory.
+    At most N - 1 (mode 0 / 1, eigsh_laplacian) or N (mode 2, eigsh_topk); 0 when not even one step fits."""
+    return int(_lib.load().dss_eigsh_max_steps(N, mode))
+
+
 @torch.no_grad()
 def eigsh_laplacian(W: torch.Tensor, N: int, K: int, lapnorm=True, tol: float = 0.0, max_steps: int = 0,
                     degree: Optional[torch.Tensor] = None

@@ -212,8 +212,12 @@ int dss_knn_color_counts(const float* rgb, int B, int Hl, int Wl, uint8_t* count
  *             continued from a fresh start vector orthogonal to the basis; 0 on ordinary spectra
  * Method: Lanczos with full re-orthogonalisation on D^-1/2 W D^-1/2 (null vector deflated analytically), Ritz
  * values by Sturm bisection in fp64. tol <= 0 selects 1e-6; max_steps <= 0 selects min(N-1, 320) (min(N, 320) for
- * dss_eigsh_topk). Restarts draw on the same budget. */
+ * dss_eigsh_topk). Restarts draw on the same budget. The Lanczos tridiagonal lives in shared memory, so a budget
+ * that does not fit (e.g. N - 1 above N = 3816) is DSS_ERR_UNSUPPORTED. */
 size_t dss_eigsh_workspace_bytes(int B, int N, int K, int max_steps);
+/* Largest max_steps whose shared memory fits the solver at N, capped at N - 1 (mode 0 / 1: dss_eigsh_laplacian) or N
+ * (mode 2: dss_eigsh_topk); 0 when no budget fits or the arguments are invalid. No device work. */
+int dss_eigsh_max_steps(int N, int mode);
 int dss_eigsh_laplacian(const float* Wmat, const float* degree, int ldw, int B, int N, int K, int lapnorm, float tol,
                         int max_steps, float* evals, float* evecs, int* info, float* resid, void* ws, size_t ws_bytes,
                         dss_stream_t stream);

@@ -67,6 +67,98 @@ def test_bad_arguments_are_rejected_before_any_device_work():
     assert lib.dss_kernel_launch_count() == n0                                              # nothing was launched
 
 
+# mode 0 (mode 2 caps at N). 1602 steps at N = 6400 take exactly the 227 KB less the kernel's 32 B of static shared
+# memory; N = 7892 is the largest the default 320 steps fit.
+MAX_STEPS = {3600: 3599, 3816: 3815, 3820: 3813, 6400: 1602, 7892: 322, 7896: 319, 7900: 316, 8300: 0}
+
+
+@pytest.mark.parametrize("N", [3600, 3816, 3817, 3820, 4801, 6400, 7000, 7892, 7893, 7896, 7900, 8300])
+@pytest.mark.parametrize("mode", [0, 1, 2])
+def test_eigsh_max_steps_is_the_largest_budget_that_fits(N, mode):
+    """dss_eigsh_max_steps(N, mode) is a budget the solver accepts and, below its cap (N - 1, or N for the plain mode),
+    one step more is DSS_ERR_UNSUPPORTED. The shared-memory check runs before the workspace check, so a workspace one
+    byte short tells an accepted budget (-3) from a refused one (-4) without any launch."""
+    _lib = load_pkg("_lib")
+    lib = _lib.load()
+    n0 = lib.dss_kernel_launch_count()
+    K = 5
+    buf = torch.zeros(1 << 12, dtype=torch.uint8)
+    p = (buf.data_ptr() + 255) // 256 * 256
+    ldw = (N + 3) // 4 * 4
+
+    def call(steps):
+        short = lib.dss_eigsh_workspace_bytes(1, N, K, steps) - 1
+        if mode == 2:
+            return lib.dss_eigsh_topk(p, ldw, 1, N, K, 0.0, steps, p, p, p, None, p, short, None)
+        return lib.dss_eigsh_laplacian(p, None, ldw, 1, N, K, 1 - mode, 0.0, steps, p, p, p, None, p, short, None)
+
+    m = lib.dss_eigsh_max_steps(N, mode)
+    cap = N if mode == 2 else N - 1
+    if N in MAX_STEPS:
+        assert m == min(MAX_STEPS[N] + (mode == 2 and MAX_STEPS[N] == N - 1), cap)
+    assert 0 <= m <= cap
+    if m > 0:
+        assert call(m) == -3, lib.dss_last_error()
+    if m < cap:
+        assert call(m + 1) == -4 and b"shared memory" in lib.dss_last_error()
+    if m == 0:   # not even the default budget fits
+        assert call(0) == -4
+    assert lib.dss_kernel_launch_count() == n0
+
+
+def test_eigsh_max_steps_rejects_bad_arguments():
+    lib = load_pkg("_lib").load()
+    assert [lib.dss_eigsh_max_steps(N, mode) for N, mode in ((1, 0), (0, 2), (100, 3), (100, -1))] == [0] * 4
+    assert [lib.dss_eigsh_max_steps(2, mode) for mode in (0, 1, 2)] == [1, 1, 2]
+
+
+@pytest.mark.parametrize("N,budget", [(900, 899), (3600, 3599), (6400, 1602), (7892, 322), (300, None), (7896, None),
+                                      (7900, None)])
+def test_solve_with_retry_asks_for_the_largest_budget_that_fits(N, budget):
+    """The extract commands' retry of non-converged images: the default budget first, then the largest that fits in
+    shared memory (not N - 1 above N = 3816); no retry where that is not above the default, the rows reported failed."""
+    extract = load_pkg("extract")
+    asked = []
+
+    def solve(sel, max_steps):
+        asked.append((sel, max_steps))
+        B = 3 if sel is None else len(sel)
+        info = torch.zeros(B, 4, dtype=torch.int32)
+        info[:, 1] = 1 if max_steps else torch.tensor([1, 0, 1][:B])    # row 1 misses the default budget
+        return torch.full((B, 2), float(max_steps)), torch.zeros(B, 2, N), info
+
+    evals, _, info, failed = extract._solve_with_retry(solve, 3, N)
+    if budget is None:
+        assert asked == [(None, 0)] and failed == [1] and int(info[1, 1]) == 0
+    else:
+        assert asked == [(None, 0), ([1], budget)] and failed == []
+        assert evals[:, 0].tolist() == [0.0, float(budget), 0.0] and info[:, 1].tolist() == [1, 1, 1]
+
+
+@pytest.mark.parametrize("N,budget", [(3600, 3599), (6400, 1602), (7896, None)])
+def test_retry_of_a_solved_batch_asks_for_the_largest_budget_that_fits(N, budget):
+    """extract_all solves a batch asynchronously and hands the default-budget results to the same retry
+    (extract._retry_bad_rows): it re-solves only the bad rows, with the budget that fits, and fills them in place."""
+    extract = load_pkg("extract")
+    asked = []
+
+    def solve(sel, max_steps):
+        asked.append((sel, max_steps))
+        info = torch.zeros(len(sel), 4, dtype=torch.int32)
+        info[:, 1] = torch.tensor([1, 0, 1])                     # row 2 of the batch fails the retry as well
+        return torch.full((len(sel), 2), float(max_steps)), torch.zeros(len(sel), 2, N), info
+
+    evals, evecs, info = torch.zeros(4, 2), torch.zeros(4, 2, N), torch.ones(4, 4, dtype=torch.int32)
+    info[[0, 2], 1] = 0
+    evecs[3, 0, 5] = float("nan")                                 # converged but non-finite: retried too
+    failed = extract._retry_bad_rows(solve, evals, evecs, info, N)
+    if budget is None:
+        assert asked == [] and failed == [0, 2, 3]
+    else:
+        assert asked == [([0, 2, 3], budget)] and failed == [2]
+        assert evals[:, 0].tolist() == [budget, 0, 0, budget] and info[:, 1].tolist() == [1, 1, 0, 1]
+
+
 @pytest.mark.parametrize("name,Hp,Wp", [("dino_vits16", 30, 30), ("dino_vits16", 23, 31), ("dino_vits16", 14, 14),
                                         ("dino_vits16", 7, 40), ("dino_vitb8", 60, 60), ("dino_vitb8", 28, 28)])
 def test_pos_embed_interpolation_matches_upstream(name, Hp, Wp):

@@ -114,10 +114,11 @@ def _solve(Wm, N, K, mode, degree=None, max_steps=0):
 
 
 def _solve_retry(Wm, N, K, mode, degree=None):
-    """As the extract commands do: the default budget, then the largest Krylov space if that did not converge."""
+    """As the extract commands do: the default budget, then the largest Krylov space that fits in shared memory
+    (N - 1 steps up to N = 3816) if that did not converge."""
     out = _solve(Wm, N, K, mode, degree)
     if int(out[2][0, 1]) != 1:
-        out = _solve(Wm, N, K, mode, degree, max_steps=N - 1)
+        out = _solve(Wm, N, K, mode, degree, max_steps=load_pkg("spectral").max_steps(N))
     return out
 
 
