@@ -3,6 +3,7 @@ covariance-eigh PCA and the data-set K-means of the reference's extract_bboxes /
 (extract/extract.py:429-599)."""
 from __future__ import annotations
 
+import math
 from typing import Tuple
 
 import torch
@@ -52,12 +53,24 @@ def covariance(X: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
 @torch.no_grad()
 def pca_components(cov: torch.Tensor, d: int, pca_dim: int) -> torch.Tensor:
     """Top ``pca_dim`` eigenvectors [pca_dim, d] of the covariance (dss_eigsh_topk). Like the eigenvector commands, a
-    solve that does not reach its tolerance is retried with the largest Krylov space, and then fails loudly."""
+    solve that does not reach its tolerance is retried with the largest Krylov space, and then fails loudly.
+
+    The solver stops at residual <= tol * max(1, ||A||): an absolute 1e-6 for a covariance with ||C|| < 1, which is
+    what L2-normalised rows give (||C|| ~ 3e-3 at d = 768). So the covariance is first multiplied by the power of two
+    that brings its largest diagonal entry into [1, 2). That is exact in fp32 and leaves the eigenvectors unchanged, and
+    since lambda_1 >= max C_ii the tolerance is then relative to ||C||.
+
+    Limitation: a cluster of distinct but nearly equal eigenvalues straddling pca_dim (relative spread ~1e-6) does not
+    break the Lanczos recurrence down, so the solver can report convergence with copies from the cluster missing and
+    return vectors from below it instead (see dss_eigsh_topk in include/dss_b200.h)."""
     if pca_dim > PCA_MAX_DIM:
         raise _lib.DssError(f"pca_dim={pca_dim} > {PCA_MAX_DIM}: the device eigensolver computes at most "
                             f"{PCA_MAX_DIM} eigenpairs")
     if not 1 <= pca_dim < d:
         raise ValueError(f"pca_dim={pca_dim} must be in [1, {d})")
+    top = float(torch.diagonal(cov[:, :d]).max())
+    if math.isfinite(top) and top > 0.0:
+        cov = cov * math.ldexp(1.0, 1 - math.frexp(top)[1])       # max C_ii * 2^k in [1, 2)
     evals, evecs, info, _ = spectral.eigsh_topk(cov[None], d, pca_dim)
     if int(info[0, 1]) != 1 or not bool(torch.isfinite(evecs).all()):
         evals, evecs, info, _ = spectral.eigsh_topk(cov[None], d, pca_dim, max_steps=d - 1)
@@ -83,7 +96,13 @@ def pca_project(X: torch.Tensor, mean: torch.Tensor, V: torch.Tensor) -> torch.T
 
 @torch.no_grad()
 def pca(X: torch.Tensor, pca_dim: int) -> torch.Tensor:
-    """scikit-learn PCA(pca_dim).fit_transform(X) by the covariance-eigh route (component signs may differ)."""
+    """scikit-learn PCA(pca_dim).fit_transform(X) by the covariance-eigh route (component signs may differ).
+    Like scikit-learn, pca_dim may not exceed the number of rows: with M rows the centred data span at most M - 1
+    directions, and the components past them are null directions of the covariance, onto which every row projects to
+    ~0. A small data set can hit this, so it is an error of the input (ValueError), not a device failure."""
+    M = X.shape[0]
+    if M < 2 or pca_dim > M:
+        raise ValueError(f"pca_dim={pca_dim} needs at least max(2, pca_dim) rows, got {M}")
     mean, cov = covariance(X)
     return pca_project(X, mean, pca_components(cov, X.shape[1], pca_dim))
 

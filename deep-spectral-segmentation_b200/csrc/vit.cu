@@ -12,6 +12,7 @@
 
 #include <algorithm>
 #include <map>
+#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -61,8 +62,8 @@ struct dss_vit {
   CUtensorMap tm_patch;
   std::vector<dss::BlockW> blocks;
   std::vector<float> pos_host;                        // [1 + grid0^2, d] fp32 host copy
-  std::map<std::pair<int, int>, float*> pos_cache;    // (Hp, Wp) -> device [T, d]
-  std::vector<std::pair<int, int>> pos_order;         // insertion order: the cache is bounded (oldest grid evicted)
+  std::map<std::tuple<int, int, bool>, float*> pos_cache;   // (Hp, Wp, stored grid) -> device [T, d]
+  std::vector<std::tuple<int, int, bool>> pos_order;        // insertion order: the cache is bounded (oldest evicted)
 };
 
 namespace dss {
@@ -90,10 +91,16 @@ static void interp_axis(int in, int out, double scale_factor, std::vector<int>& 
   (void)in;
 }
 
+// Upstream interpolate_pos_encoding returns the stored grid only when npatch == N0 and the input's PIXEL height equals
+// its width. A g x g patch grid from a non-square input (a 224 x 232 box crop at patch 16) is still resampled, with
+// scale (g + 0.1) / g, which is not the identity. `square`: the input's pixel sizes are equal, or the caller crops to
+// patch multiples first as the reference does before get_intermediate_layers (then Hp == Wp decides).
+static bool pos_is_stored(int g, int Hp, int Wp, bool square) { return Hp == g && Wp == g && square; }
+
 // pos_src [1 + g*g, d] -> pos_out [1 + Hp*Wp, d]; host memory, pure CPU (runs once per distinct image shape)
-static void interp_pos_host(const float* src, int g, int d, int Hp, int Wp, float* pos) {
+static void interp_pos_host(const float* src, int g, int d, int Hp, int Wp, bool square, float* pos) {
   std::copy(src, src + d, pos);  // CLS slot untouched
-  if (Hp == g && Wp == g) {
+  if (pos_is_stored(g, Hp, Wp, square)) {
     std::copy(src + d, src + (size_t)(g * g + 1) * d, pos + d);
     return;
   }
@@ -119,16 +126,17 @@ static void interp_pos_host(const float* src, int g, int d, int Hp, int Wp, floa
     }
 }
 
-static int get_pos(dss_vit* h, int Hp, int Wp, cudaStream_t st, float** out) {
-  auto key = std::make_pair(Hp, Wp);
+static int get_pos(dss_vit* h, int Hp, int Wp, bool square, cudaStream_t st, float** out) {
+  const int d = h->cfg.dim, g = h->cfg.grid0, T = Hp * Wp + 1;
+  // keyed by the identity decision too: a g x g grid from a non-square input must not get the stored entry
+  const auto key = std::make_tuple(Hp, Wp, pos_is_stored(g, Hp, Wp, square));
   auto it = h->pos_cache.find(key);
   if (it != h->pos_cache.end()) {
     *out = it->second;
     return DSS_OK;
   }
-  const int d = h->cfg.dim, g = h->cfg.grid0, T = Hp * Wp + 1;
   std::vector<float> pos((size_t)T * d);
-  interp_pos_host(h->pos_host.data(), g, d, Hp, Wp, pos.data());
+  interp_pos_host(h->pos_host.data(), g, d, Hp, Wp, square, pos.data());
   float* dev = nullptr;
   DSS_CHECK_CUDA(cudaMalloc(&dev, (size_t)T * d * sizeof(float)));
   DSS_CHECK_CUDA(cudaMemcpyAsync(dev, pos.data(), (size_t)T * d * sizeof(float), cudaMemcpyHostToDevice, st));
@@ -203,7 +211,10 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   }
   int rc;
   float* pos = nullptr;
-  if ((rc = get_pos(h, Hp, Wp, st, &pos))) return rc;
+  // forward_k's and localization's inputs are cropped or padded to patch multiples by the reference before the model
+  // sees them, so their patch grid decides; the model's own forward (box crops) and the token hook take the image as is
+  const bool square = (mode == 1 || mode == 2) ? H == W : Hp == Wp;
+  if ((rc = get_pos(h, Hp, Wp, square, st, &pos))) return rc;
 
   CUtensorMap tm_patches, tm_xn, tm_attn, tm_hid;
   const int Kp = 3 * P * P;
@@ -472,7 +483,7 @@ extern "C" int dss_vit_pos_embed(dss_vit_t* h, int Hp, int Wp, float* out, dss_s
   DSS_REQUIRE(Hp > 0 && Wp > 0, "vit_pos_embed: empty grid");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   float* pos = nullptr;
-  int rc = get_pos(h, Hp, Wp, st, &pos);
+  int rc = get_pos(h, Hp, Wp, Hp == Wp, st, &pos);
   if (rc) return rc;
   DSS_CHECK_CUDA(cudaMemcpyAsync(out, pos, ((size_t)Hp * Wp + 1) * h->cfg.dim * sizeof(float),
                                  cudaMemcpyDeviceToDevice, st));
@@ -482,6 +493,6 @@ extern "C" int dss_vit_pos_embed(dss_vit_t* h, int Hp, int Wp, float* out, dss_s
 extern "C" int dss_pos_embed_interp_host(const float* pos_embed_host, int grid0, int d, int Hp, int Wp,
                                          float* out_host) {
   DSS_REQUIRE(pos_embed_host && out_host && grid0 > 0 && d > 0 && Hp > 0 && Wp > 0, "pos_embed_interp_host: bad args");
-  interp_pos_host(pos_embed_host, grid0, d, Hp, Wp, out_host);
+  interp_pos_host(pos_embed_host, grid0, d, Hp, Wp, Hp == Wp, out_host);
   return DSS_OK;
 }

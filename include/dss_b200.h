@@ -99,12 +99,16 @@ size_t dss_vit_workspace_bytes(const dss_vit_t* h, int B, int H, int W);
 int dss_vit_forward_k(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, int which_block, float* k_out,
                       void* ws, size_t ws_bytes, dss_stream_t stream);
 
-/* Debug/parity hook: residual stream x [B, T, d] fp32 after `n_blocks` full blocks (T = N + 1, CLS first). */
+/* Debug/parity hook: residual stream x [B, T, d] fp32 after `n_blocks` full blocks (T = N + 1, CLS first). Like
+ * dss_vit_forward_cls it takes the image uncropped: a grid0 x grid0 patch grid from an H != W image gets the
+ * resampled positional embedding, as upstream interpolate_pos_encoding decides from the pixel sizes. */
 int dss_vit_forward_tokens(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, int n_blocks, float* x_out,
                            void* ws, size_t ws_bytes, dss_stream_t stream);
 
 /* The model's own forward (upstream VisionTransformer.forward: all blocks, final LayerNorm, CLS token), which the
- * reference calls on bounding-box crops (extract/extract.py:537-541, extract_bbox_features): cls_out [B, d] fp32. */
+ * reference calls on bounding-box crops (extract/extract.py:537-541, extract_bbox_features): cls_out [B, d] fp32.
+ * The crop is not cut to patch multiples first, so the stored positional grid is used only when H == W (pixels) and
+ * the patch grid is grid0 x grid0, as upstream decides; otherwise it is interpolated. */
 int dss_vit_forward_cls(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, float* cls_out, void* ws,
                         size_t ws_bytes, dss_stream_t stream);
 
@@ -205,8 +209,12 @@ int dss_knn_color_counts(const float* rgb, int B, int Hl, int Wl, uint8_t* count
  * Outputs: evals [B, K] ascending, evecs [B, K, N] with the reference's sign rule applied (extract.py:237-240),
  * info [B, 4] int32, resid [B, K] fp32 residual estimates (may be NULL):
  *   info[b,0] Lanczos steps taken, restarts included
- *   info[b,1] 1 when the K pairs returned are eigenpairs to tol (repeated eigenvalues with all their copies, vectors
- *             orthonormal), else 0: the step budget ran out first; pairs that do not exist yet are NaN
+ *   info[b,1] 1 when the K pairs returned are eigenpairs to tol * max(1, ||A||) (vectors orthonormal), else 0: the
+ *             step budget ran out first; pairs that do not exist yet are NaN. An exactly repeated eigenvalue breaks
+ *             the recurrence down and is returned with all its copies (restarts, info[b,3]); a cluster of distinct
+ *             but nearly equal eigenvalues (relative spread ~1e-6) straddling the K-th does not break it down, and
+ *             copies from it can be missed while info[b,1] is 1. The tolerance has an absolute floor: scale A so
+ *             that ||A|| >= 1 for a relative one (cluster.pca_components does).
  *   info[b,2] dss_eigsh_topk only: a negative eigenvalue is larger in magnitude than the K-th (see below); else 0
  *   info[b,3] restarts: Lanczos breakdowns (an invariant Krylov subspace, e.g. at an eigenvalue of multiplicity > 1)
  *             continued from a fresh start vector orthogonal to the basis; 0 on ordinary spectra

@@ -49,3 +49,44 @@ def extract_bbox(segmap: np.ndarray, image_id, P: int, num_erode: int, num_dilat
             outputs["bboxes"].append(bbox)
             outputs["bboxes_original_resolution"].append([x * P for x in bbox])
     return outputs
+
+
+def edge_maps(H: int, W: int, seed: int = 0) -> dict:
+    """Hand-built label maps at an H x W grid for the morphology's edges (name -> uint8 map): every one of the 256 values
+    at once, only 0, only 255, 1-pixel lines, a 0 / 255 checkerboard (every pixel isolated: erosion empties it at step
+    1), squares of sides 1, 3, 5, ... (side 2s - 1 empties at erosion step s), segments touching each border and
+    corner (where erosion's outside-is-set and dilation's outside-is-unset rules differ), random rectangles."""
+    g = np.random.default_rng(seed)
+    y, x = np.mgrid[0:H, 0:W]
+    maps = {"all_values": np.resize(g.permutation(256), H * W).reshape(H, W),
+            "zeros": np.zeros((H, W)), "ones255": np.full((H, W), 255),
+            "checker": ((y + x) % 2) * 255}
+    lines = np.zeros((H, W))
+    lines[y % 4 == 1] = 1 + (y[y % 4 == 1] // 4) % 100
+    lines[x % 5 == 2] = 101 + (x[x % 5 == 2] // 5) % 100
+    maps["lines"] = lines
+    sq = np.full((H, W), 7)
+    r0, c0, v = int(H > 2), int(W > 2), 1      # off the border where there is room: clipped squares on a strip
+    for side in range(1, 40, 2):
+        if c0 >= W:
+            r0, c0 = r0 + side + 1, int(W > 2)
+        if r0 >= H:
+            break
+        sq[r0:r0 + side, c0:c0 + side] = 10 + v
+        c0 += side + 1
+        v += 1
+    maps["squares"] = sq
+    border = np.full((H, W), 50)
+    border[:, : max(1, W // 6)] = 51
+    border[:, W - max(1, W // 7):] = 52
+    border[: max(1, H // 5)] = 53
+    border[H - max(1, H // 8):] = 54
+    border[0, 0], border[0, W - 1], border[H - 1, 0], border[H - 1, W - 1] = 60, 61, 62, 63
+    border[H // 2, W // 2] = 64
+    maps["border"] = border
+    rects = np.zeros((H, W))
+    for v in g.choice(np.arange(1, 256), size=min(40, H * W), replace=False):
+        r, c = g.integers(0, H), g.integers(0, W)
+        rects[r:r + g.integers(1, max(2, H // 2)), c:c + g.integers(1, max(2, W // 2))] = v
+    maps["rects"] = rects
+    return {k: np.ascontiguousarray(m, dtype=np.uint8) for k, m in maps.items()}
