@@ -60,10 +60,7 @@ PROTOTYPES = {
                                         c_void_p]),
     "dss_debug_gemm_trace": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int,
                                      c_void_p, c_size_t, c_void_p]),
-    "dss_op_gemm_ln_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_float,
-                                   c_int, c_void_p]),
     "dss_op_layernorm_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
-    "dss_op_attention_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "dss_op_attention_tc_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "dss_op_im2col_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "dss_affinity_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),

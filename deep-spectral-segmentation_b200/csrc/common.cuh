@@ -1,5 +1,5 @@
 // Shared device/host helpers for libdss_b200 (sm_90a only).
-// PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor), wgmma, cp.async, ldmatrix, mma.sync.
+// PTX wrappers for mbarrier, TMA (cp.async.bulk.tensor), wgmma, thread-block clusters.
 #pragma once
 #include <cuda.h>  // CUtensorMap (types only; the driver entry point is resolved at run time, no -lcuda)
 #include <cuda_fp16.h>
@@ -46,16 +46,13 @@ int make_tmap_f16(CUtensorMap* tm, const void* ptr, int rows, int cols, int box_
 int make_tmap_out(CUtensorMap* tm, const void* ptr, int rows, int cols, int is_f32);
 int make_tmap_out3d_f32(CUtensorMap* tm, const void* ptr, int images, int rows, int ld);
 int make_tmap_out3d_f16(CUtensorMap* tm, const void* ptr, int images, int rows, int cols);
-// persistent wgmma GEMMs (gemm.cu, gemm_ln.cu)
+// persistent wgmma GEMMs (gemm.cu)
 int gemm_tile_n();
 int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, const float* bias, void* out,
                 int M, int N, int K, int epi, const float* aux, int rin, int rout, cudaStream_t st, int kclass, int bn);
 int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int images, int Nimg, int d, float* Wout, int ldw,
                      int ncols, const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts,
                      float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st);
-int gemm_ln_tile_n(int N);
-int gemm_ln_f16_tc(const CUtensorMap& tmB, const CUtensorMap& tmC, const float* x, const float* gamma, const float* beta,
-                   const float* bias, int M, int N, float eps, bool gelu, cudaStream_t st, int kclass);
 // ViT kernels (vit_kernels.cu, attention_tc.cu)
 int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
 int launch_im2col_pad(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
@@ -307,35 +304,6 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// ---- Ampere-style async copy + legacy tensor-core path (used by the attention kernel)
-__device__ __forceinline__ void cp_async_16(uint32_t smem_dst, const void* gsrc, bool valid) {
-  const int src_bytes = valid ? 16 : 0;  // src-size 0 => zero fill
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_dst), "l"(gsrc), "r"(src_bytes) : "memory");
-}
-__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void cp_async_wait() {
-  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
-}
-__device__ __forceinline__ void ldmatrix_x4(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2, uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-               : "r"(addr));
-}
-__device__ __forceinline__ void ldmatrix_x4_trans(uint32_t addr, uint32_t& r0, uint32_t& r1, uint32_t& r2,
-                                                  uint32_t& r3) {
-  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r0), "=r"(r1), "=r"(r2), "=r"(r3)
-               : "r"(addr));
-}
-// D(16x8,f32) += A(16x16,f16,row) * B(16x8,f16,col)
-__device__ __forceinline__ void mma_m16n8k16_f16(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   __half2 h = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&h);
@@ -371,11 +339,10 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-// LayerNorm arithmetic of one row held as float4 chunks per lane, shared by layernorm_f16_kernel and the fused LayerNorm
-// GEMM (gemm_ln.cu) so that the fused GEMM's A operand is bit for bit the stand-alone kernel's output. Every rounding is
-// explicit (no contraction is left to the compiler, which chose differently in the two kernels): x - mean is one fused
-// multiply-add on the row sum S (the mean itself is never rounded), the squares pair as fma(a, a, b * b), the variance is
-// fma(Q, 1 / d, eps), and y = fma((x - mean) * rstd, gamma, beta).
+// LayerNorm arithmetic of one row held as float4 chunks per lane (layernorm_f16_kernel). Every rounding is explicit (no
+// contraction is left to the compiler), so the output is fixed by the source rather than by the compiler's choices:
+// x - mean is one fused multiply-add on the row sum S (the mean itself is never rounded), the squares pair as
+// fma(a, a, b * b), the variance is fma(Q, 1 / d, eps), and y = fma((x - mean) * rstd, gamma, beta).
 __device__ __forceinline__ float ln_sum4(float4 v) { return __fadd_rn(__fadd_rn(v.x, v.y), __fadd_rn(v.z, v.w)); }
 __device__ __forceinline__ float4 ln_center4(float4 v, float S, float inv_d) {
   return make_float4(__fmaf_rn(S, -inv_d, v.x), __fmaf_rn(S, -inv_d, v.y), __fmaf_rn(S, -inv_d, v.z),

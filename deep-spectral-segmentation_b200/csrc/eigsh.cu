@@ -18,10 +18,10 @@
 // One start vector sees a single direction of every eigenspace, so at an eigenvalue of multiplicity > 1 the Krylov space
 // becomes invariant (breakdown) before all copies are found. The iteration then restarts from a fresh vector orthogonal
 // to the basis: T becomes block diagonal, and Ritz vectors are taken per block, so each copy gets its own vector.
-// Three instantiations exist (<4, 1, 512> the default, <2, 2, 512> and <4, 2, 256> two CTAs per SM); dss_debug_eigsh
-// runs any of them on the same inputs, for the A/B of EIG_PAIR_DEFAULT and for the tests of the paired ones.
+// Three instantiations exist: <4, 1, 512>, one CTA per SM, and <2, 2, 512> and <4, 2, 256>, two CTAs per SM. The entry
+// points launch the default selection (eig_per_sm); dss_debug_eigsh runs any of them on the same inputs, for the A/B of
+// EIG_PAIR_DEFAULT and for the tests of the paired ones.
 #include <math.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -34,10 +34,6 @@ constexpr int EIG_MAX_K = 64;
 
 constexpr int EIG_STRIP_CH = 4;                    // float4 column chunks per lane and strip
 constexpr int EIG_STRIP = 32 * 4 * EIG_STRIP_CH;   // 512 columns per strip
-// Up to this N two CTAs (images) could share an SM with the <2, 2> instantiation (64 registers, 2 x 2 loads in flight per
-// lane). The default is <4, 1> -- one CTA per SM, 128 registers, all 16 loads of a row group's column blocks in flight
-// per lane; <2, 2> is only kept for tuning (DSS_EIG_VARIANT=1).
-constexpr int EIG_SMALL_N = 0;
 
 struct EigParams {
   const float* W;     // [B, N, ldw]
@@ -702,15 +698,10 @@ static int eig_resolve(int N, int K, int max_steps, bool plain) {
   return mmax;
 }
 
-// CTAs per SM: 2 when two images' shared memory fits (N <= ~2000) -- the <4, 2, 256> instantiation, two 256-thread CTAs
-// at 128 registers, so that one image's vector phases (reorthogonalisation, Ritz test) overlap the other's mat-vec --
-// else 1 (<4, 1, 512>). DSS_EIG_VARIANT (tuning): 1 forces <2, 2, 512>, 2 forces <4, 1, 512>, 3 forces the pairing.
-static int eig_variant() {
-  static const int variant = [] { const char* e = getenv("DSS_EIG_VARIANT"); return e ? atoi(e) : 0; }();
-  return variant;
-}
-
-// variant: 1 = <2, 2, 512>, 2 = <4, 1, 512>, 3 = <4, 2, 256>, anything else = the default
+// CTAs per SM. The default, variant 0, is 1 (<4, 1, 512>); with EIG_PAIR_DEFAULT it is 2 when two images' shared memory
+// fits (N <= ~2000) -- the <4, 2, 256> instantiation, two 256-thread CTAs at 128 registers, so that one image's vector
+// phases (reorthogonalisation, Ritz test) overlap the other's mat-vec. dss_debug_eigsh forces a variant:
+// 1 = <2, 2, 512>, 2 = <4, 1, 512>, 3 = <4, 2, 256>.
 static int eig_per_sm(int Npad, int mmax, int variant) {
   const size_t smem = eig_smem_bytes(Npad, mmax);
   const int fit = (int)((size_t)(220 * 1024) / (smem + 1024));
@@ -746,7 +737,7 @@ static size_t eig_workspace_bytes(int B, int N, int K, int max_steps, int varian
 using namespace dss;
 
 extern "C" size_t dss_eigsh_workspace_bytes(int B, int N, int K, int max_steps) {
-  return eig_workspace_bytes(B, N, K, max_steps, eig_variant());
+  return eig_workspace_bytes(B, N, K, max_steps, 0);
 }
 
 // forced: the variant was asked for explicitly (dss_debug_eigsh), so a pairing that does not fit is an error instead of
@@ -811,13 +802,13 @@ extern "C" int dss_eigsh_max_steps(int N, int mode) {
 extern "C" int dss_eigsh_laplacian(const float* Wmat, const float* degree, int ldw, int B, int N, int K, int lapnorm,
                                    float tol, int max_steps, float* evals, float* evecs, int* info, float* resid,
                                    void* ws, size_t ws_bytes, dss_stream_t stream) {
-  return eigsh_launch(Wmat, degree, ldw, B, N, K, lapnorm ? 0 : 1, tol, max_steps, eig_variant(), false, evals, evecs, info,
+  return eigsh_launch(Wmat, degree, ldw, B, N, K, lapnorm ? 0 : 1, tol, max_steps, 0, false, evals, evecs, info,
                       resid, ws, ws_bytes, stream);
 }
 
 extern "C" int dss_eigsh_topk(const float* Amat, int lda, int B, int N, int K, float tol, int max_steps, float* evals,
                               float* evecs, int* info, float* resid, void* ws, size_t ws_bytes, dss_stream_t stream) {
-  return eigsh_launch(Amat, nullptr, lda, B, N, K, 2, tol, max_steps, eig_variant(), false, evals, evecs, info, resid, ws,
+  return eigsh_launch(Amat, nullptr, lda, B, N, K, 2, tol, max_steps, 0, false, evals, evecs, info, resid, ws,
                       ws_bytes, stream);
 }
 

@@ -1,7 +1,7 @@
-// The pipeline the persistent wgmma GEMM kernels share (gemm.cu: cooperative and ping-pong schedules; gemm_ln.cu: fused
-// LayerNorm): a ring of 64-deep K slabs filled by TMA and released by the MMA warp groups of both CTAs of a cluster
-// pair, the wgmma k-steps of one slab, the 128 B-swizzled output staging box with its TMA store, and the cluster-pair
-// launch. Each kernel keeps its own tile schedule, producer and epilogue arithmetic.
+// The pipeline the persistent wgmma GEMM kernels of gemm.cu share (cooperative and ping-pong schedules): a ring of
+// 64-deep K slabs filled by TMA and released by the MMA warp groups of both CTAs of a cluster pair, the wgmma k-steps
+// of one slab, the 128 B-swizzled output staging box with its TMA store, and the cluster-pair launch. Each kernel keeps
+// its own tile schedule, producer and epilogue arithmetic.
 #pragma once
 #include "common.cuh"
 

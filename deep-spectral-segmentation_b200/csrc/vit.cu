@@ -8,7 +8,6 @@
 // The block the reference hooks is pruned to LN1 + the K third of its qkv projection, CLS row dropped in the
 // GEMM epilogue, which writes the fp32 features directly in the reference's [B, N, d] layout.
 #include <math.h>
-#include <stdlib.h>
 
 #include <algorithm>
 #include <map>
@@ -46,7 +45,6 @@ struct BlockW {
   __half *qkv_w, *proj_w, *fc1_w, *fc2_w;
   CUtensorMap tm_qkv, tm_k, tm_proj, tm_fc1, tm_fc2;
   CUtensorMap tm_q, tm_v;             // q and v thirds of the qkv weight (localization features)
-  CUtensorMap tm_qkv_ln, tm_fc1_ln;   // weight maps of the LayerNorm-fused kernel (its own tile width)
 };
 
 }  // namespace dss
@@ -236,37 +234,21 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
     return rc;
   if ((rc = launch_cls_row(w.x, h->cls, pos, B, T, d, st))) return rc;
 
-  // LayerNorm kernel + GEMM by default: on an H100 (400 W) this measured 3 526 - 3 554 images/s against 3 284 - 3 291
-  // with the LayerNorm fused into the A-operand producer of the qkv / fc1 GEMMs (gemm_ln.cu, DSS_VIT_FUSED_LN=1; K = 384
-  // only: a 128 x 768 fp16 panel does not fit next to the weight ring), whose panel turnover is not hidden
-  static const bool fused_ln_env = [] { const char* e = getenv("DSS_VIT_FUSED_LN"); return e && atoi(e) != 0; }();
-  const bool fused_ln = fused_ln_env && d == 384;
+  // LayerNorm kernel + GEMM: LayerNorm fused into the qkv / fc1 GEMMs measured slower (DESIGN.md section 9)
   for (int l = 0; l < n_full; ++l) {
     const BlockW& bw = h->blocks[l];
-    if (fused_ln) {
-      if ((rc = gemm_ln_f16_tc(bw.tm_qkv_ln, tm_qkv_out, w.x, bw.ln1_w, bw.ln1_b, bw.qkv_b, M, 3 * d, c.ln_eps, false, st,
-                               KC_GEMM_QKV)))
-        return rc;
-    } else {
-      if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
-      if ((rc = gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, w.qkv, M, 3 * d, d, DSS_EPI_BIAS_F16, nullptr, 0, 0, st,
-                            KC_GEMM_QKV, gemm_tile_n())))
-        return rc;
-    }
+    if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
+    if ((rc = gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, w.qkv, M, 3 * d, d, DSS_EPI_BIAS_F16, nullptr, 0, 0, st,
+                          KC_GEMM_QKV, gemm_tile_n())))
+      return rc;
     if ((rc = launch_attention_tc(w.qkv, w.attn, B, T, c.heads, st))) return rc;
     if ((rc = gemm_f16_tc(tm_attn, bw.tm_proj, &tm_x_out, bw.proj_b, w.x, M, d, d, DSS_EPI_BIAS_RESID_F32, nullptr, 0, 0, st,
                           KC_GEMM_PROJ, gemm_tile_n())))
       return rc;
-    if (fused_ln) {
-      if ((rc = gemm_ln_f16_tc(bw.tm_fc1_ln, tm_hid_out, w.x, bw.ln2_w, bw.ln2_b, bw.fc1_b, M, c.mlp_ratio * d, c.ln_eps, true,
-                               st, KC_GEMM_FC1)))
-        return rc;
-    } else {
-      if ((rc = launch_layernorm(w.x, bw.ln2_w, bw.ln2_b, w.xn, M, d, c.ln_eps, st))) return rc;
-      if ((rc = gemm_f16_tc(tm_xn, bw.tm_fc1, &tm_hid_out, bw.fc1_b, w.hid, M, c.mlp_ratio * d, d, DSS_EPI_BIAS_GELU_F16,
-                            nullptr, 0, 0, st, KC_GEMM_FC1, gemm_tile_n())))
-        return rc;
-    }
+    if ((rc = launch_layernorm(w.x, bw.ln2_w, bw.ln2_b, w.xn, M, d, c.ln_eps, st))) return rc;
+    if ((rc = gemm_f16_tc(tm_xn, bw.tm_fc1, &tm_hid_out, bw.fc1_b, w.hid, M, c.mlp_ratio * d, d, DSS_EPI_BIAS_GELU_F16,
+                          nullptr, 0, 0, st, KC_GEMM_FC1, gemm_tile_n())))
+      return rc;
     if ((rc = gemm_f16_tc(tm_hid, bw.tm_fc2, &tm_x_out, bw.fc2_b, w.x, M, d, c.mlp_ratio * d, DSS_EPI_BIAS_RESID_F32, nullptr, 0,
                           0, st, KC_GEMM_FC2, gemm_tile_n())))
       return rc;
@@ -415,10 +397,6 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     if ((rc = make_tmap_f16(&b.tm_proj, b.proj_w, (int)d, (int)d, gemm_tile_n() / 2))) return rc;
     if ((rc = make_tmap_f16(&b.tm_fc1, b.fc1_w, (int)hid, (int)d, gemm_tile_n() / 2))) return rc;
     if ((rc = make_tmap_f16(&b.tm_fc2, b.fc2_w, (int)d, (int)hid, gemm_tile_n() / 2))) return rc;
-    if (d == 384) {
-      if ((rc = make_tmap_f16(&b.tm_qkv_ln, b.qkv_w, (int)(3 * d), (int)d, gemm_ln_tile_n((int)(3 * d)) / 2))) return rc;
-      if ((rc = make_tmap_f16(&b.tm_fc1_ln, b.fc1_w, (int)hid, (int)d, gemm_ln_tile_n((int)hid) / 2))) return rc;
-    }
   }
   // host copy of the positional grid for interpolation; drop stale interpolations
   const size_t npos = ((size_t)c.grid0 * c.grid0 + 1) * d;

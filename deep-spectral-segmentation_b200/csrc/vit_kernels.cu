@@ -1,4 +1,4 @@
-// Non-GEMM kernels of the DINO ViT forward: pixel normalisation + im2col, CLS row, LayerNorm, attention.
+// Non-GEMM kernels of the DINO ViT forward: pixel normalisation + im2col, CLS row, LayerNorm, CLS attention row.
 #include <math.h>
 
 #include "common.cuh"
@@ -72,7 +72,7 @@ __global__ void cls_row_kernel(float* __restrict__ x, const float* __restrict__ 
 
 // ---------------------------------------------------------------------------------------------------------------
 // LayerNorm: one warp per row, row kept in registers, two-pass variance (mean, then E[(x-mean)^2]) like torch,
-// in the arithmetic of the ln_* helpers (common.cuh) that the fused LayerNorm GEMM shares.
+// in the explicitly rounded arithmetic of the ln_* helpers (common.cuh).
 template <int D>
 __global__ void __launch_bounds__(256)
 layernorm_f16_kernel(const float* __restrict__ x, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -104,180 +104,6 @@ layernorm_f16_kernel(const float* __restrict__ x, const float* __restrict__ gamm
     const float4 bt = __ldg(reinterpret_cast<const float4*>(beta) + lane + 32 * i);
     const uint2 o = ln_out4(v[i], rstd, g, bt);
     yr[lane + 32 * i] = o;
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------
-// Attention, head dim 64: O = softmax(Q K^T / 8) V per (image, head), flash-style online softmax.
-// CTA = 4 warps x 16 query rows; K/V streamed in 64-key tiles through a 2-stage cp.async ring;
-// QK^T and PV on mma.sync m16n8k16 (fp16 in, fp32 accumulate); P never leaves registers.
-// Shared tiles are [64 rows][64 halves] = 128 B rows with the 16 B chunk index XOR-swizzled by (row & 7).
-constexpr int ATT_BM = 64, ATT_BN = 64, ATT_D = 64, ATT_THREADS = 128;
-
-// loads a [64 x 64] half tile (rows row0.. of a [T, ld] matrix slice starting at column col0) with zero fill
-__device__ __forceinline__ void att_load_tile(uint32_t tile_base, const __half* g, int row0, int T, long long ld,
-                                              int tid) {
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int idx = tid + i * ATT_THREADS;  // 0..511
-    const int r = idx >> 3, ch = idx & 7;
-    const bool ok = (row0 + r) < T;
-    const __half* src = g + (long long)(ok ? row0 + r : 0) * ld + ch * 8;
-    cp_async_16(sw128_addr(tile_base, r, ch), src, ok);
-  }
-}
-
-__global__ void __launch_bounds__(ATT_THREADS)
-attention_f16_kernel(const __half* __restrict__ qkv, __half* __restrict__ out, int T, int heads) {
-  __shared__ __align__(128) uint8_t smem[(1 + 2 + 2) * ATT_BM * ATT_D * 2];  // Q | K0 K1 | V0 V1 = 40 KB
-  const int d = heads * ATT_D;
-  const long long ld = 3LL * d;
-  const int qt = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const __half* qg = qkv + (long long)b * T * ld + h * ATT_D;
-  const __half* kg = qg + d;
-  const __half* vg = qg + 2 * d;
-  const uint32_t sQ = smem_u32(smem);
-  const uint32_t sK = sQ + ATT_BM * ATT_D * 2;
-  const uint32_t sV = sK + 2 * ATT_BN * ATT_D * 2;
-  const int q0 = qt * ATT_BM;
-  const int ntiles = (T + ATT_BN - 1) / ATT_BN;
-
-  att_load_tile(sQ, qg, q0, T, ld, tid);
-  att_load_tile(sK, kg, 0, T, ld, tid);
-  att_load_tile(sV, vg, 0, T, ld, tid);
-  cp_async_commit();
-
-  // softmax in base 2: p = 2^(s*c - m*c), c = log2(e)/sqrt(64)
-  const float sc = 1.4426950408889634f * 0.125f;
-  float m_run[2] = {-INFINITY, -INFINITY};
-  float l_run[2] = {0.f, 0.f};
-  float o[8][4];
-#pragma unroll
-  for (int i = 0; i < 8; ++i) o[i][0] = o[i][1] = o[i][2] = o[i][3] = 0.f;
-  uint32_t qf[4][4];
-
-  for (int j = 0; j < ntiles; ++j) {
-    const int st = j & 1;
-    if (j + 1 < ntiles) {
-      att_load_tile(sK + (st ^ 1) * ATT_BN * ATT_D * 2, kg, (j + 1) * ATT_BN, T, ld, tid);
-      att_load_tile(sV + (st ^ 1) * ATT_BN * ATT_D * 2, vg, (j + 1) * ATT_BN, T, ld, tid);
-      cp_async_commit();
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
-    __syncthreads();
-    if (j == 0) {
-      // Q fragments (A operand, 16 rows of this warp x 64) stay in registers for the whole kernel
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        const int r = warp * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;
-        const int ch = ks * 2 + (lane >> 4);
-        ldmatrix_x4(sw128_addr(sQ, r, ch), qf[ks][0], qf[ks][1], qf[ks][2], qf[ks][3]);
-      }
-    }
-    const uint32_t kt = sK + st * ATT_BN * ATT_D * 2;
-    const uint32_t vt = sV + st * ATT_BN * ATT_D * 2;
-
-    // S = Q K^T : 8 n-tiles (8 keys each) x 4 k-steps
-    float s[8][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) s[i][0] = s[i][1] = s[i][2] = s[i][3] = 0.f;
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {  // pairs of n-tiles
-        uint32_t b0, b1, b2, b3;
-        const int r = np * 16 + (lane & 7) + (lane >> 4) * 8;  // key row
-        const int ch = ks * 2 + ((lane >> 3) & 1);
-        ldmatrix_x4(sw128_addr(kt, r, ch), b0, b1, b2, b3);
-        mma_m16n8k16_f16(s[np * 2], qf[ks], b0, b1);
-        mma_m16n8k16_f16(s[np * 2 + 1], qf[ks], b2, b3);
-      }
-    }
-    // mask keys beyond T (only the last tile can be partial)
-    const int kbase = j * ATT_BN;
-    if (kbase + ATT_BN > T) {
-#pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int key = kbase + i * 8 + (lane & 3) * 2;
-        if (key >= T) s[i][0] = s[i][2] = -INFINITY;
-        if (key + 1 >= T) s[i][1] = s[i][3] = -INFINITY;
-      }
-    }
-    // online softmax; thread owns rows (lane/4) [regs 0,1] and (lane/4 + 8) [regs 2,3]
-    float mx[2] = {m_run[0], m_run[1]};
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      mx[0] = fmaxf(mx[0], fmaxf(s[i][0], s[i][1]));
-      mx[1] = fmaxf(mx[1], fmaxf(s[i][2], s[i][3]));
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
-      mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
-    }
-    float corr[2], msc[2];
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      corr[r] = exp2f((m_run[r] - mx[r]) * sc);  // first tile: exp2(-inf) = 0
-      m_run[r] = mx[r];
-      msc[r] = mx[r] * sc;
-      l_run[r] *= corr[r];
-    }
-    float rs[2] = {0.f, 0.f};
-    uint32_t pf[4][4];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float p0 = exp2f(fmaf(s[i][0], sc, -msc[0]));
-      const float p1 = exp2f(fmaf(s[i][1], sc, -msc[0]));
-      const float p2 = exp2f(fmaf(s[i][2], sc, -msc[1]));
-      const float p3 = exp2f(fmaf(s[i][3], sc, -msc[1]));
-      rs[0] += p0 + p1;
-      rs[1] += p2 + p3;
-      // accumulator layout of two adjacent n-tiles == A-operand layout of one 16-wide k-step
-      pf[i >> 1][(i & 1) * 2 + 0] = pack_half2(p0, p1);
-      pf[i >> 1][(i & 1) * 2 + 1] = pack_half2(p2, p3);
-    }
-    l_run[0] += rs[0];
-    l_run[1] += rs[1];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      o[i][0] *= corr[0]; o[i][1] *= corr[0];
-      o[i][2] *= corr[1]; o[i][3] *= corr[1];
-    }
-    // O += P V : 4 k-steps (16 keys) x 8 n-tiles (8 head dims); V read transposed by ldmatrix
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-#pragma unroll
-      for (int np = 0; np < 4; ++np) {
-        uint32_t b0, b1, b2, b3;
-        const int r = ks * 16 + (lane & 7) + ((lane >> 3) & 1) * 8;  // key row
-        const int ch = np * 2 + (lane >> 4);                          // head-dim chunk
-        ldmatrix_x4_trans(sw128_addr(vt, r, ch), b0, b1, b2, b3);
-        mma_m16n8k16_f16(o[np * 2], pf[ks], b0, b1);
-        mma_m16n8k16_f16(o[np * 2 + 1], pf[ks], b2, b3);
-      }
-    }
-    __syncthreads();  // all warps done with stage `st` before it is refilled
-  }
-
-  // finalise: row sums across the 4 lanes of a quad, normalise, store f16
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 1);
-    l_run[r] += __shfl_xor_sync(0xffffffffu, l_run[r], 2);
-  }
-  const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
-  const int row0 = q0 + warp * 16 + (lane >> 2);
-  __half* og = out + (long long)b * T * d + h * ATT_D + (lane & 3) * 2;
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    if (row0 < T)
-      *reinterpret_cast<uint32_t*>(og + (long long)row0 * d + i * 8) = pack_half2(o[i][0] * inv0, o[i][1] * inv0);
-    if (row0 + 8 < T)
-      *reinterpret_cast<uint32_t*>(og + (long long)(row0 + 8) * d + i * 8) = pack_half2(o[i][2] * inv1, o[i][3] * inv1);
   }
 }
 
@@ -413,16 +239,6 @@ int launch_layernorm(const float* x, const float* g, const float* b, void* y, in
   return DSS_OK;
 }
 
-int launch_attention(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st) {
-  DSS_REQUIRE(B > 0 && T > 0 && heads > 0, "attention: empty problem");
-  dim3 grid(cdiv(T, ATT_BM), heads, B);
-  LaunchScope scope(st, KC_ATTENTION);
-  attention_f16_kernel<<<grid, ATT_THREADS, 0, st>>>(reinterpret_cast<const __half*>(qkv),
-                                                     reinterpret_cast<__half*>(out), T, heads);
-  DSS_CHECK_CUDA(cudaGetLastError());
-  return DSS_OK;
-}
-
 }  // namespace dss
 
 using namespace dss;
@@ -430,9 +246,6 @@ using namespace dss;
 extern "C" int dss_op_layernorm_f16(const float* x, const float* gamma, const float* beta, void* y, int M, int d,
                                     float eps, dss_stream_t stream) {
   return launch_layernorm(x, gamma, beta, y, M, d, eps, static_cast<cudaStream_t>(stream));
-}
-extern "C" int dss_op_attention_f16(const void* qkv, void* out, int B, int T, int heads, dss_stream_t stream) {
-  return launch_attention(qkv, out, B, T, heads, static_cast<cudaStream_t>(stream));
 }
 extern "C" int dss_op_im2col_f16(const uint8_t* images_u8, void* patches, int B, int H, int W, int P,
                                  dss_stream_t stream) {

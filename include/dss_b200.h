@@ -156,16 +156,11 @@ int dss_debug_gemm_schedule(const void* A, const void* Wt, const float* bias, vo
  * trace_bytes smaller than needed is rejected (DSS_ERR_BAD_ARG, the message names the size). */
 int dss_debug_gemm_trace(const void* A, const void* Wt, const float* bias, void* out, int M, int N, int K, int epilogue,
                          int schedule, unsigned long long* trace, size_t trace_bytes, dss_stream_t stream);
-/* LayerNorm fused into the GEMM's A-operand producer (the qkv / fc1 layers of ViT-S; K must be 384):
- * out f16 [M, N] = (gelu ? gelu_erf : id)(LayerNorm(x f32 [M, K]; gamma, beta, eps) @ Wt f16 [N, K]^T + bias); N % 128 == 0 */
-int dss_op_gemm_ln_f16(const float* x, const float* gamma, const float* beta, const void* Wt, const float* bias,
-                       void* out, int M, int N, int K, float eps, int gelu, dss_stream_t stream);
 /* y f16 [M, d] = LayerNorm(x f32 [M, d]) * gamma + beta, d in {384, 768} */
 int dss_op_layernorm_f16(const float* x, const float* gamma, const float* beta, void* y, int M, int d, float eps,
                          dss_stream_t stream);
-/* qkv f16 [B, T, 3*d] (q | k | v, heads of 64 inside each) -> out f16 [B, T, d] = softmax(q k^T / 8) v */
-int dss_op_attention_f16(const void* qkv, void* out, int B, int T, int heads, dss_stream_t stream);
-/* same contract on wgmma (TMA-fed QK^T and PV, S, P and O in registers); the ViT forward uses this one */
+/* qkv f16 [B, T, 3*d] (q | k | v, heads of 64 inside each) -> out f16 [B, T, d] = softmax(q k^T / 8) v, d = 64 * heads,
+ * on wgmma (TMA-fed QK^T and PV, S, P and O in registers); the attention of the ViT forward */
 int dss_op_attention_tc_f16(const void* qkv, void* out, int B, int T, int heads, dss_stream_t stream);
 /* images_u8 [B,H,W,3] -> patches f16 [B*N, 3*P*P], column order (c, py, px), normalised */
 int dss_op_im2col_f16(const uint8_t* images_u8, void* patches, int B, int H, int W, int P, dss_stream_t stream);

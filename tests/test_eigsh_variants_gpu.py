@@ -3,10 +3,10 @@
 csrc/eigsh.cu compiles lanczos_laplacian_kernel three times: <4, 1, 512> (variant 2, the default), <2, 2, 512> (variant 1)
 and <4, 2, 256> (variant 3). The paired ones run two CTAs per SM with their own rows per warp and pass, load-group
 width, warp count (so their own order of combining the column accumulators and every block sum) and grid (2 x SMs
-CTAs, each with its own basis slice). DSS_EIG_VARIANT is read once per process, so only the debug entry reaches them
-from a test. Here they get the edge battery of test_eigsh_edges_gpu.py, with its float64 truth and tolerances, and the
-geometry of the pairing itself: batches around 2 x SMs, the benchmark's step, the shared-memory limit of the pairing
-and the workspace it needs. Variant 2 through the debug entry is the control: bitwise the product entry points."""
+CTAs, each with its own basis slice). Here they get the edge battery of test_eigsh_edges_gpu.py, with its float64 truth
+and tolerances, and the geometry of the pairing itself: batches around 2 x SMs, the benchmark's step, the shared-memory
+limit of the pairing and the workspace it needs. Variant 2 through the debug entry is the control: bitwise the product
+entry points."""
 import numpy as np
 import pytest
 import torch

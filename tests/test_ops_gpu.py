@@ -96,7 +96,7 @@ def test_layernorm(cuda, d):
     assert err <= 1e-3 * ref.abs().max().item() + 1e-3, err   # fp16 output rounding only
 
 
-@pytest.mark.parametrize("impl", ["dss_op_attention_tc_f16", "dss_op_attention_f16"])
+@pytest.mark.parametrize("impl", ["dss_op_attention_tc_f16"])
 @pytest.mark.parametrize("B,T,heads", [(1, 64, 6), (2, 197, 6), (2, 901, 6), (1, 130, 12), (3, 257, 6), (4, 577, 6),
                                        (40, 901, 6), (30, 257, 6), (70, 100, 6)])
 def test_attention(cuda, B, T, heads, impl):
