@@ -42,6 +42,7 @@ PROTOTYPES = {
     "dss_profile_read": (c_int, [C.POINTER(ProfileEntry), c_int]),
     "dss_vit_create": (c_int, [C.POINTER(VitConfig), C.POINTER(c_void_p)]),
     "dss_vit_destroy": (None, [c_void_p]),
+    "dss_vit_set_precision": (c_int, [c_void_p, c_int]),
     "dss_vit_load_weights": (c_int, [c_void_p, C.POINTER(VitWeights), c_void_p]),
     "dss_vit_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int]),
     "dss_vit_forward_k": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
@@ -63,6 +64,11 @@ PROTOTYPES = {
     "dss_op_layernorm_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
     "dss_op_attention_tc_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "dss_op_im2col_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
+    "dss_op_split_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "dss_op_layernorm_split_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_float, c_void_p]),
+    "dss_op_gelu_split_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "dss_op_im2col_split_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p]),
+    "dss_op_attention_split_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "dss_affinity_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "dss_affinity": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p, c_int, c_void_p,
                              c_void_p, c_size_t, c_void_p]),
@@ -121,6 +127,7 @@ AFF_NORMALIZE, AFF_THRESHOLD_AT_ZERO, AFF_NO_MAX_SCALE = 1, 2, 4
 LOC_OK, LOC_NO_GRID, LOC_SEED_IN_BACKGROUND, LOC_EMPTY_COMPONENT = range(4)
 SEGEVAL_SEMANTIC, SEGEVAL_BINARY, SEGEVAL_FIELDS = 0, 1, 13
 DSS_ERR_UNSUPPORTED = -4
+VIT_PRECISION = {"fp16": 0, "fp32": 1}   # DSS_VIT_PRECISION_FP16 / _FP32
 
 _lib = None
 

@@ -53,11 +53,7 @@ rownorm_split_kernel(const float* __restrict__ f, __half* __restrict__ S, unsign
   for (int k = lane; k < dpad; k += 32) {
     float v = 0.f;
     if (k < d) v = normalize ? x[k] / denom : x[k] * pre;
-    const __half hi = __float2half_rn(v);
-    const float hif = __half2float(hi);
-    s[k] = hi;
-    s[dpad + k] = __float2half_rn(hif * 0.015625f);
-    s[2 * dpad + k] = __float2half_rn((v - hif) * 64.0f);
+    split_f16(v, s[k], s[dpad + k], s[2 * dpad + k]);
     s2 = fmaf(v, v, s2);
   }
   s2 = warp_sum(s2);

@@ -60,6 +60,15 @@ int launch_cls_attention(const void* qkv, int B, int T, int heads, float* out, c
 int launch_cls_row(float* x, const float* cls, const float* pos, int B, int T, int d, cudaStream_t st);
 int launch_layernorm(const float* x, const float* g, const float* b, void* y, int M, int d, float eps, cudaStream_t st);
 int launch_attention_tc(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st);
+// split-fp16 operands of DSS_VIT_PRECISION_FP32 (vit_split.cu, attention_split.cu)
+int launch_split_rows(const float* x, void* out, long long rows, int cols, int order, cudaStream_t st, int kclass);
+int launch_im2col_split(const uint8_t* img, void* patches, int B, int H, int W, int P, int pad, cudaStream_t st);
+int launch_layernorm_split(const float* x, const float* g, const float* b, void* y, int M, int d, float eps,
+                           cudaStream_t st);
+int launch_gelu_split(const float* h, void* out, long long M, int n, cudaStream_t st);
+int launch_qkv_split(const float* qkv, void* out, long long M, int d, cudaStream_t st);
+int launch_attention_split(const void* qkv_split, void* out, int B, int T, int heads, cudaStream_t st);
+int launch_cls_attention_f32(const float* qkv, int B, int T, int heads, float* out, cudaStream_t st);
 
 // ---------------------------------------------------------------- launch accounting / per-class device timing
 enum KernelClass {
@@ -307,6 +316,23 @@ __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.
 __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   __half2 h = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&h);
+}
+
+// Split-fp16 operand format (the affinity's Gram product and the fp32-precision ViT): x = hi + lo, hi = fp16(x),
+// lo = x - hi (exact in fp32, |lo| <= 2^-11 |x|), stored as the three fp16 values hi, hi/64 and 64 lo. A product of
+// an A-order row [hi | hi/64 | 64 lo] with a B-order row [hi' | 64 lo' | hi'/64] is hi hi' + hi lo' + lo hi' (lo lo'
+// dropped); the 2^+-6 factors keep the small terms above the fp16 subnormal range for |x| >= 2^-8 (DESIGN.md section 3).
+struct SplitF16 { __half hi, hi_s, lo_s; };   // hi, hi / 64, 64 lo
+__device__ __forceinline__ void split_f16(float v, __half& hi, __half& hi_s, __half& lo_s) {
+  hi = __float2half_rn(v);
+  const float hif = __half2float(hi);
+  hi_s = __float2half_rn(hif * 0.015625f);
+  lo_s = __float2half_rn((v - hif) * 64.0f);
+}
+__device__ __forceinline__ SplitF16 split_f16(float v) {
+  SplitF16 s;
+  split_f16(v, s.hi, s.hi_s, s.lo_s);
+  return s;
 }
 
 // Exact-erf GELU, branch-free:  gelu(x) = x Phi(x) = relu(x) - |x| q(|x|),  q(a) = 0.5 erfc(a / sqrt 2) = 2^P(u),

@@ -5,6 +5,8 @@
 // Per block:  LN1 -> [wgmma GEMM] qkv (f16) -> wgmma flash attention -> [wgmma GEMM + residual] proj
 //             LN2 -> [wgmma GEMM + GELU] fc1 (f16) -> [wgmma GEMM + residual] fc2
 // The residual stream stays fp32; GEMM operands are fp16 (11-bit significand, same as TF32), accumulation fp32.
+// DSS_VIT_PRECISION_FP32 (dss_vit_set_precision) runs the same blocks on split-fp16 operands (vit_split.cu,
+// attention_split.cu): fp32-equivalent products on the fp16 tensor cores at three times the tensor-core work.
 // The block the reference hooks is pruned to LN1 + the K third of its qkv projection, CLS row dropped in the
 // GEMM epilogue, which writes the fp32 features directly in the reference's [B, N, d] layout.
 #include <math.h>
@@ -51,6 +53,7 @@ struct BlockW {
 
 struct dss_vit {
   dss_vit_config cfg;
+  int precision = DSS_VIT_PRECISION_FP16;   // DSS_VIT_PRECISION_FP32: every weight packed as split fp16 (vit_split.cu)
   bool loaded = false;
   void* arena = nullptr;  // one device allocation holding every packed weight
   size_t arena_bytes = 0;
@@ -157,6 +160,9 @@ static int get_pos(dss_vit* h, int Hp, int Wp, bool square, cudaStream_t st, flo
   return DSS_OK;
 }
 
+// DSS_VIT_PRECISION_FP32 (split): patches, xn and attn hold three fp16 groups per value (A order), qkv holds the
+// split attention operands [B*T, 9d] and, after attention, the split MLP hidden activations [B*T, 12d] (the same
+// buffer), and f32 holds the fp32 GEMM outputs that are split next: qkv [B*T, 3d], then the fc1 output [B*T, 4d].
 struct VitWs {
   __half* patches;  // [B*Np, 3P^2]
   float* x;         // [B*T, d]     residual stream
@@ -164,10 +170,11 @@ struct VitWs {
   __half* attn;     // [B*T, d]     attention output (GEMM A operand)
   __half* qkv;      // [B*T, 3d]
   __half* hid;      // [B*T, 4d]
+  float* f32;       // split only
   size_t total;
 };
 
-static VitWs carve(const dss_vit_config& c, int B, int Hp, int Wp, void* base) {
+static VitWs carve(const dss_vit_config& c, int B, int Hp, int Wp, void* base, int precision) {
   const int Np = Hp * Wp, T = Np + 1, d = c.dim;
   const size_t M = (size_t)B * T;
   uint8_t* p = reinterpret_cast<uint8_t*>(base);
@@ -178,14 +185,106 @@ static VitWs carve(const dss_vit_config& c, int B, int Hp, int Wp, void* base) {
     return r;
   };
   VitWs w;
+  const size_t hd = (size_t)c.mlp_ratio * d;
+  if (precision == DSS_VIT_PRECISION_FP32) {
+    w.patches = reinterpret_cast<__half*>(take((size_t)B * Np * 9 * c.patch * c.patch * 2));
+    w.x = reinterpret_cast<float*>(take(M * d * 4));
+    w.xn = reinterpret_cast<__half*>(take(M * 3 * d * 2));
+    w.attn = reinterpret_cast<__half*>(take(M * 3 * d * 2));
+    w.qkv = w.hid = reinterpret_cast<__half*>(take(M * std::max<size_t>(9 * d, 3 * hd) * 2));
+    w.f32 = reinterpret_cast<float*>(take(M * std::max<size_t>(3 * d, hd) * 4));
+    w.total = off;
+    return w;
+  }
   w.patches = reinterpret_cast<__half*>(take((size_t)B * Np * 3 * c.patch * c.patch * 2));
   w.x = reinterpret_cast<float*>(take(M * d * 4));
   w.xn = reinterpret_cast<__half*>(take(M * d * 2));
   w.attn = reinterpret_cast<__half*>(take(M * d * 2));
   w.qkv = reinterpret_cast<__half*>(take(M * 3 * d * 2));
   w.hid = reinterpret_cast<__half*>(take(M * (size_t)c.mlp_ratio * d * 2));
+  w.f32 = nullptr;
   w.total = off;
   return w;
+}
+
+// modes 1 and 2 after the blocks: the residual stream, or the final LayerNorm of the CLS rows
+static int vit_tail(const dss_vit* h, const float* x, int mode, float* out, int B, int T, cudaStream_t st) {
+  const int d = h->cfg.dim;
+  if (mode == 2) {
+    // upstream VisionTransformer.forward: x = norm(x); return x[:, 0]  (LayerNorm is row-wise: only the CLS rows)
+    DSS_REQUIRE(h->norm_w && h->norm_b, "vit: the final LayerNorm weights (norm.weight / norm.bias) were not loaded");
+    LaunchScope scope(st, KC_LAYERNORM);
+    layernorm_rows_f32_kernel<<<cdiv(B, 4), 128, 0, st>>>(x, (long long)T * d, h->norm_w, h->norm_b, out, B, d,
+                                                          h->cfg.ln_eps);
+    DSS_CHECK_CUDA(cudaGetLastError());
+  } else {
+    DSS_CHECK_CUDA(cudaMemcpyAsync(out, x, (size_t)B * T * d * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  }
+  return DSS_OK;
+}
+
+// vit_run of DSS_VIT_PRECISION_FP32: the same sequence on split operands. Every GEMM runs the fp16 path's kernel and
+// epilogue at K' = 3 K; the qkv and fc1 GEMMs write fp32 (DSS_EPI_BIAS_F32), which qkv_split_kernel /
+// gelu_split_kernel turn into the next product's split operands.
+static int vit_run_split(dss_vit* h, const VitWs& w, const uint8_t* img, int B, int H, int W, int Hp, int Wp,
+                         int n_full, int mode, float* out, const float* pos, cudaStream_t st, int pad, int which,
+                         float* cls_attn) {
+  const dss_vit_config& c = h->cfg;
+  const int P = c.patch, d = c.dim, hd = c.mlp_ratio * d;
+  const int Np = Hp * Wp, T = Np + 1, M = B * T, Kp = 3 * P * P;
+  int rc;
+  CUtensorMap tm_patches, tm_xn, tm_attn, tm_hid, tm_x_out, tm_qkv_out, tm_hid_out;
+  if ((rc = make_tmap_f16(&tm_patches, w.patches, B * Np, 3 * Kp, 128))) return rc;
+  if ((rc = make_tmap_f16(&tm_xn, w.xn, M, 3 * d, 128))) return rc;
+  if ((rc = make_tmap_f16(&tm_attn, w.attn, M, 3 * d, 128))) return rc;
+  if ((rc = make_tmap_f16(&tm_hid, w.hid, M, 3 * hd, 128))) return rc;
+  if ((rc = make_tmap_out(&tm_x_out, w.x, M, d, 1))) return rc;
+  if ((rc = make_tmap_out(&tm_qkv_out, w.f32, M, 3 * d, 1))) return rc;
+  if ((rc = make_tmap_out(&tm_hid_out, w.f32, M, hd, 1))) return rc;
+
+  if ((rc = launch_im2col_split(img, w.patches, B, H, W, P, pad, st))) return rc;
+  if ((rc = gemm_f16_tc(tm_patches, h->tm_patch, nullptr, h->patch_b, w.x, B * Np, d, 3 * Kp, DSS_EPI_PATCH_F32, pos, Np,
+                        T, st, KC_GEMM_PATCH, 128)))
+    return rc;
+  if ((rc = launch_cls_row(w.x, h->cls, pos, B, T, d, st))) return rc;
+  auto qkv_f32 = [&](const BlockW& bw) {
+    return gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, w.f32, M, 3 * d, 3 * d, DSS_EPI_BIAS_F32, nullptr, 0, 0, st,
+                       KC_GEMM_QKV, gemm_tile_n());
+  };
+  for (int l = 0; l < n_full; ++l) {
+    const BlockW& bw = h->blocks[l];
+    if ((rc = launch_layernorm_split(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
+    if ((rc = qkv_f32(bw))) return rc;
+    if ((rc = launch_qkv_split(w.f32, w.qkv, M, d, st))) return rc;
+    if ((rc = launch_attention_split(w.qkv, w.attn, B, T, c.heads, st))) return rc;
+    if ((rc = gemm_f16_tc(tm_attn, bw.tm_proj, &tm_x_out, bw.proj_b, w.x, M, d, 3 * d, DSS_EPI_BIAS_RESID_F32, nullptr, 0,
+                          0, st, KC_GEMM_PROJ, gemm_tile_n())))
+      return rc;
+    if ((rc = launch_layernorm_split(w.x, bw.ln2_w, bw.ln2_b, w.xn, M, d, c.ln_eps, st))) return rc;
+    if ((rc = gemm_f16_tc(tm_xn, bw.tm_fc1, &tm_hid_out, bw.fc1_b, w.f32, M, hd, 3 * d, DSS_EPI_BIAS_F32, nullptr, 0, 0,
+                          st, KC_GEMM_FC1, gemm_tile_n())))
+      return rc;
+    if ((rc = launch_gelu_split(w.f32, w.hid, M, hd, st))) return rc;
+    if ((rc = gemm_f16_tc(tm_hid, bw.tm_fc2, &tm_x_out, bw.fc2_b, w.x, M, d, 3 * hd, DSS_EPI_BIAS_RESID_F32, nullptr, 0,
+                          0, st, KC_GEMM_FC2, gemm_tile_n())))
+      return rc;
+  }
+  if (mode == 0 || mode == 3) {
+    const BlockW& bw = h->blocks[n_full];
+    if ((rc = launch_layernorm_split(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
+    if (out) {
+      const CUtensorMap& tm = which == 0 ? bw.tm_q : (which == 1 ? bw.tm_k : bw.tm_v);
+      if ((rc = gemm_f16_tc(tm_xn, tm, nullptr, bw.qkv_b + (size_t)which * d, out, M, d, 3 * d, DSS_EPI_DROPCLS_F32,
+                            nullptr, T, Np, st, KC_GEMM_KPROJ, 128)))
+        return rc;
+    }
+    if (mode == 3 && cls_attn) {
+      if ((rc = qkv_f32(bw))) return rc;
+      if ((rc = launch_cls_attention_f32(w.f32, B, T, c.heads, cls_attn, st))) return rc;
+    }
+    return DSS_OK;
+  }
+  return vit_tail(h, w.x, mode, out, B, T, st);
 }
 
 // mode 0: K projection of block n_full (features), 1: residual stream [B, T, d], 2: final-norm CLS token [B, d],
@@ -202,7 +301,7 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   DSS_REQUIRE(B > 0 && Hp > 0 && Wp > 0, "vit: image %dx%d smaller than one %d-pixel patch", H, W, P);
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "vit: workspace must be 256-byte aligned");
   const int Np = Hp * Wp, T = Np + 1, M = B * T;
-  VitWs w = carve(c, B, Hp, Wp, ws);
+  VitWs w = carve(c, B, Hp, Wp, ws, h->precision);
   if (ws_bytes < w.total) {
     set_error("vit: workspace too small (%zu < %zu)", ws_bytes, w.total);
     return DSS_ERR_WORKSPACE;
@@ -213,6 +312,8 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   // sees them, so their patch grid decides; the model's own forward (box crops) and the token hook take the image as is
   const bool square = (mode == 1 || mode == 2) ? H == W : Hp == Wp;
   if ((rc = get_pos(h, Hp, Wp, square, st, &pos))) return rc;
+  if (h->precision == DSS_VIT_PRECISION_FP32)
+    return vit_run_split(h, w, img, B, H, W, Hp, Wp, n_full, mode, out, pos, st, pad, which, cls_attn);
 
   CUtensorMap tm_patches, tm_xn, tm_attn, tm_hid;
   const int Kp = 3 * P * P;
@@ -275,14 +376,8 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
         return rc;
       if ((rc = launch_cls_attention(w.qkv, B, T, c.heads, cls_attn, st))) return rc;
     }
-  } else if (mode == 2) {
-    // upstream VisionTransformer.forward: x = norm(x); return x[:, 0]  (LayerNorm is row-wise: only the CLS rows)
-    DSS_REQUIRE(h->norm_w && h->norm_b, "vit: the final LayerNorm weights (norm.weight / norm.bias) were not loaded");
-    LaunchScope scope(st, KC_LAYERNORM);
-    layernorm_rows_f32_kernel<<<cdiv(B, 4), 128, 0, st>>>(w.x, (long long)T * d, h->norm_w, h->norm_b, out, B, d, c.ln_eps);
-    DSS_CHECK_CUDA(cudaGetLastError());
   } else {
-    DSS_CHECK_CUDA(cudaMemcpyAsync(out, w.x, (size_t)M * d * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    return vit_tail(h, w.x, mode, out, B, T, st);
   }
   return DSS_OK;
 }
@@ -311,11 +406,24 @@ extern "C" void dss_vit_destroy(dss_vit_t* h) {
   delete h;
 }
 
+extern "C" int dss_vit_set_precision(dss_vit_t* h, int precision) {
+  DSS_REQUIRE(h, "vit_set_precision: null handle");
+  DSS_REQUIRE(precision == DSS_VIT_PRECISION_FP16 || precision == DSS_VIT_PRECISION_FP32,
+              "vit_set_precision: precision must be DSS_VIT_PRECISION_FP16 (0) or DSS_VIT_PRECISION_FP32 (1), got %d",
+              precision);
+  DSS_REQUIRE(!h->arena, "vit_set_precision: the weights are already packed for precision %d; set the precision "
+              "before dss_vit_load_weights", h->precision);
+  h->precision = precision;
+  return DSS_OK;
+}
+
 extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_stream_t stream) {
   DSS_REQUIRE(h && w && w->blocks, "vit_load_weights: null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const dss_vit_config& c = h->cfg;
   const size_t d = c.dim, P = c.patch, hid = (size_t)c.mlp_ratio * d, Kp = 3 * P * P;
+  // split weights (DSS_VIT_PRECISION_FP32): every row [hi | 64 lo | hi/64], three times as wide
+  const size_t ks = h->precision == DSS_VIT_PRECISION_FP32 ? 3 : 1;
   // arena layout: f16 weights first (1 KB aligned for TMA), then fp32 vectors
   size_t off = 0;
   auto reserve = [&](size_t bytes) {
@@ -323,13 +431,13 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     off += align_up(bytes, 1024);
     return o;
   };
-  const size_t o_patch_w = reserve(d * Kp * 2), o_patch_b = reserve(d * 4), o_cls = reserve(d * 4);
+  const size_t o_patch_w = reserve(d * Kp * 2 * ks), o_patch_b = reserve(d * 4), o_cls = reserve(d * 4);
   const size_t o_norm_w = reserve(d * 4), o_norm_b = reserve(d * 4);
   struct Off { size_t qkv_w, proj_w, fc1_w, fc2_w, ln1_w, ln1_b, ln2_w, ln2_b, qkv_b, proj_b, fc1_b, fc2_b; };
   std::vector<Off> bo(c.depth);
   for (int l = 0; l < c.depth; ++l) {
-    bo[l].qkv_w = reserve(3 * d * d * 2); bo[l].proj_w = reserve(d * d * 2);
-    bo[l].fc1_w = reserve(hid * d * 2); bo[l].fc2_w = reserve(d * hid * 2);
+    bo[l].qkv_w = reserve(3 * d * d * 2 * ks); bo[l].proj_w = reserve(d * d * 2 * ks);
+    bo[l].fc1_w = reserve(hid * d * 2 * ks); bo[l].fc2_w = reserve(d * hid * 2 * ks);
     bo[l].ln1_w = reserve(d * 4); bo[l].ln1_b = reserve(d * 4); bo[l].ln2_w = reserve(d * 4); bo[l].ln2_b = reserve(d * 4);
     bo[l].qkv_b = reserve(3 * d * 4); bo[l].proj_b = reserve(d * 4); bo[l].fc1_b = reserve(hid * 4); bo[l].fc2_b = reserve(d * 4);
   }
@@ -339,8 +447,10 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     h->arena_bytes = off;
   }
   uint8_t* base = reinterpret_cast<uint8_t*>(h->arena);
-  auto cvt = [&](const float* src, size_t o, size_t n) -> int {
+  // weight [rows, n / rows] fp32 -> fp16 operand at offset o
+  auto cvt = [&](const float* src, size_t o, size_t n, size_t rows) -> int {
     DSS_REQUIRE(src, "vit_load_weights: null weight pointer");
+    if (ks == 3) return launch_split_rows(src, base + o, (long long)rows, (int)(n / rows), 1, st, KC_MISC);
     LaunchScope scope(st, KC_MISC);
     f32_to_f16_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(src, reinterpret_cast<__half*>(base + o), n);
     DSS_CHECK_CUDA(cudaGetLastError());
@@ -352,7 +462,7 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     return DSS_OK;
   };
   int rc;
-  if ((rc = cvt(w->patch_w, o_patch_w, d * Kp))) return rc;
+  if ((rc = cvt(w->patch_w, o_patch_w, d * Kp, d))) return rc;
   if ((rc = cpy(w->patch_b, o_patch_b, d))) return rc;
   if ((rc = cpy(w->cls_token, o_cls, d))) return rc;
   h->patch_w = reinterpret_cast<__half*>(base + o_patch_w);
@@ -365,15 +475,15 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     h->norm_w = reinterpret_cast<float*>(base + o_norm_w);
     h->norm_b = reinterpret_cast<float*>(base + o_norm_b);
   }
-  if ((rc = make_tmap_f16(&h->tm_patch, h->patch_w, (int)d, (int)Kp, 128 / 2))) return rc;
+  if ((rc = make_tmap_f16(&h->tm_patch, h->patch_w, (int)d, (int)(Kp * ks), 128 / 2))) return rc;
   h->blocks.resize(c.depth);
   for (int l = 0; l < c.depth; ++l) {
     const dss_vit_block_weights& s = w->blocks[l];
     BlockW& b = h->blocks[l];
-    if ((rc = cvt(s.qkv_w, bo[l].qkv_w, 3 * d * d))) return rc;
-    if ((rc = cvt(s.proj_w, bo[l].proj_w, d * d))) return rc;
-    if ((rc = cvt(s.fc1_w, bo[l].fc1_w, hid * d))) return rc;
-    if ((rc = cvt(s.fc2_w, bo[l].fc2_w, d * hid))) return rc;
+    if ((rc = cvt(s.qkv_w, bo[l].qkv_w, 3 * d * d, 3 * d))) return rc;
+    if ((rc = cvt(s.proj_w, bo[l].proj_w, d * d, d))) return rc;
+    if ((rc = cvt(s.fc1_w, bo[l].fc1_w, hid * d, hid))) return rc;
+    if ((rc = cvt(s.fc2_w, bo[l].fc2_w, d * hid, d))) return rc;
     if ((rc = cpy(s.ln1_w, bo[l].ln1_w, d))) return rc;
     if ((rc = cpy(s.ln1_b, bo[l].ln1_b, d))) return rc;
     if ((rc = cpy(s.ln2_w, bo[l].ln2_w, d))) return rc;
@@ -390,13 +500,14 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     b.ln2_w = reinterpret_cast<float*>(base + bo[l].ln2_w); b.ln2_b = reinterpret_cast<float*>(base + bo[l].ln2_b);
     b.qkv_b = reinterpret_cast<float*>(base + bo[l].qkv_b); b.proj_b = reinterpret_cast<float*>(base + bo[l].proj_b);
     b.fc1_b = reinterpret_cast<float*>(base + bo[l].fc1_b); b.fc2_b = reinterpret_cast<float*>(base + bo[l].fc2_b);
-    if ((rc = make_tmap_f16(&b.tm_qkv, b.qkv_w, (int)(3 * d), (int)d, gemm_tile_n() / 2))) return rc;
-    if ((rc = make_tmap_f16(&b.tm_k, b.qkv_w + d * d, (int)d, (int)d, 128 / 2))) return rc;
-    if ((rc = make_tmap_f16(&b.tm_q, b.qkv_w, (int)d, (int)d, 128 / 2))) return rc;
-    if ((rc = make_tmap_f16(&b.tm_v, b.qkv_w + 2 * d * d, (int)d, (int)d, 128 / 2))) return rc;
-    if ((rc = make_tmap_f16(&b.tm_proj, b.proj_w, (int)d, (int)d, gemm_tile_n() / 2))) return rc;
-    if ((rc = make_tmap_f16(&b.tm_fc1, b.fc1_w, (int)hid, (int)d, gemm_tile_n() / 2))) return rc;
-    if ((rc = make_tmap_f16(&b.tm_fc2, b.fc2_w, (int)d, (int)hid, gemm_tile_n() / 2))) return rc;
+    const int kd = (int)(d * ks), khid = (int)(hid * ks);   // row widths of the packed weights
+    if ((rc = make_tmap_f16(&b.tm_qkv, b.qkv_w, (int)(3 * d), kd, gemm_tile_n() / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_k, b.qkv_w + d * kd, (int)d, kd, 128 / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_q, b.qkv_w, (int)d, kd, 128 / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_v, b.qkv_w + 2 * d * kd, (int)d, kd, 128 / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_proj, b.proj_w, (int)d, kd, gemm_tile_n() / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_fc1, b.fc1_w, (int)hid, kd, gemm_tile_n() / 2))) return rc;
+    if ((rc = make_tmap_f16(&b.tm_fc2, b.fc2_w, (int)d, khid, gemm_tile_n() / 2))) return rc;
   }
   // host copy of the positional grid for interpolation; drop stale interpolations
   const size_t npos = ((size_t)c.grid0 * c.grid0 + 1) * d;
@@ -413,14 +524,14 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
 
 extern "C" size_t dss_vit_workspace_bytes(const dss_vit_t* h, int B, int H, int W) {
   if (!h || B <= 0 || H < h->cfg.patch || W < h->cfg.patch) return 0;
-  return carve(h->cfg, B, H / h->cfg.patch, W / h->cfg.patch, nullptr).total;
+  return carve(h->cfg, B, H / h->cfg.patch, W / h->cfg.patch, nullptr, h->precision).total;
 }
 
 extern "C" size_t dss_vit_forward_last_workspace_bytes(const dss_vit_t* h, int B, int H, int W, int pad) {
   if (!h || B <= 0 || H <= 0 || W <= 0) return 0;
   const int P = h->cfg.patch;
   if (!pad) return dss_vit_workspace_bytes(h, B, H, W);
-  return carve(h->cfg, B, cdiv(H, P), cdiv(W, P), nullptr).total;
+  return carve(h->cfg, B, cdiv(H, P), cdiv(W, P), nullptr, h->precision).total;
 }
 
 extern "C" int dss_vit_forward_last(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, int pad, int which,

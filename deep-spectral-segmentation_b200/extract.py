@@ -24,6 +24,7 @@ import torch
 
 from . import _lib, cluster, io_pipeline, segment, spectral
 from . import extract_utils as utils
+from . import vit as vit_mod
 
 torch.set_grad_enabled(False)  # extract.py:838
 
@@ -114,9 +115,10 @@ class _Batcher:
 def extract_features(images_list: str, images_root: Optional[str], model_name: str, batch_size: int, output_dir: str,
                      which_block: int = -1, checkpoint: Optional[str] = None, seed: Optional[int] = None,
                      random_init: bool = False, yes: Optional[bool] = None, num_workers: Optional[int] = None,
-                     num_workers_out: int = 4, writer: str = "process"):
+                     num_workers_out: int = 4, writer: str = "process", precision: str = "fp16"):
     """
-    Extract features from a list of images.
+    Extract features from a list of images. ``precision='fp32'`` computes the ViT on split-fp16 operands and
+    reproduces the fp32 model's features (see vit.DinoViT); the default 'fp16' is the faster path.
 
     Example:
         python extract.py extract_features \
@@ -126,13 +128,14 @@ def extract_features(images_list: str, images_root: Optional[str], model_name: s
             --model_name dino_vits16 \
             --batch_size 1
     """
+    vit_mod.check_precision(precision)
     utils.make_output_dir(output_dir, assume_yes=yes)
     model_name = model_name.lower()
     if not ("dino" in model_name or "mocov3" in model_name):
         raise ValueError(model_name)
     dev = _device()
     model, _, patch_size, _ = utils.get_model(model_name, checkpoint=checkpoint, seed=seed, device=dev,
-                                              random_init=random_init)
+                                              random_init=random_init, precision=precision)
     filenames = Path(images_list).read_text().splitlines()
     dataset = utils.ImagesDataset(filenames=filenames, images_root=images_root)
     print(f"Dataset size: {len(dataset)=}")
@@ -477,10 +480,11 @@ def extract_multi_region_segmentations(features_dir: str, eigs_dir: str, output_
 # ---------------------------------------------------------------------------------------------------------------
 def extract_bbox_features(images_root: str, bbox_file: str, model_name: str, output_file: str,
                           checkpoint: Optional[str] = None, seed: Optional[int] = None, random_init: bool = False,
-                          batch_size: int = 64):
+                          batch_size: int = 64, precision: str = "fp16"):
     """
     DINO CLS embedding of every bounding-box crop (reference extract/extract.py:500-544), same command / file
     contract: each dict of ``bbox_file`` gains 'features' [n_boxes, d] fp32. Crops of equal size are batched.
+    ``precision``: ViT arithmetic, as in extract_features.
 
     Example:
         python extract.py extract_bbox_features \
@@ -490,12 +494,13 @@ def extract_bbox_features(images_root: str, bbox_file: str, model_name: str, out
             --output_file "./data/VOC2012/multi_region_bboxes/fixed/bbox_features_e2_d5.pth" \
     """
     from PIL import Image
+    vit_mod.check_precision(precision)
     bbox_list = torch.load(bbox_file, weights_only=False)
     total_num_boxes = sum(len(d["bboxes"]) for d in bbox_list)
     print(f"Loaded bounding box list. There are {total_num_boxes} total bounding boxes.")
     dev = _device()
     model, _, patch_size, _ = utils.get_model(model_name.lower(), checkpoint=checkpoint, seed=seed, device=dev,
-                                              random_init=random_init)
+                                              random_init=random_init, precision=precision)
     feats: Dict[Tuple[int, int], torch.Tensor] = {}   # (image row, box row) -> [d]
 
     def flush(shape_key, items):
@@ -773,11 +778,12 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
                 random_init: bool = False, yes: Optional[bool] = None, single_region_dir: Optional[str] = None,
                 multi_region_dir: Optional[str] = None, non_adaptive_num_segments: int = 4, adaptive: bool = False,
                 infer_bg_index: bool = True, threshold: float = 0.0, num_workers: Optional[int] = None,
-                num_workers_out: int = 4, writer: str = "process"):
+                num_workers_out: int = 4, writer: str = "process", precision: str = "fp16"):
     """Fused extract_features + extract_eigs (+ the two segmentation commands): features and eigenvectors never leave
     the GPU between the stages. Writes the eigs files and, if the directories are given, the features files and the
     single- / multi-region segmentation PNGs, all in the reference's layouts. Decoding, pinned staging and the file
-    writers run on threads (io_pipeline.py)."""
+    writers run on threads (io_pipeline.py). ``precision``: ViT arithmetic, as in extract_features."""
+    vit_mod.check_precision(precision)
     for dname in (features_dir, eigs_dir, single_region_dir, multi_region_dir):
         if dname:
             utils.make_output_dir(dname, assume_yes=yes)
@@ -786,7 +792,7 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
     _check_supported("laplacian", which_color_matrix, image_color_lambda)
     dev = _device()
     model, _, patch_size, _ = utils.get_model(model_name, checkpoint=checkpoint, seed=seed, device=dev,
-                                              random_init=random_init)
+                                              random_init=random_init, precision=precision)
     filenames = Path(images_list).read_text().splitlines()
     dataset = utils.ImagesDataset(filenames=filenames, images_root=images_root)
     all_failed: List[str] = []

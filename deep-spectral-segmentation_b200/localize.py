@@ -224,6 +224,8 @@ def parse_args(argv=None):
     parser.add_argument("--random_init", action="store_true", help="Use randomly initialised weights (tests only).")
     parser.add_argument("--seed", type=int, default=None, help="Seed of the random weights (implies --random_init).")
     parser.add_argument("--batch_size", type=int, default=16, help="Images per ViT batch (images of one size).")
+    parser.add_argument("--precision", type=str, default="fp16", choices=["fp16", "fp32"],
+                        help="ViT arithmetic: fp16 operands (fast) or split-fp16 operands with the fp32 model's results.")
     args = parser.parse_args(argv)
     if args.image_path is not None:
         args.save_predictions = False
@@ -385,7 +387,7 @@ def main(argv=None) -> Optional[float]:
         preds = _eigseg_precomputed(args, items)
     else:
         model, _, _, _ = vit_mod.get_model(ARCH_MAP[(args.arch, args.patch_size)], checkpoint=args.checkpoint,
-                                           seed=args.seed, random_init=args.random_init)
+                                           seed=args.seed, random_init=args.random_init, precision=args.precision)
         preds = _from_images(args, items, model)
 
     preds_dict = {it.name: preds[it.name] for it in items}

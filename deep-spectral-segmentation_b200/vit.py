@@ -21,6 +21,16 @@ LN_EPS = 1e-6
 TRAIN_IMG = 224
 
 
+PRECISIONS = ("fp16", "fp32")
+
+
+def check_precision(precision: str) -> str:
+    """'fp16' (fp16 operands, the throughput path) or 'fp32' (split-fp16 operands: the fp32 model's results)."""
+    if precision not in PRECISIONS:
+        raise ValueError(f"precision must be one of {PRECISIONS} (got {precision!r})")
+    return precision
+
+
 def arch(name: str):
     name = name.lower()
     if "dino" not in name or name not in ARCHS:
@@ -70,9 +80,14 @@ def flat_param_order(name: str):
 
 
 class DinoViT:
-    """Device handle around dss_vit_t. ``forward_k(images_u8)`` == the reference's hooked K features."""
+    """Device handle around dss_vit_t. ``forward_k(images_u8)`` == the reference's hooked K features.
 
-    def __init__(self, name: str, state_dict: Dict[str, torch.Tensor], device="cuda"):
+    ``precision='fp16'`` runs every ViT GEMM and the attention on fp16 operands (K features within about 3e-3 relative
+    L2 of the fp32 model); ``'fp32'`` splits every operand into three fp16 values for fp32-equivalent products and
+    reproduces the fp32 model, at three times the tensor-core work and weight memory."""
+
+    def __init__(self, name: str, state_dict: Dict[str, torch.Tensor], device="cuda", precision: str = "fp16"):
+        self.precision = check_precision(precision)
         self.name = name.lower()
         self.patch_size, self.dim, self.depth, self.num_heads = arch(self.name)
         self.device = torch.device(device)
@@ -84,6 +99,7 @@ class DinoViT:
         h = C.c_void_p()
         _lib.check(self.lib.dss_vit_create(C.byref(cfg), C.byref(h)), "dss_vit_create")
         self._h = h
+        _lib.check(self.lib.dss_vit_set_precision(h, _lib.VIT_PRECISION[self.precision]), "dss_vit_set_precision")
         self._ws: Optional[torch.Tensor] = None
         self.load_state_dict(state_dict)
 
@@ -260,7 +276,7 @@ def find_checkpoint(name: str, checkpoint: Optional[str] = None) -> Optional[str
 
 
 def get_model(name: str, checkpoint: Optional[str] = None, seed: Optional[int] = None, device="cuda", state_dict=None,
-              random_init: bool = False):
+              random_init: bool = False, precision: str = "fp16"):
     """Mirror of utils.get_model (extract_utils.py:40-50): returns (model, val_transform, patch_size, num_heads).
 
     ``val_transform`` is None: ToTensor + Normalize are fused into the device im2col kernel, the model takes the
@@ -268,7 +284,8 @@ def get_model(name: str, checkpoint: Optional[str] = None, seed: Optional[int] =
     ``state_dict``, ``checkpoint``, $DSS_DINO_CHECKPOINT or the torch.hub cache (see find_checkpoint). Without any of
     them the call RAISES -- features of a randomly initialised ViT under the name 'dino_vits16' would be garbage in
     the reference's file layout -- unless the caller opts in with ``random_init=True`` or a ``seed`` (tests, benchmarks:
-    the upstream init recipe), which prints a loud warning."""
+    the upstream init recipe), which prints a loud warning. ``precision``: see DinoViT."""
+    check_precision(precision)
     name = name.lower()
     arch(name)
     if state_dict is None:
@@ -285,5 +302,5 @@ def get_model(name: str, checkpoint: Optional[str] = None, seed: Optional[int] =
                 f"{name}: pretrained DINO weights not found. The reference downloads them with torch.hub "
                 f"(extract_utils.py:42), which needs the network; pass checkpoint=<{HUB_FILES[name]}>, set "
                 "$DSS_DINO_CHECKPOINT, or opt into random weights with random_init=True / seed=<int> (tests only).")
-    model = DinoViT(name, state_dict, device=device)
+    model = DinoViT(name, state_dict, device=device, precision=precision)
     return model, None, model.patch_size, model.num_heads

@@ -86,6 +86,17 @@ typedef struct {
 
 int dss_vit_create(const dss_vit_config* cfg, dss_vit_t** out);
 void dss_vit_destroy(dss_vit_t* h);
+/* Arithmetic of a handle's ViT forward. The two modes compute different results:
+ *   DSS_VIT_PRECISION_FP16 (the default): fp16 operands in every GEMM and in attention, fp32 accumulation; K features
+ *     within about 3e-3 relative L2 of the fp32 model. The throughput path.
+ *   DSS_VIT_PRECISION_FP32: every operand of the GEMMs and of attention's two products split as x = hi + lo into three
+ *     fp16 values (hi, hi/64, 64 lo), so that each fp16 tensor-core product is hi hi' + hi lo' + lo hi'
+ *     (fp32-equivalent; error bound in DESIGN.md section 3); softmax, LayerNorm and exact-erf GELU in fp32. Reproduces
+ *     the fp32 reference; three times the tensor-core work, three times the weight memory and a larger workspace.
+ * Call before dss_vit_load_weights (the weights are packed for the mode); afterwards, or with another value,
+ * DSS_ERR_BAD_ARG. The workspace queries report the size for the handle's mode. */
+enum { DSS_VIT_PRECISION_FP16 = 0, DSS_VIT_PRECISION_FP32 = 1 };
+int dss_vit_set_precision(dss_vit_t* h, int precision);
 /* Packs the weights into the library's fp16 operand layout (synchronises `stream` before returning). */
 int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_stream_t stream);
 
@@ -164,6 +175,24 @@ int dss_op_layernorm_f16(const float* x, const float* gamma, const float* beta, 
 int dss_op_attention_tc_f16(const void* qkv, void* out, int B, int T, int heads, dss_stream_t stream);
 /* images_u8 [B,H,W,3] -> patches f16 [B*N, 3*P*P], column order (c, py, px), normalised */
 int dss_op_im2col_f16(const uint8_t* images_u8, void* patches, int B, int H, int W, int P, dss_stream_t stream);
+/* Split-fp16 operators of DSS_VIT_PRECISION_FP32. Each fp32 value v becomes hi = fp16(v), hi/64 and 64 (v - hi), stored
+ * as three groups of a row: A order [hi | hi/64 | 64 lo] for activations, B order [hi | 64 lo | hi/64] for weights, so
+ * that dss_op_gemm_f16 over K' = 3 K of an A-order [M, 3K] and a B-order [N, 3K] operand is the fp32-equivalent product.
+ * x [rows, cols] fp32 -> out f16 [rows, 3 cols]; order 0 = A, 1 = B. */
+int dss_op_split_f16(const float* x, void* out, int rows, int cols, int order, dss_stream_t stream);
+/* dss_op_layernorm_f16's fp32 value, split: y f16 [M, 3d] in A order */
+int dss_op_layernorm_split_f16(const float* x, const float* gamma, const float* beta, void* y, int M, int d, float eps,
+                               dss_stream_t stream);
+/* h f32 [M, n] -> out f16 [M, 3n] = split(gelu(h)) in A order, exact-erf GELU in fp32 (0.5 x (1 + erf(x / sqrt 2))) */
+int dss_op_gelu_split_f16(const float* h, void* out, int M, int n, dss_stream_t stream);
+/* dss_op_im2col_f16's fp32 value (pad != 0: dss_op_im2col_pad_f16's grid), split: patches f16 [B*N, 3 * 3P^2] in A order */
+int dss_op_im2col_split_f16(const uint8_t* images_u8, void* patches, int B, int H, int W, int P, int pad,
+                            dss_stream_t stream);
+/* Attention of DSS_VIT_PRECISION_FP32: qkv f32 [B, T, 3d] (q | k | v, heads of 64) -> out f16 [B, T, 3d] = split(softmax(
+ * q k^T / 8) v) in A order (each group d wide, head h at columns 64 h), the proj GEMM's operand. qkv_split f16
+ * [B, T, 9d] is scratch: per head h, Q' = split(q) in A order at columns 192 h, K' and V' = split(k), split(v) in B order
+ * at 3d + 192 h and 6d + 192 h. S = Q' K'^T and P V on the fp16 tensor cores with P split in registers; softmax fp32. */
+int dss_op_attention_split_f16(const float* qkv, void* qkv_split, void* out, int B, int T, int heads, dss_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------------------------
  * Affinity + graph Laplacian eigensolver (replaces extract/extract.py:148,191-195,207-235,237-240)
@@ -390,7 +419,8 @@ int dss_dinoseg_boxes(const float* cls_attn, int B, int heads, int N, int head, 
  *   feats_out [B, N, d] fp32 (may be NULL): the `which` third of its qkv projection (0 = q, 1 = k, 2 = v), CLS row
  *     dropped (the qkv hook of main.py:283-322);
  *   cls_attn_out [B, heads, N] fp32 (may be NULL): softmax(q_0 k_j / 8) over all T = N + 1 tokens, patch entries
- *     (get_last_selfattention(...)[:, :, 0, 1:]), from the fp16 qkv the attention kernels read.
+ *     (get_last_selfattention(...)[:, :, 0, 1:]), from the fp16 qkv the attention kernels read (the fp32 qkv under
+ *     DSS_VIT_PRECISION_FP32).
  * At least one output is required. Workspace: dss_vit_forward_last_workspace_bytes (0 if the image is smaller than a
  * patch in crop mode). */
 size_t dss_vit_forward_last_workspace_bytes(const dss_vit_t* h, int B, int H, int W, int pad);
