@@ -53,7 +53,7 @@ rownorm_split_kernel(const float* __restrict__ f, __half* __restrict__ S, unsign
   for (int k = lane; k < dpad; k += 32) {
     float v = 0.f;
     if (k < d) v = normalize ? x[k] / denom : x[k] * pre;
-    split_f16(v, s[k], s[dpad + k], s[2 * dpad + k]);
+    store_split(s + k, dpad, 0, v);
     s2 = fmaf(v, v, s2);
   }
   s2 = warp_sum(s2);

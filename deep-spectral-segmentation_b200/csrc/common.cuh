@@ -53,22 +53,19 @@ int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
 int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int images, int Nimg, int d, float* Wout, int ldw,
                      int ncols, const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts,
                      float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st);
-// ViT kernels (vit_kernels.cu, attention_tc.cu)
-int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
-int launch_im2col_pad(const uint8_t* img, void* patches, int B, int H, int W, int P, cudaStream_t st);
-int launch_cls_attention(const void* qkv, int B, int T, int heads, float* out, cudaStream_t st);
+// ViT kernels (vit_kernels.cu, attention.cu). split: the operand is written in the split-fp16 format of
+// DSS_VIT_PRECISION_FP32 (A order), three groups per value (split_f16 below)
+int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P, int pad, bool split, cudaStream_t st);
 int launch_cls_row(float* x, const float* cls, const float* pos, int B, int T, int d, cudaStream_t st);
-int launch_layernorm(const float* x, const float* g, const float* b, void* y, int M, int d, float eps, cudaStream_t st);
-int launch_attention_tc(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st);
-// split-fp16 operands of DSS_VIT_PRECISION_FP32 (vit_split.cu, attention_split.cu)
+int launch_layernorm(const float* x, const float* g, const float* b, void* y, int M, int d, float eps, bool split,
+                     cudaStream_t st);
+// qkv: f16 [B*T, 3d] (f32_keys false) or the fp32 qkv GEMM output of DSS_VIT_PRECISION_FP32 (f32_keys true)
+int launch_cls_attention(const void* qkv, bool f32_keys, int B, int T, int heads, float* out, cudaStream_t st);
 int launch_split_rows(const float* x, void* out, long long rows, int cols, int order, cudaStream_t st, int kclass);
-int launch_im2col_split(const uint8_t* img, void* patches, int B, int H, int W, int P, int pad, cudaStream_t st);
-int launch_layernorm_split(const float* x, const float* g, const float* b, void* y, int M, int d, float eps,
-                           cudaStream_t st);
 int launch_gelu_split(const float* h, void* out, long long M, int n, cudaStream_t st);
 int launch_qkv_split(const float* qkv, void* out, long long M, int d, cudaStream_t st);
+int launch_attention_tc(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st);
 int launch_attention_split(const void* qkv_split, void* out, int B, int T, int heads, cudaStream_t st);
-int launch_cls_attention_f32(const float* qkv, int B, int T, int heads, float* out, cudaStream_t st);
 
 // ---------------------------------------------------------------- launch accounting / per-class device timing
 enum KernelClass {
@@ -266,6 +263,15 @@ __device__ __forceinline__ uint32_t sw128_addr(uint32_t base, int row, int chunk
 // d[i .. i+7] as read-write asm operands
 #define DSS_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
                     "+f"(d[i + 6]), "+f"(d[i + 7])
+// D[64 x 64] (+)= A(smem) * B(smem), both K-major
+__device__ __forceinline__ void wgmma_m64n64_ss(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "%32, %33, p, 1, 1, 0, 0;\n\t}"
+      : DSS_ACC8(0), DSS_ACC8(8), DSS_ACC8(16), DSS_ACC8(24)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 // D[64 x 128] (+)= A(smem) * B(smem), both K-major
 __device__ __forceinline__ void wgmma_m64n128_ss(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
@@ -317,6 +323,17 @@ __device__ __forceinline__ uint32_t pack_half2(float lo, float hi) {
   __half2 h = __floats2half2_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&h);
 }
+__device__ __forceinline__ uint32_t pack_h2(__half lo, __half hi) {
+  __half2 h = __halves2half2(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&h);
+}
+
+// one MUFU.EX2 (2 ulp), flushes denormal results to zero; exp2f would add range checks and fix-ups per element
+__device__ __forceinline__ float ex2_approx(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
 
 // Split-fp16 operand format (the affinity's Gram product and the fp32-precision ViT): x = hi + lo, hi = fp16(x),
 // lo = x - hi (exact in fp32, |lo| <= 2^-11 |x|), stored as the three fp16 values hi, hi/64 and 64 lo. A product of
@@ -333,6 +350,18 @@ __device__ __forceinline__ SplitF16 split_f16(float v) {
   SplitF16 s;
   split_f16(v, s.hi, s.hi_s, s.lo_s);
   return s;
+}
+// The one writer of the format: the three groups of a value (or of a pair packed by pack_h2) at o, o + stride and
+// o + 2 stride, in A order [hi | hi/64 | 64 lo] (order 0) or B order [hi | 64 lo | hi/64] (order != 0).
+template <typename E>
+__device__ __forceinline__ void store_split(E* o, int stride, int order, E hi, E hi_s, E lo_s) {
+  o[0] = hi;
+  o[stride] = order ? lo_s : hi_s;
+  o[2 * stride] = order ? hi_s : lo_s;
+}
+__device__ __forceinline__ void store_split(__half* o, int stride, int order, float v) {
+  const SplitF16 s = split_f16(v);
+  store_split(o, stride, order, s.hi, s.hi_s, s.lo_s);
 }
 
 // Exact-erf GELU, branch-free:  gelu(x) = x Phi(x) = relu(x) - |x| q(|x|),  q(a) = 0.5 erfc(a / sqrt 2) = 2^P(u),
@@ -355,9 +384,7 @@ __device__ __forceinline__ float gelu_erf(float x) {
   p = __fmaf_rn(p, u, DSS_GELU_P2);
   p = __fmaf_rn(p, u, DSS_GELU_P1);
   p = __fmaf_rn(p, u, DSS_GELU_P0);
-  float q;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(q) : "f"(p));
-  return __fmaf_rn(na, q, fmaxf(x, 0.f));
+  return __fmaf_rn(na, ex2_approx(p), fmaxf(x, 0.f));
 }
 
 __device__ __forceinline__ float warp_sum(float v) {
@@ -365,7 +392,7 @@ __device__ __forceinline__ float warp_sum(float v) {
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-// LayerNorm arithmetic of one row held as float4 chunks per lane (layernorm_f16_kernel). Every rounding is explicit (no
+// LayerNorm arithmetic of one row held as float4 chunks per lane (layernorm_kernel). Every rounding is explicit (no
 // contraction is left to the compiler), so the output is fixed by the source rather than by the compiler's choices:
 // x - mean is one fused multiply-add on the row sum S (the mean itself is never rounded), the squares pair as
 // fma(a, a, b * b), the variance is fma(Q, 1 / d, eps), and y = fma((x - mean) * rstd, gamma, beta).
@@ -378,12 +405,10 @@ __device__ __forceinline__ float ln_sq4(float4 a) {
   return __fadd_rn(__fmaf_rn(a.x, a.x, __fmul_rn(a.y, a.y)), __fmaf_rn(a.z, a.z, __fmul_rn(a.w, a.w)));
 }
 __device__ __forceinline__ float ln_rstd(float Q, float inv_d, float eps) { return rsqrtf(__fmaf_rn(Q, inv_d, eps)); }
-// the four outputs of a centred chunk a, as two packed half2
-__device__ __forceinline__ uint2 ln_out4(float4 a, float rstd, float4 g, float4 b) {
-  uint2 o;
-  o.x = pack_half2(__fmaf_rn(__fmul_rn(a.x, rstd), g.x, b.x), __fmaf_rn(__fmul_rn(a.y, rstd), g.y, b.y));
-  o.y = pack_half2(__fmaf_rn(__fmul_rn(a.z, rstd), g.z, b.z), __fmaf_rn(__fmul_rn(a.w, rstd), g.w, b.w));
-  return o;
+// the four outputs of a centred chunk a
+__device__ __forceinline__ float4 ln_out4(float4 a, float rstd, float4 g, float4 b) {
+  return make_float4(__fmaf_rn(__fmul_rn(a.x, rstd), g.x, b.x), __fmaf_rn(__fmul_rn(a.y, rstd), g.y, b.y),
+                     __fmaf_rn(__fmul_rn(a.z, rstd), g.z, b.z), __fmaf_rn(__fmul_rn(a.w, rstd), g.w, b.w));
 }
 __device__ __forceinline__ double warp_sum(double v) {
 #pragma unroll

@@ -5,8 +5,9 @@
 // Per block:  LN1 -> [wgmma GEMM] qkv (f16) -> wgmma flash attention -> [wgmma GEMM + residual] proj
 //             LN2 -> [wgmma GEMM + GELU] fc1 (f16) -> [wgmma GEMM + residual] fc2
 // The residual stream stays fp32; GEMM operands are fp16 (11-bit significand, same as TF32), accumulation fp32.
-// DSS_VIT_PRECISION_FP32 (dss_vit_set_precision) runs the same blocks on split-fp16 operands (vit_split.cu,
-// attention_split.cu): fp32-equivalent products on the fp16 tensor cores at three times the tensor-core work.
+// DSS_VIT_PRECISION_FP32 (dss_vit_set_precision) runs the same blocks on split-fp16 operands (the split producers of
+// vit_kernels.cu, attention_split_kernel): fp32-equivalent products on the fp16 tensor cores at three times the
+// tensor-core work.
 // The block the reference hooks is pruned to LN1 + the K third of its qkv projection, CLS row dropped in the
 // GEMM epilogue, which writes the fp32 features directly in the reference's [B, N, d] layout.
 #include <math.h>
@@ -53,7 +54,7 @@ struct BlockW {
 
 struct dss_vit {
   dss_vit_config cfg;
-  int precision = DSS_VIT_PRECISION_FP16;   // DSS_VIT_PRECISION_FP32: every weight packed as split fp16 (vit_split.cu)
+  int precision = DSS_VIT_PRECISION_FP16;   // DSS_VIT_PRECISION_FP32: every weight packed as split fp16 (B order)
   bool loaded = false;
   void* arena = nullptr;  // one device allocation holding every packed weight
   size_t arena_bytes = 0;
@@ -160,23 +161,24 @@ static int get_pos(dss_vit* h, int Hp, int Wp, bool square, cudaStream_t st, flo
   return DSS_OK;
 }
 
-// DSS_VIT_PRECISION_FP32 (split): patches, xn and attn hold three fp16 groups per value (A order), qkv holds the
-// split attention operands [B*T, 9d] and, after attention, the split MLP hidden activations [B*T, 12d] (the same
-// buffer), and f32 holds the fp32 GEMM outputs that are split next: qkv [B*T, 3d], then the fc1 output [B*T, 4d].
+// ks = 1 (DSS_VIT_PRECISION_FP16) or 3 (DSS_VIT_PRECISION_FP32, split): patches, xn and attn hold ks fp16 groups per
+// value (A order). Split, qkv holds the split attention operands [B*T, 9d] and, after attention, the split MLP hidden
+// activations [B*T, 12d] (the same buffer), and f32 holds the fp32 GEMM outputs that are split next: qkv [B*T, 3d],
+// then the fc1 output [B*T, 4d].
 struct VitWs {
-  __half* patches;  // [B*Np, 3P^2]
+  __half* patches;  // [B*Np, ks 3P^2]
   float* x;         // [B*T, d]     residual stream
-  __half* xn;       // [B*T, d]     LayerNorm output (GEMM A operand)
-  __half* attn;     // [B*T, d]     attention output (GEMM A operand)
-  __half* qkv;      // [B*T, 3d]
-  __half* hid;      // [B*T, 4d]
+  __half* xn;       // [B*T, ks d]  LayerNorm output (GEMM A operand)
+  __half* attn;     // [B*T, ks d]  attention output (GEMM A operand)
+  __half* qkv;      // [B*T, 3d] (fp16) | [B*T, 9d] (split)
+  __half* hid;      // [B*T, ks 4d]
   float* f32;       // split only
   size_t total;
 };
 
 static VitWs carve(const dss_vit_config& c, int B, int Hp, int Wp, void* base, int precision) {
   const int Np = Hp * Wp, T = Np + 1, d = c.dim;
-  const size_t M = (size_t)B * T;
+  const size_t M = (size_t)B * T, ks = precision == DSS_VIT_PRECISION_FP32 ? 3 : 1;
   uint8_t* p = reinterpret_cast<uint8_t*>(base);
   size_t off = 0;
   auto take = [&](size_t bytes) {
@@ -186,23 +188,19 @@ static VitWs carve(const dss_vit_config& c, int B, int Hp, int Wp, void* base, i
   };
   VitWs w;
   const size_t hd = (size_t)c.mlp_ratio * d;
-  if (precision == DSS_VIT_PRECISION_FP32) {
-    w.patches = reinterpret_cast<__half*>(take((size_t)B * Np * 9 * c.patch * c.patch * 2));
-    w.x = reinterpret_cast<float*>(take(M * d * 4));
-    w.xn = reinterpret_cast<__half*>(take(M * 3 * d * 2));
-    w.attn = reinterpret_cast<__half*>(take(M * 3 * d * 2));
-    w.qkv = w.hid = reinterpret_cast<__half*>(take(M * std::max<size_t>(9 * d, 3 * hd) * 2));
-    w.f32 = reinterpret_cast<float*>(take(M * std::max<size_t>(3 * d, hd) * 4));
-    w.total = off;
-    return w;
-  }
-  w.patches = reinterpret_cast<__half*>(take((size_t)B * Np * 3 * c.patch * c.patch * 2));
+  w.patches = reinterpret_cast<__half*>(take((size_t)B * Np * ks * 3 * c.patch * c.patch * 2));
   w.x = reinterpret_cast<float*>(take(M * d * 4));
-  w.xn = reinterpret_cast<__half*>(take(M * d * 2));
-  w.attn = reinterpret_cast<__half*>(take(M * d * 2));
-  w.qkv = reinterpret_cast<__half*>(take(M * 3 * d * 2));
-  w.hid = reinterpret_cast<__half*>(take(M * (size_t)c.mlp_ratio * d * 2));
-  w.f32 = nullptr;
+  w.xn = reinterpret_cast<__half*>(take(M * ks * d * 2));
+  w.attn = reinterpret_cast<__half*>(take(M * ks * d * 2));
+  const size_t qkv_bytes = M * ks * 3 * d * 2, hid_bytes = M * ks * hd * 2;
+  if (ks == 3) {
+    w.qkv = w.hid = reinterpret_cast<__half*>(take(std::max(qkv_bytes, hid_bytes)));
+    w.f32 = reinterpret_cast<float*>(take(M * std::max<size_t>(3 * d, hd) * 4));
+  } else {
+    w.qkv = reinterpret_cast<__half*>(take(qkv_bytes));
+    w.hid = reinterpret_cast<__half*>(take(hid_bytes));
+    w.f32 = nullptr;
+  }
   w.total = off;
   return w;
 }
@@ -223,84 +221,24 @@ static int vit_tail(const dss_vit* h, const float* x, int mode, float* out, int 
   return DSS_OK;
 }
 
-// vit_run of DSS_VIT_PRECISION_FP32: the same sequence on split operands. Every GEMM runs the fp16 path's kernel and
-// epilogue at K' = 3 K; the qkv and fc1 GEMMs write fp32 (DSS_EPI_BIAS_F32), which qkv_split_kernel /
-// gelu_split_kernel turn into the next product's split operands.
-static int vit_run_split(dss_vit* h, const VitWs& w, const uint8_t* img, int B, int H, int W, int Hp, int Wp,
-                         int n_full, int mode, float* out, const float* pos, cudaStream_t st, int pad, int which,
-                         float* cls_attn) {
-  const dss_vit_config& c = h->cfg;
-  const int P = c.patch, d = c.dim, hd = c.mlp_ratio * d;
-  const int Np = Hp * Wp, T = Np + 1, M = B * T, Kp = 3 * P * P;
-  int rc;
-  CUtensorMap tm_patches, tm_xn, tm_attn, tm_hid, tm_x_out, tm_qkv_out, tm_hid_out;
-  if ((rc = make_tmap_f16(&tm_patches, w.patches, B * Np, 3 * Kp, 128))) return rc;
-  if ((rc = make_tmap_f16(&tm_xn, w.xn, M, 3 * d, 128))) return rc;
-  if ((rc = make_tmap_f16(&tm_attn, w.attn, M, 3 * d, 128))) return rc;
-  if ((rc = make_tmap_f16(&tm_hid, w.hid, M, 3 * hd, 128))) return rc;
-  if ((rc = make_tmap_out(&tm_x_out, w.x, M, d, 1))) return rc;
-  if ((rc = make_tmap_out(&tm_qkv_out, w.f32, M, 3 * d, 1))) return rc;
-  if ((rc = make_tmap_out(&tm_hid_out, w.f32, M, hd, 1))) return rc;
-
-  if ((rc = launch_im2col_split(img, w.patches, B, H, W, P, pad, st))) return rc;
-  if ((rc = gemm_f16_tc(tm_patches, h->tm_patch, nullptr, h->patch_b, w.x, B * Np, d, 3 * Kp, DSS_EPI_PATCH_F32, pos, Np,
-                        T, st, KC_GEMM_PATCH, 128)))
-    return rc;
-  if ((rc = launch_cls_row(w.x, h->cls, pos, B, T, d, st))) return rc;
-  auto qkv_f32 = [&](const BlockW& bw) {
-    return gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, w.f32, M, 3 * d, 3 * d, DSS_EPI_BIAS_F32, nullptr, 0, 0, st,
-                       KC_GEMM_QKV, gemm_tile_n());
-  };
-  for (int l = 0; l < n_full; ++l) {
-    const BlockW& bw = h->blocks[l];
-    if ((rc = launch_layernorm_split(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
-    if ((rc = qkv_f32(bw))) return rc;
-    if ((rc = launch_qkv_split(w.f32, w.qkv, M, d, st))) return rc;
-    if ((rc = launch_attention_split(w.qkv, w.attn, B, T, c.heads, st))) return rc;
-    if ((rc = gemm_f16_tc(tm_attn, bw.tm_proj, &tm_x_out, bw.proj_b, w.x, M, d, 3 * d, DSS_EPI_BIAS_RESID_F32, nullptr, 0,
-                          0, st, KC_GEMM_PROJ, gemm_tile_n())))
-      return rc;
-    if ((rc = launch_layernorm_split(w.x, bw.ln2_w, bw.ln2_b, w.xn, M, d, c.ln_eps, st))) return rc;
-    if ((rc = gemm_f16_tc(tm_xn, bw.tm_fc1, &tm_hid_out, bw.fc1_b, w.f32, M, hd, 3 * d, DSS_EPI_BIAS_F32, nullptr, 0, 0,
-                          st, KC_GEMM_FC1, gemm_tile_n())))
-      return rc;
-    if ((rc = launch_gelu_split(w.f32, w.hid, M, hd, st))) return rc;
-    if ((rc = gemm_f16_tc(tm_hid, bw.tm_fc2, &tm_x_out, bw.fc2_b, w.x, M, d, 3 * hd, DSS_EPI_BIAS_RESID_F32, nullptr, 0,
-                          0, st, KC_GEMM_FC2, gemm_tile_n())))
-      return rc;
-  }
-  if (mode == 0 || mode == 3) {
-    const BlockW& bw = h->blocks[n_full];
-    if ((rc = launch_layernorm_split(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
-    if (out) {
-      const CUtensorMap& tm = which == 0 ? bw.tm_q : (which == 1 ? bw.tm_k : bw.tm_v);
-      if ((rc = gemm_f16_tc(tm_xn, tm, nullptr, bw.qkv_b + (size_t)which * d, out, M, d, 3 * d, DSS_EPI_DROPCLS_F32,
-                            nullptr, T, Np, st, KC_GEMM_KPROJ, 128)))
-        return rc;
-    }
-    if (mode == 3 && cls_attn) {
-      if ((rc = qkv_f32(bw))) return rc;
-      if ((rc = launch_cls_attention_f32(w.f32, B, T, c.heads, cls_attn, st))) return rc;
-    }
-    return DSS_OK;
-  }
-  return vit_tail(h, w.x, mode, out, B, T, st);
-}
-
 // mode 0: K projection of block n_full (features), 1: residual stream [B, T, d], 2: final-norm CLS token [B, d],
-// 3: block n_full's `which` projection third (out, may be NULL) and CLS attention row (cls_attn, may be NULL).
-// pad: zero-padded ceil grid instead of the crop.
+// 3: block n_full's `which` projection third (out, may be NULL) and CLS attention row (cls_attn, may be NULL); mode 0
+// is mode 3 with which = 1 and no CLS attention row. pad: zero-padded ceil grid instead of the crop.
+// DSS_VIT_PRECISION_FP32 runs the same sequence on split operands: every GEMM runs the fp16 path's kernel and epilogue
+// at K' = 3 K; the qkv and fc1 GEMMs write fp32 (DSS_EPI_BIAS_F32), which qkv_split_kernel / gelu_split_kernel turn
+// into the next product's split operands.
 static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_full, int mode, float* out, void* ws,
                    size_t ws_bytes, cudaStream_t st, int pad = 0, int which = 1, float* cls_attn = nullptr) {
-  const bool k_proj = mode == 0;
   DSS_REQUIRE(h && h->loaded, "vit: weights not loaded");
   DSS_REQUIRE(img && (out || cls_attn) && ws, "vit: null pointer");
   const dss_vit_config& c = h->cfg;
-  const int P = c.patch, d = c.dim;
+  const int P = c.patch, d = c.dim, hd = c.mlp_ratio * d;
   const int Hp = pad ? cdiv(H, P) : H / P, Wp = pad ? cdiv(W, P) : W / P;
   DSS_REQUIRE(B > 0 && Hp > 0 && Wp > 0, "vit: image %dx%d smaller than one %d-pixel patch", H, W, P);
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "vit: workspace must be 256-byte aligned");
-  const int Np = Hp * Wp, T = Np + 1, M = B * T;
+  const int Np = Hp * Wp, T = Np + 1, M = B * T, Kp = 3 * P * P;
+  const bool split = h->precision == DSS_VIT_PRECISION_FP32;
+  const int ks = split ? 3 : 1;   // fp16 values per operand value
   VitWs w = carve(c, B, Hp, Wp, ws, h->precision);
   if (ws_bytes < w.total) {
     set_error("vit: workspace too small (%zu < %zu)", ws_bytes, w.total);
@@ -312,72 +250,68 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   // sees them, so their patch grid decides; the model's own forward (box crops) and the token hook take the image as is
   const bool square = (mode == 1 || mode == 2) ? H == W : Hp == Wp;
   if ((rc = get_pos(h, Hp, Wp, square, st, &pos))) return rc;
-  if (h->precision == DSS_VIT_PRECISION_FP32)
-    return vit_run_split(h, w, img, B, H, W, Hp, Wp, n_full, mode, out, pos, st, pad, which, cls_attn);
 
   CUtensorMap tm_patches, tm_xn, tm_attn, tm_hid;
-  const int Kp = 3 * P * P;
-  if ((rc = make_tmap_f16(&tm_patches, w.patches, B * Np, Kp, 128))) return rc;
-  if ((rc = make_tmap_f16(&tm_xn, w.xn, M, d, 128))) return rc;
-  if ((rc = make_tmap_f16(&tm_attn, w.attn, M, d, 128))) return rc;
-  if ((rc = make_tmap_f16(&tm_hid, w.hid, M, c.mlp_ratio * d, 128))) return rc;
-  // output maps of the TMA-store epilogues: residual stream (fp32, reduce-add), qkv and MLP hidden (fp16)
+  if ((rc = make_tmap_f16(&tm_patches, w.patches, B * Np, ks * Kp, 128))) return rc;
+  if ((rc = make_tmap_f16(&tm_xn, w.xn, M, ks * d, 128))) return rc;
+  if ((rc = make_tmap_f16(&tm_attn, w.attn, M, ks * d, 128))) return rc;
+  if ((rc = make_tmap_f16(&tm_hid, w.hid, M, ks * hd, 128))) return rc;
+  // output maps of the TMA-store epilogues: residual stream (fp32, reduce-add), qkv and MLP hidden (fp16, or the fp32
+  // outputs that are split next)
   CUtensorMap tm_x_out, tm_qkv_out, tm_hid_out;
   if ((rc = make_tmap_out(&tm_x_out, w.x, M, d, 1))) return rc;
-  if ((rc = make_tmap_out(&tm_qkv_out, w.qkv, M, 3 * d, 0))) return rc;
-  if ((rc = make_tmap_out(&tm_hid_out, w.hid, M, c.mlp_ratio * d, 0))) return rc;
+  if ((rc = make_tmap_out(&tm_qkv_out, split ? (void*)w.f32 : w.qkv, M, 3 * d, split))) return rc;
+  if ((rc = make_tmap_out(&tm_hid_out, split ? (void*)w.f32 : w.hid, M, hd, split))) return rc;
 
   // tokens: x[b, 1+n, :] = patch_embed + pos ; x[b, 0, :] = cls + pos[0]
-  if ((rc = pad ? launch_im2col_pad(img, w.patches, B, H, W, P, st) : launch_im2col(img, w.patches, B, H, W, P, st)))
-    return rc;
-  if ((rc = gemm_f16_tc(tm_patches, h->tm_patch, nullptr, h->patch_b, w.x, B * Np, d, Kp, DSS_EPI_PATCH_F32, pos, Np, T, st,
-                        KC_GEMM_PATCH, 128)))
+  if ((rc = launch_im2col(img, w.patches, B, H, W, P, pad, split, st))) return rc;
+  if ((rc = gemm_f16_tc(tm_patches, h->tm_patch, nullptr, h->patch_b, w.x, B * Np, d, ks * Kp, DSS_EPI_PATCH_F32, pos, Np,
+                        T, st, KC_GEMM_PATCH, 128)))
     return rc;
   if ((rc = launch_cls_row(w.x, h->cls, pos, B, T, d, st))) return rc;
 
+  // the full qkv projection: the attention operands (fp16), or the fp32 values they are split from
+  auto qkv_gemm = [&](const BlockW& bw) {
+    return gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, split ? (void*)w.f32 : w.qkv, M, 3 * d, ks * d,
+                       split ? DSS_EPI_BIAS_F32 : DSS_EPI_BIAS_F16, nullptr, 0, 0, st, KC_GEMM_QKV, gemm_tile_n());
+  };
   // LayerNorm kernel + GEMM: LayerNorm fused into the qkv / fc1 GEMMs measured slower (DESIGN.md section 9)
   for (int l = 0; l < n_full; ++l) {
     const BlockW& bw = h->blocks[l];
-    if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
-    if ((rc = gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, w.qkv, M, 3 * d, d, DSS_EPI_BIAS_F16, nullptr, 0, 0, st,
-                          KC_GEMM_QKV, gemm_tile_n())))
+    if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, split, st))) return rc;
+    if ((rc = qkv_gemm(bw))) return rc;
+    if (split) {
+      if ((rc = launch_qkv_split(w.f32, w.qkv, M, d, st))) return rc;
+      if ((rc = launch_attention_split(w.qkv, w.attn, B, T, c.heads, st))) return rc;
+    } else {
+      if ((rc = launch_attention_tc(w.qkv, w.attn, B, T, c.heads, st))) return rc;
+    }
+    if ((rc = gemm_f16_tc(tm_attn, bw.tm_proj, &tm_x_out, bw.proj_b, w.x, M, d, ks * d, DSS_EPI_BIAS_RESID_F32, nullptr,
+                          0, 0, st, KC_GEMM_PROJ, gemm_tile_n())))
       return rc;
-    if ((rc = launch_attention_tc(w.qkv, w.attn, B, T, c.heads, st))) return rc;
-    if ((rc = gemm_f16_tc(tm_attn, bw.tm_proj, &tm_x_out, bw.proj_b, w.x, M, d, d, DSS_EPI_BIAS_RESID_F32, nullptr, 0, 0, st,
-                          KC_GEMM_PROJ, gemm_tile_n())))
+    if ((rc = launch_layernorm(w.x, bw.ln2_w, bw.ln2_b, w.xn, M, d, c.ln_eps, split, st))) return rc;
+    if ((rc = gemm_f16_tc(tm_xn, bw.tm_fc1, &tm_hid_out, bw.fc1_b, split ? (void*)w.f32 : w.hid, M, hd, ks * d,
+                          split ? DSS_EPI_BIAS_F32 : DSS_EPI_BIAS_GELU_F16, nullptr, 0, 0, st, KC_GEMM_FC1,
+                          gemm_tile_n())))
       return rc;
-    if ((rc = launch_layernorm(w.x, bw.ln2_w, bw.ln2_b, w.xn, M, d, c.ln_eps, st))) return rc;
-    if ((rc = gemm_f16_tc(tm_xn, bw.tm_fc1, &tm_hid_out, bw.fc1_b, w.hid, M, c.mlp_ratio * d, d, DSS_EPI_BIAS_GELU_F16,
-                          nullptr, 0, 0, st, KC_GEMM_FC1, gemm_tile_n())))
-      return rc;
-    if ((rc = gemm_f16_tc(tm_hid, bw.tm_fc2, &tm_x_out, bw.fc2_b, w.x, M, d, c.mlp_ratio * d, DSS_EPI_BIAS_RESID_F32, nullptr, 0,
+    if (split && (rc = launch_gelu_split(w.f32, w.hid, M, hd, st))) return rc;
+    if ((rc = gemm_f16_tc(tm_hid, bw.tm_fc2, &tm_x_out, bw.fc2_b, w.x, M, d, ks * hd, DSS_EPI_BIAS_RESID_F32, nullptr, 0,
                           0, st, KC_GEMM_FC2, gemm_tile_n())))
       return rc;
   }
-  if (k_proj) {
-    const BlockW& bw = h->blocks[n_full];
-    if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
-    // K third of the qkv projection (weight rows [d, 2d)), CLS rows dropped: out[b, n, :] == qkv[b, 1+n, d:2d]
-    if ((rc = gemm_f16_tc(tm_xn, bw.tm_k, nullptr, bw.qkv_b + d, out, M, d, d, DSS_EPI_DROPCLS_F32, nullptr, T, Np, st,
-                          KC_GEMM_KPROJ, 128)))
+  if (mode == 1 || mode == 2) return vit_tail(h, w.x, mode, out, B, T, st);
+
+  const BlockW& bw = h->blocks[n_full];
+  if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, split, st))) return rc;
+  if (out) {   // qkv[b, 1+n, which*d : (which+1)*d] in fp32, CLS rows dropped (which = 1: the K features)
+    const CUtensorMap& tm = which == 0 ? bw.tm_q : (which == 1 ? bw.tm_k : bw.tm_v);
+    if ((rc = gemm_f16_tc(tm_xn, tm, nullptr, bw.qkv_b + (size_t)which * d, out, M, d, ks * d, DSS_EPI_DROPCLS_F32,
+                          nullptr, T, Np, st, KC_GEMM_KPROJ, 128)))
       return rc;
-  } else if (mode == 3) {
-    const BlockW& bw = h->blocks[n_full];
-    if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, st))) return rc;
-    if (out) {   // qkv[b, 1+n, which*d : (which+1)*d] in fp32, as dss_vit_forward_k writes the K third
-      const CUtensorMap& tm = which == 0 ? bw.tm_q : (which == 1 ? bw.tm_k : bw.tm_v);
-      if ((rc = gemm_f16_tc(tm_xn, tm, nullptr, bw.qkv_b + (size_t)which * d, out, M, d, d, DSS_EPI_DROPCLS_F32, nullptr, T,
-                            Np, st, KC_GEMM_KPROJ, 128)))
-        return rc;
-    }
-    if (cls_attn) {   // the full qkv projection the attention kernels read, then the CLS row of the softmax
-      if ((rc = gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, w.qkv, M, 3 * d, d, DSS_EPI_BIAS_F16, nullptr, 0, 0, st,
-                            KC_GEMM_QKV, gemm_tile_n())))
-        return rc;
-      if ((rc = launch_cls_attention(w.qkv, B, T, c.heads, cls_attn, st))) return rc;
-    }
-  } else {
-    return vit_tail(h, w.x, mode, out, B, T, st);
+  }
+  if (cls_attn) {   // the full qkv projection the attention kernels read, then the CLS row of the softmax
+    if ((rc = qkv_gemm(bw))) return rc;
+    if ((rc = launch_cls_attention(split ? (const void*)w.f32 : w.qkv, split, B, T, c.heads, cls_attn, st))) return rc;
   }
   return DSS_OK;
 }
