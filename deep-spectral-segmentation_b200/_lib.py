@@ -50,6 +50,12 @@ PROTOTYPES = {
     "dss_vit_forward_tokens": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                        c_void_p]),
     "dss_vit_forward_cls": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "dss_vit_ragged_workspace_bytes": (c_size_t, [c_void_p, c_void_p, c_int, c_int]),
+    "dss_vit_forward_k_ragged": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t,
+                                         c_void_p]),
+    "dss_vit_forward_cls_ragged": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "dss_vit_pos_embed_ragged": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "dss_vit_pos_cache_entries": (c_int, [c_void_p]),
     "dss_vit_pos_embed": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "dss_pos_embed_interp_host": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "dss_op_gemm_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
@@ -126,8 +132,9 @@ EPI_BIAS_F16, EPI_BIAS_GELU_F16, EPI_BIAS_RESID_F32, EPI_BIAS_F32, EPI_PATCH_F32
 AFF_NORMALIZE, AFF_THRESHOLD_AT_ZERO, AFF_NO_MAX_SCALE = 1, 2, 4
 LOC_OK, LOC_NO_GRID, LOC_SEED_IN_BACKGROUND, LOC_EMPTY_COMPONENT = range(4)
 SEGEVAL_SEMANTIC, SEGEVAL_BINARY, SEGEVAL_FIELDS = 0, 1, 13
-DSS_ERR_UNSUPPORTED = -4
+DSS_ERR_BAD_ARG, DSS_ERR_UNSUPPORTED = -1, -4
 VIT_PRECISION = {"fp16": 0, "fp32": 1}   # DSS_VIT_PRECISION_FP16 / _FP32
+VIT_RAGGED_K, VIT_RAGGED_CLS = 0, 1          # DSS_VIT_RAGGED_K / _CLS
 
 _lib = None
 

@@ -124,6 +124,27 @@ __device__ __forceinline__ void softmax_rowsum(float (&l_run)[2]) {
   }
 }
 
+// Where a CTA's query tile lies: image b, its T token rows from row0(), the tile's first query q0(bm) of the image.
+// A uniform batch of B images of T tokens: CTA (x, head, b) runs tile x of image b.
+struct UniformTile {
+  int b, T;
+  __device__ __forceinline__ int q0(int bm) const { return blockIdx.x * bm; }
+  __device__ __forceinline__ int row0() const { return b * T; }
+};
+// A ragged batch (vit.cu): CTA (x, head) runs tile x - tile_prefix[b] of the image b whose tiles
+// [tile_prefix[b], tile_prefix[b + 1]) contain x.
+struct RaggedTile {
+  int b, T, first, tok_off;
+  __device__ __forceinline__ RaggedTile(const RaggedImage* imgs, const int* tile_prefix, int B) {
+    b = ragged_find(B, blockIdx.x, [&](int i) { return tile_prefix[i]; });
+    first = tile_prefix[b];
+    tok_off = imgs[b].tok_off;
+    T = imgs[b].Hp * imgs[b].Wp + 1;
+  }
+  __device__ __forceinline__ int q0(int bm) const { return ((int)blockIdx.x - first) * bm; }
+  __device__ __forceinline__ int row0() const { return tok_off; }
+};
+
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int FA_BM = 128, FA_BN = 128, FA_D = 64, FA_THREADS = 256;
 constexpr int FA_TILE = FA_BM * FA_D * 2;             // 16 KB: one [128 x 64] fp16 tile
@@ -131,9 +152,12 @@ constexpr int FA_KV_STAGES = 2;
 // Q (reused as the output box) | K ring | V ring = 80 KB: two CTAs per SM
 constexpr int FA_SMEM = FA_TILE * (1 + 2 * FA_KV_STAGES) + 1024;
 
-__global__ void __launch_bounds__(FA_THREADS, 2)
-attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO, int T,
-                       int heads) {
+// One CTA: the query tile `loc` names, head blockIdx.y. RAGGED (packed images of different sizes): tmO is the 2D output
+// [rows, d]; an image's last tile, if it ends past T, is stored from registers row by row, so it writes no row of the
+// next image; `out` is that output.
+template <bool RAGGED, typename Loc>
+__device__ __forceinline__ void attention_wgmma_tile(const CUtensorMap& tmQKV, const CUtensorMap& tmO, Loc loc,
+                                                     int heads, __half* out) {
   extern __shared__ uint8_t fa_smem[];
   __shared__ __align__(8) uint64_t bars[1 + 2 * FA_KV_STAGES];
   const uint32_t raw = smem_u32(fa_smem);
@@ -143,10 +167,11 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int wg = tid >> 7, wi = (tid >> 5) & 3;
-  const int q0 = blockIdx.x * FA_BM, h = blockIdx.y, b = blockIdx.z;
+  const int q0 = loc.q0(FA_BM), h = blockIdx.y, b = loc.b;
   const int d = heads * FA_D;
+  const int T = loc.T;
   const int nt = (T + FA_BN - 1) / FA_BN;
-  const int row0 = b * T;   // first row of this image in [B*T, 3d]
+  const int row0 = loc.row0();   // first row of this image in [rows, 3d]
 
   auto load_kv = [&](int j) {
     const int s = j % FA_KV_STAGES;
@@ -206,6 +231,20 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
   softmax_rowsum(l_run);
   const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
   const int r0 = 64 * wg + 16 * wi + (lane >> 2);
+  if constexpr (RAGGED) {
+    if (q0 + FA_BM > T) {   // the image's last, partial tile: masked direct stores
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = q0 + r0 + 8 * hh;
+        if (row >= T) continue;
+        const float inv = hh ? inv1 : inv0;
+        uint32_t* orow = reinterpret_cast<uint32_t*>(out + ((long long)row0 + row) * d + h * FA_D + fc);
+#pragma unroll
+        for (int i = 0; i < 8; ++i) orow[4 * i] = pack_half2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv);
+      }
+      return;
+    }
+  }
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
 #pragma unroll
@@ -221,10 +260,26 @@ attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_c
   fence_proxy_async_smem();
   __syncthreads();
   if (tid == 0) {
-    tma_store_3d(&tmO, sQ, h * FA_D, q0, b);
+    if constexpr (RAGGED)
+      tma_store_2d(&tmO, sQ, h * FA_D, row0 + q0);
+    else
+      tma_store_3d(&tmO, sQ, h * FA_D, q0, b);
     tma_store_commit();
     tma_store_wait_all<0>();
   }
+}
+
+__global__ void __launch_bounds__(FA_THREADS, 2)
+attention_wgmma_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO, int T,
+                       int heads) {
+  attention_wgmma_tile<false>(tmQKV, tmO, UniformTile{(int)blockIdx.z, T}, heads, nullptr);
+}
+
+__global__ void __launch_bounds__(FA_THREADS, 2)
+attention_wgmma_ragged_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmO,
+                              const RaggedImage* __restrict__ imgs, const int* __restrict__ tile_prefix, int B,
+                              int heads, __half* __restrict__ out) {
+  attention_wgmma_tile<true>(tmQKV, tmO, RaggedTile(imgs, tile_prefix, B), heads, out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -234,8 +289,10 @@ constexpr int AS_Q = 3 * 2 * AS_BOX;                   // Q': 3 groups x 128 row
 constexpr int AS_KV = 3 * AS_BOX;                      // one K' or V' stage: 3 groups x 64 keys
 constexpr int AS_SMEM = AS_Q + 2 * AS_STAGES * AS_KV + 1024;
 
-__global__ void __launch_bounds__(AS_THREADS, 1)
-attention_split_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __restrict__ out, int T, int heads) {
+// One CTA: the query tile `loc` names, head blockIdx.y (rows past T are not stored).
+template <typename Loc>
+__device__ __forceinline__ void attention_split_tile(const CUtensorMap& tmQKV, __half* __restrict__ out, Loc loc,
+                                                     int heads) {
   extern __shared__ uint8_t as_smem[];
   __shared__ __align__(8) uint64_t bars[1 + 2 * AS_STAGES];
   const uint32_t base = (smem_u32(as_smem) + 1023u) & ~1023u;
@@ -244,10 +301,11 @@ attention_split_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __rest
 
   const int tid = threadIdx.x, lane = tid & 31;
   const int wg = tid >> 7, wi = (tid >> 5) & 3;
-  const int q0 = blockIdx.x * AS_BM, h = blockIdx.y, b = blockIdx.z;
+  const int q0 = loc.q0(AS_BM), h = blockIdx.y;
   const int d = heads * 64;
+  const int T = loc.T;
   const int nt = (T + AS_BN - 1) / AS_BN;
-  const int row0 = b * T;
+  const int row0 = loc.row0();
 
   auto load_kv = [&](int j) {
     const int s = j % AS_STAGES;
@@ -338,6 +396,18 @@ attention_split_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __rest
   }
 }
 
+__global__ void __launch_bounds__(AS_THREADS, 1)
+attention_split_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __restrict__ out, int T, int heads) {
+  attention_split_tile(tmQKV, out, UniformTile{(int)blockIdx.z, T}, heads);
+}
+
+__global__ void __launch_bounds__(AS_THREADS, 1)
+attention_split_ragged_kernel(const __grid_constant__ CUtensorMap tmQKV, __half* __restrict__ out,
+                              const RaggedImage* __restrict__ imgs, const int* __restrict__ tile_prefix, int B,
+                              int heads) {
+  attention_split_tile(tmQKV, out, RaggedTile(imgs, tile_prefix, B), heads);
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 int launch_attention_tc(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st) {
   DSS_REQUIRE(B > 0 && T > 0 && heads > 0, "attention: empty problem");
@@ -372,6 +442,45 @@ int launch_attention_split(const void* qkv_split, void* out, int B, int T, int h
   dim3 grid(cdiv(T, AS_BM), heads, B);
   LaunchScope scope(st, KC_ATTENTION);
   attention_split_kernel<<<grid, AS_THREADS, AS_SMEM, st>>>(tm, reinterpret_cast<__half*>(out), T, heads);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
+int launch_attention_tc_ragged(const void* qkv, void* out, const RaggedImage* imgs, const int* tile_prefix, int B,
+                               long long M, int tiles, int heads, cudaStream_t st) {
+  DSS_REQUIRE(B > 0 && M > 0 && tiles > 0 && heads > 0, "attention_ragged: empty problem");
+  static bool attr_set = false;
+  if (!attr_set) {
+    DSS_CHECK_CUDA(cudaFuncSetAttribute(attention_wgmma_ragged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        FA_SMEM));
+    attr_set = true;
+  }
+  CUtensorMap tm, tmO;
+  int rc = make_tmap_f16(&tm, qkv, (int)M, 3 * heads * FA_D, FA_BM);
+  if (rc) return rc;
+  if ((rc = make_tmap_out(&tmO, out, (int)M, heads * FA_D, 0))) return rc;
+  LaunchScope scope(st, KC_ATTENTION);
+  attention_wgmma_ragged_kernel<<<dim3(tiles, heads), FA_THREADS, FA_SMEM, st>>>(tm, tmO, imgs, tile_prefix, B, heads,
+                                                                                 reinterpret_cast<__half*>(out));
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
+int launch_attention_split_ragged(const void* qkv_split, void* out, const RaggedImage* imgs, const int* tile_prefix,
+                                  int B, long long M, int tiles, int heads, cudaStream_t st) {
+  DSS_REQUIRE(B > 0 && M > 0 && tiles > 0 && heads > 0, "attention_split_ragged: empty problem");
+  static bool attr_set = false;
+  if (!attr_set) {
+    DSS_CHECK_CUDA(cudaFuncSetAttribute(attention_split_ragged_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        AS_SMEM));
+    attr_set = true;
+  }
+  CUtensorMap tm;
+  int rc = make_tmap_f16(&tm, qkv_split, (int)M, 9 * heads * 64, 64);
+  if (rc) return rc;
+  LaunchScope scope(st, KC_ATTENTION);
+  attention_split_ragged_kernel<<<dim3(tiles, heads), AS_THREADS, AS_SMEM, st>>>(tm, reinterpret_cast<__half*>(out),
+                                                                                 imgs, tile_prefix, B, heads);
   DSS_CHECK_CUDA(cudaGetLastError());
   return DSS_OK;
 }

@@ -50,6 +50,8 @@ int make_tmap_out3d_f16(CUtensorMap* tm, const void* ptr, int images, int rows, 
 int gemm_tile_n();
 int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMap* tmC, const float* bias, void* out,
                 int M, int N, int K, int epi, const float* aux, int rin, int rout, cudaStream_t st, int kclass, int bn);
+int gemm_f16_tc_rows(const CUtensorMap& tmA, const CUtensorMap& tmB, const float* bias, void* out, int M, int N, int K,
+                     int epi, const float* aux, const int* row_map, cudaStream_t st, int kclass);
 int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int images, int Nimg, int d, float* Wout, int ldw,
                      int ncols, const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts,
                      float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st);
@@ -66,6 +68,37 @@ int launch_gelu_split(const float* h, void* out, long long M, int n, cudaStream_
 int launch_qkv_split(const float* qkv, void* out, long long M, int d, cudaStream_t st);
 int launch_attention_tc(const void* qkv, void* out, int B, int T, int heads, cudaStream_t st);
 int launch_attention_split(const void* qkv_split, void* out, int B, int T, int heads, cudaStream_t st);
+
+// ---- ragged ViT batches: B images of any sizes, packed one after another (vit.cu). Device table entry of image b:
+// its pixels start at pixel px_off of the packed [sum H W, 3] input, its patch rows at patch_off, its T = Hp Wp + 1
+// token rows (CLS first) at tok_off; its positional-interpolation indices and weights at axis_off of the axis tables
+// (Hp y entries, then Wp x entries); stored: the stored positional grid is used unchanged (identity rule).
+struct RaggedImage {
+  long long px_off;
+  int H, W, Hp, Wp;
+  int patch_off, tok_off, axis_off, stored;
+};
+// the image whose first row off(b) is the last one <= x (off nondecreasing in b, off(0) = 0)
+template <typename Off>
+__device__ __forceinline__ int ragged_find(int B, long long x, Off&& off) {
+  int lo = 0, hi = B - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if ((long long)off(mid) <= x) lo = mid; else hi = mid - 1;
+  }
+  return lo;
+}
+int launch_im2col_ragged(const uint8_t* img, void* patches, const RaggedImage* imgs, int B, long long n_patches, int P,
+                         bool split, cudaStream_t st);
+int launch_cls_row_ragged(float* x, const float* cls, const float* pos_all, const RaggedImage* imgs, int B, int d,
+                          cudaStream_t st);
+int launch_pos_ragged(const float* pos_src, int grid0, int d, const RaggedImage* imgs, int B, long long M,
+                      const int* axis_idx, const float* axis_w, float* pos_all, cudaStream_t st);
+// tile_prefix [B + 1]: image b's 128-query tiles are CTAs [tile_prefix[b], tile_prefix[b + 1])
+int launch_attention_tc_ragged(const void* qkv, void* out, const RaggedImage* imgs, const int* tile_prefix, int B,
+                               long long M, int tiles, int heads, cudaStream_t st);
+int launch_attention_split_ragged(const void* qkv_split, void* out, const RaggedImage* imgs, const int* tile_prefix,
+                                  int B, long long M, int tiles, int heads, cudaStream_t st);
 
 // ---------------------------------------------------------------- launch accounting / per-class device timing
 enum KernelClass {

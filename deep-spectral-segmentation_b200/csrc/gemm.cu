@@ -38,6 +38,10 @@ constexpr int BOX_BYTES = BM * 128;      // TMA-store path staging box: 128 rows
 
 // epilogues whose output rows are the GEMM rows: written with TMA (the row-remapping ones keep the manual path)
 constexpr int EPI_AFFINITY_F32 = 100;    // internal epilogue id (not in the public enum): batched patch-affinity tile
+// internal ids of the ragged ViT batch: DSS_EPI_PATCH_F32 / DSS_EPI_DROPCLS_F32 with the destination row of GEMM row m
+// read from p.row_map[m] (-1: skip) instead of computed from rin / rout; the patch epilogue's positional row is that
+// destination row of p.aux (laid out like the residual stream)
+constexpr int EPI_PATCH_ROWS_F32 = 101, EPI_DROPCLS_ROWS_F32 = 102;
 __host__ __device__ constexpr bool epi_uses_tma_store(int epi) {
   return epi == DSS_EPI_BIAS_F16 || epi == DSS_EPI_BIAS_GELU_F16 || epi == DSS_EPI_BIAS_RESID_F32 ||
          epi == DSS_EPI_BIAS_F32 || epi == EPI_AFFINITY_F32;
@@ -87,6 +91,8 @@ struct EpiParams {
   int ld_part;
   // phase trace (dss_debug_gemm_trace only; read by the TRACE instantiations, layout at trace_stride)
   unsigned long long* trace;
+  // destination row per GEMM row (EPI_PATCH_ROWS_F32 / EPI_DROPCLS_ROWS_F32)
+  const int* row_map;
 };
 
 // Phase trace layout, per CTA (blockIdx.x): [0] ns the producer warp spent waiting on empty ring slots, [1..3] unused,
@@ -105,6 +111,8 @@ __device__ __forceinline__ long long out_row(int m, const EpiParams& p) {
   } else if constexpr (EPI == DSS_EPI_DROPCLS_F32) {
     const int t = m % p.rin;
     return t == 0 ? -1 : (long long)(m / p.rin) * p.rout + t - 1;
+  } else if constexpr (EPI == EPI_PATCH_ROWS_F32 || EPI == EPI_DROPCLS_ROWS_F32) {
+    return __ldg(p.row_map + m);
   } else {
     return m;
   }
@@ -528,6 +536,8 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
               if (m < M) {
                 if constexpr (EPI == DSS_EPI_PATCH_F32)
                   y[i] = __ldg(reinterpret_cast<const float4*>(p.aux + (long long)((m % p.rin) + 1) * p.ldo + nc + cl));
+                if constexpr (EPI == EPI_PATCH_ROWS_F32)
+                  y[i] = __ldg(reinterpret_cast<const float4*>(p.aux + out_row<EPI>(m, p) * p.ldo + nc + cl));
               }
             }
 #pragma unroll
@@ -889,6 +899,23 @@ int gemm_f16_tc(const CUtensorMap& tmA, const CUtensorMap& tmB, const CUtensorMa
     case DSS_EPI_DROPCLS_F32: return launch_tc<DSS_EPI_DROPCLS_F32>(tmA, tmB, tmC, M, N, K, p, st, kclass, bn);
   }
   set_error("gemm: unknown epilogue %d", epi);
+  return DSS_ERR_BAD_ARG;
+}
+
+// The row-table forms of the patch and DROPCLS epilogues (ragged ViT batches): GEMM row m goes to output row
+// row_map[m] (device, -1: skip); the patch epilogue adds positional row row_map[m] of aux. Cooperative schedule, bn 128.
+int gemm_f16_tc_rows(const CUtensorMap& tmA, const CUtensorMap& tmB, const float* bias, void* out, int M, int N, int K,
+                     int epi, const float* aux, const int* row_map, cudaStream_t st, int kclass) {
+  int rc = check_gemm_args(M, N, K, DSS_EPI_BIAS_F32, bias, out, aux, 0, 0);
+  if (rc) return rc;
+  DSS_REQUIRE(row_map, "gemm: row-table epilogue needs row_map");
+  EpiParams p{out, bias, aux, N, 0, 0, 0, nullptr, nullptr, nullptr, 0.f, 0, 0, 0, nullptr, 0, nullptr, row_map};
+  if (epi == DSS_EPI_PATCH_F32) {
+    DSS_REQUIRE(aux != nullptr, "gemm: patch epilogue needs aux (pos embed)");
+    return launch_tc<EPI_PATCH_ROWS_F32>(tmA, tmB, nullptr, M, N, K, p, st, kclass, 128);
+  }
+  if (epi == DSS_EPI_DROPCLS_F32) return launch_tc<EPI_DROPCLS_ROWS_F32>(tmA, tmB, nullptr, M, N, K, p, st, kclass, 128);
+  set_error("gemm: no row-table form of epilogue %d", epi);
   return DSS_ERR_BAD_ARG;
 }
 

@@ -10,9 +10,12 @@
 // tensor-core work.
 // The block the reference hooks is pruned to LN1 + the K third of its qkv projection, CLS row dropped in the
 // GEMM epilogue, which writes the fp32 features directly in the reference's [B, N, d] layout.
+#include <limits.h>
 #include <math.h>
+#include <string.h>
 
 #include <algorithm>
+#include <cstring>
 #include <map>
 #include <tuple>
 #include <utility>
@@ -38,6 +41,14 @@ layernorm_rows_f32_kernel(const float* __restrict__ x, long long row_stride, con
   for (int i = lane; i < d; i += 32) y[(long long)row * d + i] = (xr[i] - mean) * rstd * gamma[i] + beta[i];
 }
 
+// a ragged batch's CLS rows x[tok_off_b, :] -> y [B, d] (the input of the final norm)
+__global__ void gather_cls_rows_kernel(const float* __restrict__ x, const RaggedImage* __restrict__ imgs,
+                                       float* __restrict__ y, int B, int d) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * d) return;
+  y[i] = x[(long long)imgs[i / d].tok_off * d + i % d];
+}
+
 __global__ void f32_to_f16_kernel(const float* __restrict__ src, __half* __restrict__ dst, size_t n) {
   const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) dst[i] = __float2half_rn(src[i]);
@@ -61,6 +72,7 @@ struct dss_vit {
   __half* patch_w = nullptr;
   float *patch_b = nullptr, *cls = nullptr;
   float *norm_w = nullptr, *norm_b = nullptr;   // final LayerNorm (only needed by dss_vit_forward_cls)
+  float* pos_dev = nullptr;   // [1 + grid0^2, d] the stored positional grid (ragged batches interpolate it on the device)
   CUtensorMap tm_patch;
   std::vector<dss::BlockW> blocks;
   std::vector<float> pos_host;                        // [1 + grid0^2, d] fp32 host copy
@@ -176,9 +188,10 @@ struct VitWs {
   size_t total;
 };
 
-static VitWs carve(const dss_vit_config& c, int B, int Hp, int Wp, void* base, int precision) {
-  const int Np = Hp * Wp, T = Np + 1, d = c.dim;
-  const size_t M = (size_t)B * T, ks = precision == DSS_VIT_PRECISION_FP32 ? 3 : 1;
+// n_patches patch rows and M token rows (B Np and B T for a uniform batch)
+static VitWs carve(const dss_vit_config& c, size_t n_patches, size_t M, void* base, int precision) {
+  const int d = c.dim;
+  const size_t ks = precision == DSS_VIT_PRECISION_FP32 ? 3 : 1;
   uint8_t* p = reinterpret_cast<uint8_t*>(base);
   size_t off = 0;
   auto take = [&](size_t bytes) {
@@ -188,7 +201,7 @@ static VitWs carve(const dss_vit_config& c, int B, int Hp, int Wp, void* base, i
   };
   VitWs w;
   const size_t hd = (size_t)c.mlp_ratio * d;
-  w.patches = reinterpret_cast<__half*>(take((size_t)B * Np * ks * 3 * c.patch * c.patch * 2));
+  w.patches = reinterpret_cast<__half*>(take(n_patches * ks * 3 * c.patch * c.patch * 2));
   w.x = reinterpret_cast<float*>(take(M * d * 4));
   w.xn = reinterpret_cast<__half*>(take(M * ks * d * 2));
   w.attn = reinterpret_cast<__half*>(take(M * ks * d * 2));
@@ -205,17 +218,38 @@ static VitWs carve(const dss_vit_config& c, int B, int Hp, int Wp, void* base, i
   return w;
 }
 
+// A ragged batch as vit_run sees it: B images of any sizes, n_patches patch rows and M token rows packed image after
+// image, and the device tables (in the workspace) that the shape-dependent kernels read.
+struct Ragged {
+  int B;
+  long long n_patches, M;
+  int tiles;                      // 128-query attention tiles over all images
+  const RaggedImage* imgs;        // [B]
+  const int* tile_prefix;         // [B + 1]
+  const int* patch_rows;          // [n_patches] token row of each patch row
+  const int* k_rows;              // [M] feature row of each token row (-1: CLS)
+  float* pos_all;                 // [M, d] positional rows, laid out like the residual stream
+};
+
 // modes 1 and 2 after the blocks: the residual stream, or the final LayerNorm of the CLS rows
-static int vit_tail(const dss_vit* h, const float* x, int mode, float* out, int B, int T, cudaStream_t st) {
+static int vit_tail(const dss_vit* h, const float* x, int mode, float* out, int B, int T, const Ragged* rg,
+                    cudaStream_t st) {
   const int d = h->cfg.dim;
   if (mode == 2) {
     // upstream VisionTransformer.forward: x = norm(x); return x[:, 0]  (LayerNorm is row-wise: only the CLS rows)
     DSS_REQUIRE(h->norm_w && h->norm_b, "vit: the final LayerNorm weights (norm.weight / norm.bias) were not loaded");
     LaunchScope scope(st, KC_LAYERNORM);
-    layernorm_rows_f32_kernel<<<cdiv(B, 4), 128, 0, st>>>(x, (long long)T * d, h->norm_w, h->norm_b, out, B, d,
-                                                          h->cfg.ln_eps);
+    long long stride = (long long)T * d;
+    if (rg) {   // the CLS rows gathered into pos_all, which is free once the tokens are embedded
+      gather_cls_rows_kernel<<<cdiv(B * d, 256), 256, 0, st>>>(x, rg->imgs, rg->pos_all, B, d);
+      DSS_CHECK_CUDA(cudaGetLastError());
+      x = rg->pos_all;
+      stride = d;
+    }
+    layernorm_rows_f32_kernel<<<cdiv(B, 4), 128, 0, st>>>(x, stride, h->norm_w, h->norm_b, out, B, d, h->cfg.ln_eps);
     DSS_CHECK_CUDA(cudaGetLastError());
   } else {
+    DSS_REQUIRE(!rg, "vit: no residual-stream output for ragged batches");
     DSS_CHECK_CUDA(cudaMemcpyAsync(out, x, (size_t)B * T * d * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
   return DSS_OK;
@@ -227,32 +261,39 @@ static int vit_tail(const dss_vit* h, const float* x, int mode, float* out, int 
 // DSS_VIT_PRECISION_FP32 runs the same sequence on split operands: every GEMM runs the fp16 path's kernel and epilogue
 // at K' = 3 K; the qkv and fc1 GEMMs write fp32 (DSS_EPI_BIAS_F32), which qkv_split_kernel / gelu_split_kernel turn
 // into the next product's split operands.
+// rg: a ragged batch (modes 0 and 2; H, W unused). Only the token embedding, attention, the K projection's CLS drop and
+// the final-norm rows depend on image boundaries; they read rg's tables, every other step is row-wise over M rows.
 static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_full, int mode, float* out, void* ws,
-                   size_t ws_bytes, cudaStream_t st, int pad = 0, int which = 1, float* cls_attn = nullptr) {
+                   size_t ws_bytes, cudaStream_t st, int pad = 0, int which = 1, float* cls_attn = nullptr,
+                   const Ragged* rg = nullptr) {
   DSS_REQUIRE(h && h->loaded, "vit: weights not loaded");
   DSS_REQUIRE(img && (out || cls_attn) && ws, "vit: null pointer");
   const dss_vit_config& c = h->cfg;
   const int P = c.patch, d = c.dim, hd = c.mlp_ratio * d;
-  const int Hp = pad ? cdiv(H, P) : H / P, Wp = pad ? cdiv(W, P) : W / P;
-  DSS_REQUIRE(B > 0 && Hp > 0 && Wp > 0, "vit: image %dx%d smaller than one %d-pixel patch", H, W, P);
+  const int Hp = rg ? 0 : (pad ? cdiv(H, P) : H / P), Wp = rg ? 0 : (pad ? cdiv(W, P) : W / P);
+  DSS_REQUIRE(rg || (B > 0 && Hp > 0 && Wp > 0), "vit: image %dx%d smaller than one %d-pixel patch", H, W, P);
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "vit: workspace must be 256-byte aligned");
-  const int Np = Hp * Wp, T = Np + 1, M = B * T, Kp = 3 * P * P;
+  const int Np = Hp * Wp, T = Np + 1, Kp = 3 * P * P;
+  const int M = rg ? (int)rg->M : B * T, n_patches = rg ? (int)rg->n_patches : B * Np;
   const bool split = h->precision == DSS_VIT_PRECISION_FP32;
   const int ks = split ? 3 : 1;   // fp16 values per operand value
-  VitWs w = carve(c, B, Hp, Wp, ws, h->precision);
+  VitWs w = carve(c, (size_t)n_patches, (size_t)M, ws, h->precision);
   if (ws_bytes < w.total) {
     set_error("vit: workspace too small (%zu < %zu)", ws_bytes, w.total);
     return DSS_ERR_WORKSPACE;
   }
   int rc;
   float* pos = nullptr;
-  // forward_k's and localization's inputs are cropped or padded to patch multiples by the reference before the model
-  // sees them, so their patch grid decides; the model's own forward (box crops) and the token hook take the image as is
-  const bool square = (mode == 1 || mode == 2) ? H == W : Hp == Wp;
-  if ((rc = get_pos(h, Hp, Wp, square, st, &pos))) return rc;
+  if (!rg) {
+    // forward_k's and localization's inputs are cropped or padded to patch multiples by the reference before the model
+    // sees them, so their patch grid decides; the model's own forward (box crops) and the token hook take the image as
+    // is
+    const bool square = (mode == 1 || mode == 2) ? H == W : Hp == Wp;
+    if ((rc = get_pos(h, Hp, Wp, square, st, &pos))) return rc;
+  }
 
   CUtensorMap tm_patches, tm_xn, tm_attn, tm_hid;
-  if ((rc = make_tmap_f16(&tm_patches, w.patches, B * Np, ks * Kp, 128))) return rc;
+  if ((rc = make_tmap_f16(&tm_patches, w.patches, n_patches, ks * Kp, 128))) return rc;
   if ((rc = make_tmap_f16(&tm_xn, w.xn, M, ks * d, 128))) return rc;
   if ((rc = make_tmap_f16(&tm_attn, w.attn, M, ks * d, 128))) return rc;
   if ((rc = make_tmap_f16(&tm_hid, w.hid, M, ks * hd, 128))) return rc;
@@ -264,28 +305,40 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   if ((rc = make_tmap_out(&tm_hid_out, split ? (void*)w.f32 : w.hid, M, hd, split))) return rc;
 
   // tokens: x[b, 1+n, :] = patch_embed + pos ; x[b, 0, :] = cls + pos[0]
-  if ((rc = launch_im2col(img, w.patches, B, H, W, P, pad, split, st))) return rc;
-  if ((rc = gemm_f16_tc(tm_patches, h->tm_patch, nullptr, h->patch_b, w.x, B * Np, d, ks * Kp, DSS_EPI_PATCH_F32, pos, Np,
-                        T, st, KC_GEMM_PATCH, 128)))
-    return rc;
-  if ((rc = launch_cls_row(w.x, h->cls, pos, B, T, d, st))) return rc;
+  if (rg) {
+    if ((rc = launch_im2col_ragged(img, w.patches, rg->imgs, B, n_patches, P, split, st))) return rc;
+    if ((rc = gemm_f16_tc_rows(tm_patches, h->tm_patch, h->patch_b, w.x, n_patches, d, ks * Kp, DSS_EPI_PATCH_F32,
+                               rg->pos_all, rg->patch_rows, st, KC_GEMM_PATCH)))
+      return rc;
+    if ((rc = launch_cls_row_ragged(w.x, h->cls, rg->pos_all, rg->imgs, B, d, st))) return rc;
+  } else {
+    if ((rc = launch_im2col(img, w.patches, B, H, W, P, pad, split, st))) return rc;
+    if ((rc = gemm_f16_tc(tm_patches, h->tm_patch, nullptr, h->patch_b, w.x, n_patches, d, ks * Kp, DSS_EPI_PATCH_F32,
+                          pos, Np, T, st, KC_GEMM_PATCH, 128)))
+      return rc;
+    if ((rc = launch_cls_row(w.x, h->cls, pos, B, T, d, st))) return rc;
+  }
 
   // the full qkv projection: the attention operands (fp16), or the fp32 values they are split from
   auto qkv_gemm = [&](const BlockW& bw) {
     return gemm_f16_tc(tm_xn, bw.tm_qkv, &tm_qkv_out, bw.qkv_b, split ? (void*)w.f32 : w.qkv, M, 3 * d, ks * d,
                        split ? DSS_EPI_BIAS_F32 : DSS_EPI_BIAS_F16, nullptr, 0, 0, st, KC_GEMM_QKV, gemm_tile_n());
   };
+  auto attention = [&]() {
+    if (split) {
+      if ((rc = launch_qkv_split(w.f32, w.qkv, M, d, st))) return rc;
+      return rg ? launch_attention_split_ragged(w.qkv, w.attn, rg->imgs, rg->tile_prefix, B, M, rg->tiles, c.heads, st)
+                : launch_attention_split(w.qkv, w.attn, B, T, c.heads, st);
+    }
+    return rg ? launch_attention_tc_ragged(w.qkv, w.attn, rg->imgs, rg->tile_prefix, B, M, rg->tiles, c.heads, st)
+              : launch_attention_tc(w.qkv, w.attn, B, T, c.heads, st);
+  };
   // LayerNorm kernel + GEMM: LayerNorm fused into the qkv / fc1 GEMMs measured slower (DESIGN.md section 9)
   for (int l = 0; l < n_full; ++l) {
     const BlockW& bw = h->blocks[l];
     if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, split, st))) return rc;
     if ((rc = qkv_gemm(bw))) return rc;
-    if (split) {
-      if ((rc = launch_qkv_split(w.f32, w.qkv, M, d, st))) return rc;
-      if ((rc = launch_attention_split(w.qkv, w.attn, B, T, c.heads, st))) return rc;
-    } else {
-      if ((rc = launch_attention_tc(w.qkv, w.attn, B, T, c.heads, st))) return rc;
-    }
+    if ((rc = attention())) return rc;
     if ((rc = gemm_f16_tc(tm_attn, bw.tm_proj, &tm_x_out, bw.proj_b, w.x, M, d, ks * d, DSS_EPI_BIAS_RESID_F32, nullptr,
                           0, 0, st, KC_GEMM_PROJ, gemm_tile_n())))
       return rc;
@@ -299,21 +352,173 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
                           0, st, KC_GEMM_FC2, gemm_tile_n())))
       return rc;
   }
-  if (mode == 1 || mode == 2) return vit_tail(h, w.x, mode, out, B, T, st);
+  if (mode == 1 || mode == 2) return vit_tail(h, w.x, mode, out, B, T, rg, st);
 
   const BlockW& bw = h->blocks[n_full];
   if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, split, st))) return rc;
   if (out) {   // qkv[b, 1+n, which*d : (which+1)*d] in fp32, CLS rows dropped (which = 1: the K features)
     const CUtensorMap& tm = which == 0 ? bw.tm_q : (which == 1 ? bw.tm_k : bw.tm_v);
-    if ((rc = gemm_f16_tc(tm_xn, tm, nullptr, bw.qkv_b + (size_t)which * d, out, M, d, ks * d, DSS_EPI_DROPCLS_F32,
-                          nullptr, T, Np, st, KC_GEMM_KPROJ, 128)))
-      return rc;
+    rc = rg ? gemm_f16_tc_rows(tm_xn, tm, bw.qkv_b + (size_t)which * d, out, M, d, ks * d, DSS_EPI_DROPCLS_F32, nullptr,
+                               rg->k_rows, st, KC_GEMM_KPROJ)
+            : gemm_f16_tc(tm_xn, tm, nullptr, bw.qkv_b + (size_t)which * d, out, M, d, ks * d, DSS_EPI_DROPCLS_F32,
+                          nullptr, T, Np, st, KC_GEMM_KPROJ, 128);
+    if (rc) return rc;
   }
   if (cls_attn) {   // the full qkv projection the attention kernels read, then the CLS row of the softmax
+    DSS_REQUIRE(!rg, "vit: no CLS attention output for ragged batches");
     if ((rc = qkv_gemm(bw))) return rc;
     if ((rc = launch_cls_attention(split ? (const void*)w.f32 : w.qkv, split, B, T, c.heads, cls_attn, st))) return rc;
   }
   return DSS_OK;
+}
+
+// ---- ragged batches: host plan. Workspace = the forward's buffers (carve) | pos_all [M, d] fp32 | one block of tables
+// (RaggedImage [B], tile_prefix [B + 1], patch_rows [n_patches], k_rows [M], axis indices [A] and weights [4 A], A the
+// sum of Hp + Wp over the images whose positional grid is resampled), uploaded with one copy per forward.
+struct RaggedPlan {
+  std::vector<RaggedImage> imgs;
+  std::vector<int> tile_prefix, patch_rows, k_rows, axis_idx;
+  std::vector<float> axis_w;
+  long long n_patches = 0, M = 0, axis = 0;
+  size_t vit_bytes = 0, off_pos = 0, off_tables = 0, tables_bytes = 0, total = 0;
+  size_t t_imgs = 0, t_tiles = 0, t_prows = 0, t_krows = 0, t_aidx = 0, t_aw = 0;   // offsets inside the table block
+};
+
+constexpr int RAGGED_TILE = 128;   // query rows per attention CTA (FA_BM, AS_BM)
+
+// Validates the batch and lays out its workspace; with `tables`, also fills the host tables. mode: DSS_VIT_RAGGED_*.
+static int ragged_plan(const dss_vit* h, const int* dims, int B, int mode, bool tables, RaggedPlan& pl) {
+  DSS_REQUIRE(h && dims, "vit_ragged: null pointer");
+  DSS_REQUIRE(B > 0, "vit_ragged: B must be positive (got %d)", B);
+  DSS_REQUIRE(mode == DSS_VIT_RAGGED_K || mode == DSS_VIT_RAGGED_CLS, "vit_ragged: unknown mode %d", mode);
+  const dss_vit_config& c = h->cfg;
+  const int P = c.patch, g = c.grid0;
+  long long px = 0, np = 0, M = 0, axis = 0, tiles = 0;
+  for (int b = 0; b < B; ++b) {
+    const int H = dims[2 * b], W = dims[2 * b + 1];
+    DSS_REQUIRE(H >= 0 && W >= 0, "vit_ragged: image %d has negative size %dx%d", b, H, W);
+    DSS_REQUIRE(H >= P && W >= P, "vit_ragged: image %d (%dx%d) is smaller than one %d-pixel patch", b, H, W, P);
+    const long long Hp = H / P, Wp = W / P;
+    // the identity rule of interpolate_pos_encoding: pixel H == W for the model's own forward, Hp == Wp for forward_k
+    const bool square = mode == DSS_VIT_RAGGED_CLS ? H == W : Hp == Wp;
+    if (!pos_is_stored(g, (int)Hp, (int)Wp, square)) axis += Hp + Wp;
+    px += (long long)H * W;
+    np += Hp * Wp;
+    M += Hp * Wp + 1;
+    tiles += (Hp * Wp + RAGGED_TILE) / RAGGED_TILE;
+  }
+  // row counts are the extents of the tensor maps and GEMM problems (int); tile counts a grid dimension
+  if (M > INT_MAX - 2 * RAGGED_TILE || tiles > INT_MAX) {
+    set_error("vit_ragged: %lld token rows do not fit the tensor-map extents", M);
+    return DSS_ERR_UNSUPPORTED;
+  }
+  pl.n_patches = np;
+  pl.M = M;
+  pl.axis = axis;
+  size_t off = 0;
+  auto part = [&off](size_t bytes) { const size_t o = off; off += align_up(bytes, 16); return o; };
+  pl.t_imgs = part((size_t)B * sizeof(RaggedImage));
+  pl.t_tiles = part((size_t)(B + 1) * 4);
+  pl.t_prows = part((size_t)np * 4);
+  pl.t_krows = part((size_t)M * 4);
+  pl.t_aidx = part((size_t)axis * 4);
+  pl.t_aw = part((size_t)axis * 16);
+  pl.tables_bytes = off;
+  pl.vit_bytes = carve(c, (size_t)np, (size_t)M, nullptr, h->precision).total;
+  pl.off_pos = pl.vit_bytes;
+  pl.off_tables = pl.off_pos + align_up((size_t)M * c.dim * 4, 1024);
+  pl.total = pl.off_tables + align_up(pl.tables_bytes, 1024);
+  if (!tables) return DSS_OK;
+
+  pl.imgs.resize(B);
+  pl.tile_prefix.assign(1, 0);
+  pl.patch_rows.resize((size_t)np);
+  pl.k_rows.resize((size_t)M);
+  pl.axis_idx.clear();
+  pl.axis_w.clear();
+  long long pxo = 0, po = 0, to = 0, fo = 0;
+  std::vector<int> iy, ix;
+  std::vector<float> wy, wx;
+  for (int b = 0; b < B; ++b) {
+    const int H = dims[2 * b], W = dims[2 * b + 1], Hp = H / P, Wp = W / P, Np = Hp * Wp;
+    const bool square = mode == DSS_VIT_RAGGED_CLS ? H == W : Hp == Wp;
+    RaggedImage& im = pl.imgs[b];
+    im.px_off = pxo;
+    im.H = H; im.W = W; im.Hp = Hp; im.Wp = Wp;
+    im.patch_off = (int)po;
+    im.tok_off = (int)to;
+    im.stored = pos_is_stored(g, Hp, Wp, square) ? 1 : 0;
+    im.axis_off = (int)pl.axis_idx.size();
+    if (!im.stored) {   // the per-axis indices and weights of interp_pos_host
+      interp_axis(g, Hp, ((double)Hp + 0.1) / (double)g, iy, wy);
+      interp_axis(g, Wp, ((double)Wp + 0.1) / (double)g, ix, wx);
+      pl.axis_idx.insert(pl.axis_idx.end(), iy.begin(), iy.end());
+      pl.axis_idx.insert(pl.axis_idx.end(), ix.begin(), ix.end());
+      pl.axis_w.insert(pl.axis_w.end(), wy.begin(), wy.end());
+      pl.axis_w.insert(pl.axis_w.end(), wx.begin(), wx.end());
+    }
+    pl.tile_prefix.push_back(pl.tile_prefix.back() + (Np + RAGGED_TILE) / RAGGED_TILE);
+    pl.k_rows[(size_t)to] = -1;
+    for (int n = 0; n < Np; ++n) {
+      pl.patch_rows[(size_t)(po + n)] = (int)(to + 1 + n);
+      pl.k_rows[(size_t)(to + 1 + n)] = (int)(fo + n);
+    }
+    pxo += (long long)H * W;
+    po += Np;
+    to += Np + 1;
+    fo += Np;
+  }
+  return DSS_OK;
+}
+
+// Validates a ragged batch (rmode: DSS_VIT_RAGGED_*), uploads its tables into the workspace and computes its
+// positional tables (rg.pos_all).
+static int ragged_setup(dss_vit* h, const int* dims, int B, int rmode, void* ws, size_t ws_bytes, cudaStream_t st,
+                        RaggedPlan& pl, Ragged& rg) {
+  int rc = ragged_plan(h, dims, B, rmode, true, pl);
+  if (rc) return rc;
+  DSS_REQUIRE(ws, "vit_ragged: null workspace");
+  DSS_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "vit_ragged: workspace must be 256-byte aligned");
+  DSS_REQUIRE(ws_bytes >= pl.total, "vit_ragged: workspace too small (%zu < %zu)", ws_bytes, pl.total);
+  DSS_REQUIRE(h->loaded, "vit: weights not loaded");
+
+  std::vector<uint8_t> blob(pl.tables_bytes);
+  auto put = [&blob](size_t o, const void* src, size_t bytes) { if (bytes) std::memcpy(blob.data() + o, src, bytes); };
+  put(pl.t_imgs, pl.imgs.data(), pl.imgs.size() * sizeof(RaggedImage));
+  put(pl.t_tiles, pl.tile_prefix.data(), pl.tile_prefix.size() * 4);
+  put(pl.t_prows, pl.patch_rows.data(), pl.patch_rows.size() * 4);
+  put(pl.t_krows, pl.k_rows.data(), pl.k_rows.size() * 4);
+  put(pl.t_aidx, pl.axis_idx.data(), pl.axis_idx.size() * 4);
+  put(pl.t_aw, pl.axis_w.data(), pl.axis_w.size() * 4);
+  uint8_t* base = reinterpret_cast<uint8_t*>(ws);
+  uint8_t* tb = base + pl.off_tables;
+  // pageable source: the call returns once the bytes are staged, so `blob` may go out of scope (no stream sync)
+  DSS_CHECK_CUDA(cudaMemcpyAsync(tb, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
+  rg.B = B;
+  rg.n_patches = pl.n_patches;
+  rg.M = pl.M;
+  rg.tiles = pl.tile_prefix.back();
+  rg.imgs = reinterpret_cast<const RaggedImage*>(tb + pl.t_imgs);
+  rg.tile_prefix = reinterpret_cast<const int*>(tb + pl.t_tiles);
+  rg.patch_rows = reinterpret_cast<const int*>(tb + pl.t_prows);
+  rg.k_rows = reinterpret_cast<const int*>(tb + pl.t_krows);
+  rg.pos_all = reinterpret_cast<float*>(base + pl.off_pos);
+  if ((rc = launch_pos_ragged(h->pos_dev, h->cfg.grid0, h->cfg.dim, rg.imgs, B, pl.M,
+                              reinterpret_cast<const int*>(tb + pl.t_aidx), reinterpret_cast<const float*>(tb + pl.t_aw),
+                              rg.pos_all, st)))
+    return rc;
+  return DSS_OK;
+}
+
+// n_full / mode as vit_run (0: K projection of block n_full, 2: final-norm CLS)
+static int vit_ragged(dss_vit* h, const uint8_t* img, const int* dims, int B, int n_full, int mode, float* out, void* ws,
+                      size_t ws_bytes, cudaStream_t st) {
+  DSS_REQUIRE(img && out, "vit_ragged: null pointer");
+  RaggedPlan pl;
+  Ragged rg;
+  int rc = ragged_setup(h, dims, B, mode == 0 ? DSS_VIT_RAGGED_K : DSS_VIT_RAGGED_CLS, ws, ws_bytes, st, pl, rg);
+  if (rc) return rc;
+  return vit_run(h, img, B, 0, 0, n_full, mode, out, ws, pl.vit_bytes, st, 0, 1, nullptr, &rg);
 }
 
 }  // namespace dss
@@ -367,6 +572,7 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
   };
   const size_t o_patch_w = reserve(d * Kp * 2 * ks), o_patch_b = reserve(d * 4), o_cls = reserve(d * 4);
   const size_t o_norm_w = reserve(d * 4), o_norm_b = reserve(d * 4);
+  const size_t npos = ((size_t)c.grid0 * c.grid0 + 1) * d, o_pos = reserve(npos * 4);
   struct Off { size_t qkv_w, proj_w, fc1_w, fc2_w, ln1_w, ln1_b, ln2_w, ln2_b, qkv_b, proj_b, fc1_b, fc2_b; };
   std::vector<Off> bo(c.depth);
   for (int l = 0; l < c.depth; ++l) {
@@ -399,6 +605,9 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
   if ((rc = cvt(w->patch_w, o_patch_w, d * Kp, d))) return rc;
   if ((rc = cpy(w->patch_b, o_patch_b, d))) return rc;
   if ((rc = cpy(w->cls_token, o_cls, d))) return rc;
+  DSS_REQUIRE(w->pos_embed, "vit_load_weights: null pos_embed");
+  if ((rc = cpy(w->pos_embed, o_pos, npos))) return rc;
+  h->pos_dev = reinterpret_cast<float*>(base + o_pos);
   h->patch_w = reinterpret_cast<__half*>(base + o_patch_w);
   h->patch_b = reinterpret_cast<float*>(base + o_patch_b);
   h->cls = reinterpret_cast<float*>(base + o_cls);
@@ -444,9 +653,7 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     if ((rc = make_tmap_f16(&b.tm_fc2, b.fc2_w, (int)d, khid, gemm_tile_n() / 2))) return rc;
   }
   // host copy of the positional grid for interpolation; drop stale interpolations
-  const size_t npos = ((size_t)c.grid0 * c.grid0 + 1) * d;
   h->pos_host.resize(npos);
-  DSS_REQUIRE(w->pos_embed, "vit_load_weights: null pos_embed");
   DSS_CHECK_CUDA(cudaMemcpyAsync(h->pos_host.data(), w->pos_embed, npos * 4, cudaMemcpyDeviceToHost, st));
   DSS_CHECK_CUDA(cudaStreamSynchronize(st));
   for (auto& kv : h->pos_cache) cudaFree(kv.second);
@@ -458,14 +665,16 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
 
 extern "C" size_t dss_vit_workspace_bytes(const dss_vit_t* h, int B, int H, int W) {
   if (!h || B <= 0 || H < h->cfg.patch || W < h->cfg.patch) return 0;
-  return carve(h->cfg, B, H / h->cfg.patch, W / h->cfg.patch, nullptr, h->precision).total;
+  const size_t Np = (size_t)(H / h->cfg.patch) * (W / h->cfg.patch);
+  return carve(h->cfg, (size_t)B * Np, (size_t)B * (Np + 1), nullptr, h->precision).total;
 }
 
 extern "C" size_t dss_vit_forward_last_workspace_bytes(const dss_vit_t* h, int B, int H, int W, int pad) {
   if (!h || B <= 0 || H <= 0 || W <= 0) return 0;
   const int P = h->cfg.patch;
   if (!pad) return dss_vit_workspace_bytes(h, B, H, W);
-  return carve(h->cfg, B, cdiv(H, P), cdiv(W, P), nullptr, h->precision).total;
+  const size_t Np = (size_t)cdiv(H, P) * cdiv(W, P);
+  return carve(h->cfg, (size_t)B * Np, (size_t)B * (Np + 1), nullptr, h->precision).total;
 }
 
 extern "C" int dss_vit_forward_last(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, int pad, int which,
@@ -500,6 +709,43 @@ extern "C" int dss_vit_forward_cls(dss_vit_t* h, const uint8_t* images_u8, int B
   DSS_REQUIRE(h, "vit_forward_cls: null handle");
   return vit_run(h, images_u8, B, H, W, h->cfg.depth, 2, cls_out, ws, ws_bytes, static_cast<cudaStream_t>(stream));
 }
+
+extern "C" size_t dss_vit_ragged_workspace_bytes(const dss_vit_t* h, const int* dims_host, int B, int mode) {
+  RaggedPlan pl;
+  return ragged_plan(h, dims_host, B, mode, false, pl) == DSS_OK ? pl.total : 0;
+}
+
+extern "C" int dss_vit_forward_k_ragged(dss_vit_t* h, const uint8_t* images_u8, const int* dims_host, int B,
+                                        int which_block, float* k_out, void* ws, size_t ws_bytes, dss_stream_t stream) {
+  DSS_REQUIRE(h, "vit_forward_k_ragged: null handle");
+  const int depth = h->cfg.depth;
+  DSS_REQUIRE(which_block >= -depth && which_block < depth, "vit_forward_k_ragged: which_block %d out of range",
+              which_block);
+  const int blk = which_block < 0 ? which_block + depth : which_block;
+  return vit_ragged(h, images_u8, dims_host, B, blk, 0, k_out, ws, ws_bytes, static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int dss_vit_forward_cls_ragged(dss_vit_t* h, const uint8_t* images_u8, const int* dims_host, int B,
+                                          float* cls_out, void* ws, size_t ws_bytes, dss_stream_t stream) {
+  DSS_REQUIRE(h, "vit_forward_cls_ragged: null handle");
+  return vit_ragged(h, images_u8, dims_host, B, h->cfg.depth, 2, cls_out, ws, ws_bytes,
+                    static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int dss_vit_pos_embed_ragged(dss_vit_t* h, const int* dims_host, int B, int mode, float* pos_out, void* ws,
+                                         size_t ws_bytes, dss_stream_t stream) {
+  DSS_REQUIRE(h && pos_out, "vit_pos_embed_ragged: null pointer");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RaggedPlan pl;
+  Ragged rg;
+  int rc = ragged_setup(h, dims_host, B, mode, ws, ws_bytes, st, pl, rg);
+  if (rc) return rc;
+  DSS_CHECK_CUDA(cudaMemcpyAsync(pos_out, rg.pos_all, (size_t)pl.M * h->cfg.dim * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, st));
+  return DSS_OK;
+}
+
+extern "C" int dss_vit_pos_cache_entries(const dss_vit_t* h) { return h ? (int)h->pos_cache.size() : -1; }
 
 extern "C" int dss_vit_pos_embed(dss_vit_t* h, int Hp, int Wp, float* out, dss_stream_t stream) {
   DSS_REQUIRE(h && h->loaded && out, "vit_pos_embed: handle not loaded / null out");

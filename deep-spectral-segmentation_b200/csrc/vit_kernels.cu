@@ -105,6 +105,76 @@ __global__ void im2col_split_kernel(const uint8_t* __restrict__ img, __half* __r
   store_split(out + patch * 3 * Kp + col, Kp, 0, v);
 }
 
+// im2col of a ragged batch (vit.cu): imgs[b] gives image b's pixel offset, size, patch grid and first patch row.
+// One thread = 8 consecutive pixels of one patch row, all three channels (the values and stores of im2col_f16_kernel,
+// patch-major thread order); the split form writes one patch element per thread as im2col_split_kernel does.
+template <bool SPLIT>
+__global__ void im2col_ragged_kernel(const uint8_t* __restrict__ img, __half* __restrict__ out,
+                                     const RaggedImage* __restrict__ imgs, int B, long long n_patches, int P) {
+  const int Kp = 3 * P * P, per_patch = SPLIT ? Kp : P * (P / 8);
+  const long long gid = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (gid >= n_patches * per_patch) return;
+  const long long gp = gid / per_patch;                     // patch row of the packed batch
+  const int r = (int)(gid % per_patch);
+  const int b = ragged_find(B, gp, [&](int i) { return imgs[i].patch_off; });
+  const RaggedImage im = imgs[b];
+  const int n = (int)(gp - im.patch_off), ph = n / im.Wp, pw = n % im.Wp;
+  if constexpr (SPLIT) {
+    const int c = r / (P * P), py = (r / P) % P, px = r % P;
+    const float v = pixel_value(img[(im.px_off + (long long)(ph * P + py) * im.W + pw * P + px) * 3 + c], c);
+    store_split(out + gp * 3 * Kp + r, Kp, 0, v);
+  } else {
+    const int py = r / (P / 8), px0 = (r % (P / 8)) * 8;
+    const uint8_t* src = img + (im.px_off + (long long)(ph * P + py) * im.W + pw * P + px0) * 3;
+    uint8_t raw[24];
+#pragma unroll
+    for (int i = 0; i < 24; ++i) raw[i] = __ldg(src + i);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      uint4 q;
+      q.x = pack_half2(pixel_value(raw[0 * 3 + c], c), pixel_value(raw[1 * 3 + c], c));
+      q.y = pack_half2(pixel_value(raw[2 * 3 + c], c), pixel_value(raw[3 * 3 + c], c));
+      q.z = pack_half2(pixel_value(raw[4 * 3 + c], c), pixel_value(raw[5 * 3 + c], c));
+      q.w = pack_half2(pixel_value(raw[6 * 3 + c], c), pixel_value(raw[7 * 3 + c], c));
+      *reinterpret_cast<uint4*>(out + gp * Kp + (c * P + py) * P + px0) = q;
+    }
+  }
+}
+
+// Positional tables of a ragged batch: pos_all [M, d] laid out like the residual stream, image b's rows at tok_off its
+// [T_b, d] table. The bicubic resampling of interp_pos_host (vit.cu) with the same per-axis indices and fp32 weights
+// (computed on the host), the same tap order and every product and sum rounded on its own (no contraction), so the
+// tables are the host routine's bits; the CLS row and, under the identity rule, the whole grid are copied.
+__global__ void pos_ragged_kernel(const float* __restrict__ src, int g, int d, const RaggedImage* __restrict__ imgs, int B,
+                                  long long M, const int* __restrict__ axis_idx, const float* __restrict__ axis_w,
+                                  float* __restrict__ pos_all) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= M * d) return;
+  const long long row = i / d;
+  const int c = (int)(i % d);
+  const int b = ragged_find(B, row, [&](int j) { return imgs[j].tok_off; });
+  const RaggedImage im = imgs[b];
+  const int t = (int)(row - im.tok_off);
+  if (t == 0 || im.stored) {
+    pos_all[i] = src[(long long)t * d + c];
+    return;
+  }
+  const int y = (t - 1) / im.Wp, x = (t - 1) % im.Wp;
+  const int ay = im.axis_off + y, ax = im.axis_off + im.Hp + x;
+  float o = 0.f;
+#pragma unroll
+  for (int a = 0; a < 4; ++a) {
+    const int sy = min(max(axis_idx[ay] - 1 + a, 0), g - 1);
+#pragma unroll
+    for (int bb = 0; bb < 4; ++bb) {
+      const int sx = min(max(axis_idx[ax] - 1 + bb, 0), g - 1);
+      const float wgt = __fmul_rn(axis_w[4 * ay + a], axis_w[4 * ax + bb]);
+      o = __fadd_rn(o, __fmul_rn(wgt, src[((long long)(sy * g + sx) + 1) * d + c]));
+    }
+  }
+  pos_all[i] = o;
+}
+
 // x[b, 0, :] = cls + pos[0, :]
 __global__ void cls_row_kernel(float* __restrict__ x, const float* __restrict__ cls, const float* __restrict__ pos,
                                int B, int T, int d) {
@@ -112,6 +182,15 @@ __global__ void cls_row_kernel(float* __restrict__ x, const float* __restrict__ 
   if (i >= B * d) return;
   const int b = i / d, c = i % d;
   x[(long long)b * T * d + c] = cls[c] + pos[c];
+}
+
+// ragged: x[tok_off_b, :] = cls + pos_all[tok_off_b, :]
+__global__ void cls_row_ragged_kernel(float* __restrict__ x, const float* __restrict__ cls, const float* __restrict__ pos,
+                                      const RaggedImage* __restrict__ imgs, int B, int d) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B * d) return;
+  const long long r = (long long)imgs[i / d].tok_off * d + i % d;
+  x[r] = cls[i % d] + pos[r];
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -264,6 +343,36 @@ int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P,
 int launch_cls_row(float* x, const float* cls, const float* pos, int B, int T, int d, cudaStream_t st) {
   LaunchScope scope(st, KC_CLS_ROW);
   cls_row_kernel<<<cdiv(B * d, 256), 256, 0, st>>>(x, cls, pos, B, T, d);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
+int launch_im2col_ragged(const uint8_t* img, void* patches, const RaggedImage* imgs, int B, long long n_patches, int P,
+                         bool split, cudaStream_t st) {
+  DSS_REQUIRE(img && patches && imgs && B > 0 && n_patches > 0, "im2col_ragged: bad arguments");
+  DSS_REQUIRE(P > 0 && P % 8 == 0, "im2col_ragged: patch must be a multiple of 8 (got %d)", P);
+  __half* out = reinterpret_cast<__half*>(patches);
+  LaunchScope scope(st, KC_IM2COL);
+  if (split)
+    im2col_ragged_kernel<true><<<grid_for(n_patches * 3 * P * P, 256), 256, 0, st>>>(img, out, imgs, B, n_patches, P);
+  else
+    im2col_ragged_kernel<false><<<grid_for(n_patches * P * (P / 8), 256), 256, 0, st>>>(img, out, imgs, B, n_patches, P);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
+int launch_pos_ragged(const float* pos_src, int grid0, int d, const RaggedImage* imgs, int B, long long M,
+                      const int* axis_idx, const float* axis_w, float* pos_all, cudaStream_t st) {
+  LaunchScope scope(st, KC_CLS_ROW);
+  pos_ragged_kernel<<<grid_for(M * d, 256), 256, 0, st>>>(pos_src, grid0, d, imgs, B, M, axis_idx, axis_w, pos_all);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
+int launch_cls_row_ragged(float* x, const float* cls, const float* pos_all, const RaggedImage* imgs, int B, int d,
+                          cudaStream_t st) {
+  LaunchScope scope(st, KC_CLS_ROW);
+  cls_row_ragged_kernel<<<cdiv(B * d, 256), 256, 0, st>>>(x, cls, pos_all, imgs, B, d);
   DSS_CHECK_CUDA(cudaGetLastError());
   return DSS_OK;
 }

@@ -81,6 +81,18 @@ def _eigs_items(output_dir, image_ids, which_matrix="laplacian", skip=()):
             for j, image_id in enumerate(image_ids) if j not in skip]
 
 
+def _feature_items_ragged(output_dir, items, rows, model_name, patch_size):
+    """Writer items for the feature dicts of one ragged batch: image j = (image, file, index) has the k rows
+    rows[j] = (r0, r1) of arrays['k'], saved as [1, N, d] like _feature_items."""
+    out = []
+    for (image, file, index), (r0, r1) in zip(items, rows):
+        H, W = int(image.shape[0]), int(image.shape[1])
+        extra = {"file": file, "id": Path(file).stem, "model_name": model_name, "patch_size": patch_size, "shape": (1, 3, H, W)}
+        out.append((str(Path(output_dir) / f"{Path(file).stem}.pth"), r0, extra,
+                    {"k": ("rows1", ("k", r1 - r0)), "indices": ("tensor0d", index)}))
+    return out
+
+
 class _Batcher:
     """Groups items by a shape key. A group is handed to ``flush`` when it reaches ``batch_size``; when more than
     ``max_pending`` items are waiting in total (data sets with hundreds of distinct image sizes, e.g. VOC), the
@@ -139,20 +151,17 @@ def extract_features(images_list: str, images_root: Optional[str], model_name: s
     filenames = Path(images_list).read_text().splitlines()
     dataset = utils.ImagesDataset(filenames=filenames, images_root=images_root)
     print(f"Dataset size: {len(dataset)=}")
-    rings: Dict[tuple, io_pipeline.PinnedRing] = {}
+    # batch_size images per forward in list order, whatever their sizes: one ragged ViT forward per batch
+    ring = io_pipeline.PackedRing(dev)
+    batch_size = max(1, int(batch_size))
 
     with io_pipeline.make_writer(writer, num_workers_out) as wr:
-        def flush(shape_key, items):
-            H, W = shape_key
-            ring = rings.get(shape_key)
-            if ring is None:
-                ring = rings[shape_key] = io_pipeline.PinnedRing(shape_key, max(1, int(batch_size)), dev)
-            slot, host = ring.stage([it[0] for it in items])
-            k = model.forward_k(ring.to_device(slot, host), which_block=which_block).cpu()
-            wr.submit_batch({"k": k.numpy()}, _feature_items(output_dir, [(it[1], it[2]) for it in items], model_name,
-                                                             patch_size, H, W))
+        def flush(items):
+            slot, host, dims = ring.stage([it[0] for it in items])
+            k, rows = model.forward_k_ragged(ring.to_device(slot, host), dims, which_block=which_block)
+            wr.submit_batch({"k": k.cpu().numpy()}, _feature_items_ragged(output_dir, items, rows, model_name, patch_size))
 
-        batcher = _Batcher(batch_size, flush)
+        batch = []
         todo = []
         for i in _my_share(list(range(len(dataset)))):
             output_file = Path(output_dir) / f"{Path(dataset.filenames[i]).stem}.pth"
@@ -161,8 +170,12 @@ def extract_features(images_list: str, images_root: Optional[str], model_name: s
             else:
                 todo.append(i)
         for image, file, index in io_pipeline.ImagePrefetcher(dataset.__getitem__, todo, num_workers):
-            batcher.add((int(image.shape[0]), int(image.shape[1])), (image, file, index))
-        batcher.finish()
+            batch.append((image, file, index))
+            if len(batch) == batch_size:
+                flush(batch)
+                batch = []
+        if batch:
+            flush(batch)
     print(f"Saved features to {output_dir}")
 
 
@@ -483,7 +496,8 @@ def extract_bbox_features(images_root: str, bbox_file: str, model_name: str, out
                           batch_size: int = 64, precision: str = "fp16"):
     """
     DINO CLS embedding of every bounding-box crop (reference extract/extract.py:500-544), same command / file
-    contract: each dict of ``bbox_file`` gains 'features' [n_boxes, d] fp32. Crops of equal size are batched.
+    contract: each dict of ``bbox_file`` gains 'features' [n_boxes, d] fp32. ``batch_size`` crops per ViT forward in
+    (image, box) order, whatever their sizes (one ragged forward per batch).
     ``precision``: ViT arithmetic, as in extract_features.
 
     Example:
@@ -503,13 +517,15 @@ def extract_bbox_features(images_root: str, bbox_file: str, model_name: str, out
                                               random_init=random_init, precision=precision)
     feats: Dict[Tuple[int, int], torch.Tensor] = {}   # (image row, box row) -> [d]
 
-    def flush(shape_key, items):
-        batch = torch.stack([it[0] for it in items]).to(dev)
-        cls = model.forward_cls(batch).cpu()
+    def flush(items):
+        packed, dims = vit_mod.pack_images([it[0] for it in items])
+        cls, _ = model.forward_cls_ragged(packed.to(dev), dims)
+        cls = cls.cpu()
         for j, (_, where) in enumerate(items):
             feats[where] = cls[j].clone()
 
-    batcher = _Batcher(batch_size, flush)
+    batch_size = max(1, int(batch_size))
+    batch = []
     for bi, bbox_dict in enumerate(bbox_list):
         image_filename = str(Path(images_root) / f"{bbox_dict['id']}.jpg")
         image = torch.from_numpy(np.ascontiguousarray(np.asarray(Image.open(image_filename).convert("RGB"))))
@@ -517,8 +533,12 @@ def extract_bbox_features(images_root: str, bbox_file: str, model_name: str, out
             crop = image[ymin:ymax, xmin:xmax].contiguous()          # image[:, :, ymin:ymax, xmin:xmax] at :539
             if crop.shape[0] < patch_size or crop.shape[1] < patch_size:
                 raise ValueError(f"{bbox_dict['id']}: box {(xmin, ymin, xmax, ymax)} is smaller than one patch")
-            batcher.add((int(crop.shape[0]), int(crop.shape[1])), (crop, (bi, ji)))
-    batcher.finish()
+            batch.append((crop, (bi, ji)))
+            if len(batch) == batch_size:
+                flush(batch)
+                batch = []
+    if batch:
+        flush(batch)
     for bi, bbox_dict in enumerate(bbox_list):
         bbox_dict["features"] = torch.stack([feats[(bi, ji)] for ji in range(len(bbox_dict["bboxes"]))], dim=0)
     torch.save(bbox_list, output_file)

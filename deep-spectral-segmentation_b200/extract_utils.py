@@ -32,7 +32,7 @@ def read_image_rgb(path) -> np.ndarray:
 
 def read_image_raw(path):
     """First half of read_image_rgb: (pixels, is_bgr). The colour swap is left to the caller so that it can write the
-    RGB image straight into a page-locked batch row (io_pipeline.PinnedRing.convert_async) instead of into a temporary
+    RGB image straight into a page-locked batch row (io_pipeline.BatchAssembler) instead of into a temporary
     that is then copied."""
     try:
         import cv2

@@ -4,8 +4,8 @@
 
   * ``ImagePrefetcher``  decodes JPEG/PNG files on a thread pool (cv2 / PIL release the GIL while decoding) with a
                           bounded look-ahead, yielding items in order;
-  * ``PinnedRing``       stages equally shaped uint8 images into a small ring of page-locked batches so that the
-                          host->device copy is asynchronous and the decoder never waits for the GPU;
+  * ``PackedRing``       stages uint8 images of any sizes, packed one after another, into a small ring of page-locked
+                          buffers so that the host->device copy is asynchronous and the decoder never waits for the GPU;
   * ``BatchAssembler``   the two steps above in one: decode threads colour-swap each image straight into a row of a
                           page-locked batch of its shape and hand over completed batches (used by extract_all);
   * ``AsyncWriter``      runs ``torch.save`` (same dict layouts, so ``torch.load`` consumers are unaffected) on writer
@@ -14,7 +14,7 @@
                           Python per file, and writer threads would take the interpreter lock away from the thread that
                           feeds the GPU.
 
-Pure host code: nothing here touches the device except ``PinnedRing.to_device``'s copy."""
+Pure host code: nothing here touches the device except ``PackedRing.to_device``'s copy."""
 from __future__ import annotations
 
 import os
@@ -118,81 +118,53 @@ class ImagePrefetcher:
                     f.cancel()
 
 
-class PinnedRing:
-    """Ring of page-locked uint8 batches [slots][capacity, H, W, 3] for one image shape. ``stage`` copies decoded images
-    into the next slot (host memcpy), ``to_device`` starts the asynchronous H2D copy and returns the device batch; a
-    slot is reused only after the copy that read it has completed (tracked with a CUDA event)."""
+class PackedRing:
+    """Ring of page-locked uint8 buffers that each hold one batch of images of ANY sizes packed one after another
+    ([sum H*W, 3], the input layout of the ragged ViT forwards). ``stage`` copies decoded images into the next slot
+    (host memcpy; a slot grows when a batch does not fit) and returns the packed view and the dims [B, 2];
+    ``to_device`` starts the asynchronous H2D copy and returns the device batch. A slot is reused only after the copy
+    that read it has completed (tracked with a CUDA event)."""
 
-    def __init__(self, shape: Tuple[int, int], capacity: int, device, slots: int = 2, copy_threads: int = 8):
-        H, W = shape
+    def __init__(self, device, slots: int = 2, copy_threads: int = 8):
         self.device = device
-        self.capacity = capacity
-        # torch.empty(pin_memory=True) allocates page-locked memory directly (no pageable copy first)
-        self.bufs = [torch.empty(capacity, H, W, 3, dtype=torch.uint8, pin_memory=True) for _ in range(slots)]
-        self.np_bufs = [b.numpy() for b in self.bufs]    # views of the page-locked memory
+        self.bufs: List[Optional[torch.Tensor]] = [None] * slots
         self.events: List[Optional[torch.cuda.Event]] = [None] * slots
         self.next = 0
         copy_threads = int(os.environ.get("DSS_IO_COPY_THREADS", copy_threads))
         self.copy_threads = copy_threads
         self._pool = ThreadPoolExecutor(copy_threads, thread_name_prefix="dss-stage") if copy_threads > 1 else None
 
-    def stage(self, images: Sequence[torch.Tensor]) -> Tuple[int, torch.Tensor]:
+    def stage(self, images: Sequence[torch.Tensor]) -> Tuple[int, torch.Tensor, torch.Tensor]:
+        import numpy as np
         slot = self.next
         self.next = (self.next + 1) % len(self.bufs)
         if self.events[slot] is not None:
             self.events[slot].synchronize()
-        buf = self.bufs[slot][:len(images)]
-        import numpy as np
-        dst = self.np_bufs[slot]
+        dims = torch.tensor([[int(im.shape[0]), int(im.shape[1])] for im in images], dtype=torch.int32)
+        sizes = [int(h) * int(w) for h, w in dims.tolist()]
+        total = sum(sizes)
+        if self.bufs[slot] is None or self.bufs[slot].shape[0] < total:
+            # torch.empty(pin_memory=True) allocates page-locked memory directly (no pageable copy first)
+            self.bufs[slot] = torch.empty(total, 3, dtype=torch.uint8, pin_memory=True)
+        buf = self.bufs[slot][:total]
+        dst = buf.numpy()
+        offs = np.cumsum([0] + sizes)
+
+        def copy(j):
+            np.copyto(dst[offs[j]:offs[j + 1]], images[j].numpy().reshape(-1, 3))
         # numpy's copy loop releases the interpreter lock (torch's Tensor.copy_ on CPU tensors does not), so a few threads
         # copy in parallel
         if self._pool is None or len(images) < 2 * self.copy_threads:
-            for j, im in enumerate(images):
-                np.copyto(dst[j], im.numpy())
+            for j in range(len(images)):
+                copy(j)
         else:
             n = self.copy_threads
 
             def part(t):
                 for j in range(t, len(images), n):
-                    np.copyto(dst[j], images[j].numpy())
+                    copy(j)
             list(self._pool.map(part, range(n)))
-        return slot, buf
-
-    # ---- incremental staging: the caller assigns (slot, row) as images arrive and the copies run on the pool while it
-    # keeps pulling decoded images; the batch is complete when its futures are
-    def begin(self) -> int:
-        slot = self.next
-        self.next = (self.next + 1) % len(self.bufs)
-        if self.events[slot] is not None:
-            self.events[slot].synchronize()
-        return slot
-
-    def copy_async(self, slot: int, j: int, image: torch.Tensor):
-        import numpy as np
-        dst, src = self.np_bufs[slot][j], image.numpy()
-        if self._pool is None:
-            np.copyto(dst, src)
-            return None
-        return self._pool.submit(np.copyto, dst, src)
-
-    def convert_async(self, slot: int, j: int, pixels, is_bgr: bool):
-        """Like copy_async for a freshly decoded numpy image: a BGR image (cv2.imread) is colour-swapped DIRECTLY into
-        row j of the page-locked batch (one pass over the pixels instead of swap-into-a-temporary + copy)."""
-        import numpy as np
-        dst = self.np_bufs[slot][j]
-
-        def work():
-            if is_bgr:
-                import cv2
-                out = cv2.cvtColor(pixels, cv2.COLOR_BGR2RGB, dst=dst)
-                if out is not dst and not np.shares_memory(out, dst):   # cv2 reallocates when dst does not fit
-                    np.copyto(dst, out)
-            else:
-                np.copyto(dst, pixels)
-        if self._pool is None:
-            work()
-            return None
-        return self._pool.submit(work)
+        return slot, buf, dims
 
     def to_device(self, slot: int, host_batch: torch.Tensor) -> torch.Tensor:
         dev = host_batch.to(self.device, non_blocking=True)
@@ -453,6 +425,9 @@ def _materialise(arrays, j, extra, fields):
             obj[key] = torch.from_numpy(np.array(arrays[val][j]))
         elif how == "slice1":         # tensor arrays[val][j:j+1] (keeps the leading batch dimension of 1)
             obj[key] = torch.from_numpy(np.array(arrays[val][j:j + 1]))
+        elif how == "rows1":          # tensor arrays[name][j:j+n] as [1, n, ...] (val = (name, n))
+            name, n = val
+            obj[key] = torch.from_numpy(np.array(arrays[name][j:j + n]).reshape(1, n, *arrays[name].shape[1:]))
         elif how == "np_slice":       # numpy array arrays[val][j]
             obj[key] = np.array(arrays[val][j])
         elif how == "tensor0d":       # 0-d int64 tensor
@@ -460,6 +435,12 @@ def _materialise(arrays, j, extra, fields):
         else:
             raise ValueError(how)
     return obj
+
+
+def _row_end(item) -> int:
+    """One past the last array row a writer item reads: j + 1, or j + n for a ("rows1", (name, n)) field."""
+    _, j, _, fields = item
+    return j + max([val[1] for how, val in fields.values() if how == "rows1"] or [1])
 
 
 def _writer_process_main(q, errq, doneq):
@@ -488,7 +469,8 @@ def _writer_process_main(q, errq, doneq):
 class ProcessWriter:
     """Writer processes for the per-image .pth files. ``submit_batch(arrays, items)``: ``arrays`` maps names to numpy
     arrays with a leading batch dimension (sent once per batch), ``items`` is a list of (path, row j, extra dict, fields)
-    where fields maps dict keys to ("slice" | "slice1" | "np_slice", array name) or ("tensor0d", int); the worker builds
+    where fields maps dict keys to ("slice" | "slice1" | "np_slice", array name), ("rows1", (array name, rows)) or
+    ("tensor0d", int); the worker builds
     each dict and torch.saves it. Started with the 'spawn' method (no fork of a process that holds a CUDA context and
     running threads). Importing torch in the children takes a second or two, so the pool is PERSISTENT: make_writer()
     hands out the same processes to every command of this interpreter; ``close()`` only waits until everything that
@@ -517,13 +499,13 @@ class ProcessWriter:
         self._check()
         n = len(self.procs)
         # split the batch over the writers in contiguous row ranges; each message carries only its rows of the arrays
-        rows = sorted(it_[1] for it_ in items)
-        per = -(-len(rows) // n)
+        spans = sorted((it_[1], _row_end(it_)) for it_ in items)
+        per = -(-len(spans) // n)
         for w in range(n):
-            sel = rows[w * per:(w + 1) * per]
+            sel = spans[w * per:(w + 1) * per]
             if not sel:
                 continue
-            lo, hi = sel[0], sel[-1] + 1
+            lo, hi = sel[0][0], max(end for _, end in sel)
             part = [(path, j - lo, extra, fields) for path, j, extra, fields in items if lo <= j < hi]
             self.q.put(({name: a[lo:hi] for name, a in arrays.items()}, part))
             self.submitted += len(part)

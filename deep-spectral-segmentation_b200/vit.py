@@ -7,7 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
-from typing import Dict, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
 
@@ -214,11 +214,85 @@ class DinoViT:
                                                      _lib.stream_ptr(self.device)), "dss_vit_forward_last")
         return f, a
 
+    def _ragged_args(self, images, dims):
+        """(packed uint8 [sum H W, 3] CUDA tensor, host int32 dims [B, 2]) from a list of [H, W, 3] images or a packed
+        tensor plus dims."""
+        if dims is None:
+            packed, dims = pack_images(images)
+        else:
+            packed, dims = images, torch.as_tensor(dims, dtype=torch.int32).reshape(-1, 2).contiguous()
+        _lib.require_cuda(packed, "images")
+        if packed.dtype != torch.uint8 or packed.shape[-1] != 3 or packed.numel() != 3 * int((dims[:, 0].long() * dims[:, 1].long()).sum()):
+            raise _lib.DssError("ragged images must be uint8 RGB, packed [sum H*W, 3] as dims describes")
+        return packed.contiguous(), dims
+
+    def _ragged_workspace(self, dims: torch.Tensor, mode: int) -> torch.Tensor:
+        need = int(self.lib.dss_vit_ragged_workspace_bytes(self._h, dims.data_ptr(), dims.shape[0], mode))
+        if need == 0:
+            # the entry point names the offending image
+            _lib.check(_lib.DSS_ERR_BAD_ARG, "dss_vit_ragged_workspace_bytes")
+        if self._ws is None or self._ws.numel() < need:
+            self._ws = torch.empty(need, dtype=torch.uint8, device=self.device)
+        return self._ws
+
+    @torch.no_grad()
+    def forward_k_ragged(self, images, dims=None, which_block: int = -1):
+        """forward_k over images of different sizes in one forward. ``images``: a list of uint8 [H, W, 3] CUDA tensors,
+        or a packed uint8 [sum H*W, 3] tensor with ``dims`` [B, 2] = (H, W) per image. Returns (k [sum N_b, d] fp32,
+        rows): image b's features are k[rows[b][0]:rows[b][1]], the bits forward_k gives for that image alone."""
+        packed, dims = self._ragged_args(images, dims)
+        B, P = dims.shape[0], self.patch_size
+        rows = ragged_rows(dims.tolist(), P)
+        with torch.cuda.device(self.device):
+            ws = self._ragged_workspace(dims, _lib.VIT_RAGGED_K)
+            out = torch.empty(rows[-1][1] if rows else 0, self.dim, dtype=torch.float32, device=self.device)
+            _lib.check(self.lib.dss_vit_forward_k_ragged(self._h, packed.data_ptr(), dims.data_ptr(), B, which_block,
+                                                         out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                         _lib.stream_ptr(self.device)), "dss_vit_forward_k_ragged")
+        return out, rows
+
+    @torch.no_grad()
+    def forward_cls_ragged(self, images, dims=None):
+        """forward_cls over images of different sizes in one forward (arguments as forward_k_ragged). Returns
+        (cls [B, d] fp32, rows) with rows[b] = (b, b + 1)."""
+        packed, dims = self._ragged_args(images, dims)
+        B = dims.shape[0]
+        with torch.cuda.device(self.device):
+            ws = self._ragged_workspace(dims, _lib.VIT_RAGGED_CLS)
+            out = torch.empty(B, self.dim, dtype=torch.float32, device=self.device)
+            _lib.check(self.lib.dss_vit_forward_cls_ragged(self._h, packed.data_ptr(), dims.data_ptr(), B,
+                                                           out.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                           _lib.stream_ptr(self.device)), "dss_vit_forward_cls_ragged")
+        return out, [(b, b + 1) for b in range(B)]
+
     def pos_embed(self, Hp: int, Wp: int) -> torch.Tensor:
         with torch.cuda.device(self.device):
             out = torch.empty(Hp * Wp + 1, self.dim, dtype=torch.float32, device=self.device)
             _lib.check(self.lib.dss_vit_pos_embed(self._h, Hp, Wp, out.data_ptr(), _lib.stream_ptr(self.device)))
         return out
+
+
+def pack_images(images) -> Tuple[torch.Tensor, torch.Tensor]:
+    """A list of uint8 [H, W, 3] images -> (packed [sum H*W, 3], host int32 dims [B, 2]), images one after another:
+    the input layout of the ragged forwards."""
+    if len(images) == 0:
+        raise _lib.DssError("a ragged batch needs at least one image")
+    for im in images:
+        if im.dtype != torch.uint8 or im.dim() != 3 or im.shape[-1] != 3:
+            raise _lib.DssError("ragged images must be uint8 [H, W, 3]")
+    dims = torch.tensor([[int(im.shape[0]), int(im.shape[1])] for im in images], dtype=torch.int32)
+    return torch.cat([im.reshape(-1, 3) for im in images]), dims
+
+
+def ragged_rows(dims, patch_size: int) -> List[Tuple[int, int]]:
+    """Row range (start, end) of each image's features in forward_k_ragged's packed output: N_b = (H_b // P)(W_b // P)
+    rows per image, image after image."""
+    rows, r = [], 0
+    for H, W in dims:
+        n = (int(H) // patch_size) * (int(W) // patch_size)
+        rows.append((r, r + n))
+        r += n
+    return rows
 
 
 def pos_embed_interp_host(pos_embed: torch.Tensor, grid0: int, Hp: int, Wp: int) -> torch.Tensor:

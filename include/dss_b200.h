@@ -123,6 +123,32 @@ int dss_vit_forward_tokens(dss_vit_t* h, const uint8_t* images_u8, int B, int H,
 int dss_vit_forward_cls(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, float* cls_out, void* ws,
                         size_t ws_bytes, dss_stream_t stream);
 
+/* Ragged batches: B images of any sizes in one forward, each treated exactly as the uniform call treats it alone
+ * (the crop to patch multiples, its positional grid and the identity rule of interpolate_pos_encoding: pixel H == W for
+ * _cls, Hp == Wp for _k), so every image's outputs are the bits of that image run alone.
+ * images_u8 packs the images one after another: [sum H_b W_b, 3] uint8 RGB, image b at byte offset
+ * 3 * sum_{i<b} H_i W_i; dims_host [B, 2] = {H_b, W_b} (host memory). Outputs are packed the same way:
+ * k_out [sum N_b, d] fp32 (image b's N_b = (H_b/P)(W_b/P) rows follow image b-1's), cls_out [B, d] fp32.
+ * Workspace: dss_vit_ragged_workspace_bytes(h, dims_host, B, mode) with mode DSS_VIT_RAGGED_K or DSS_VIT_RAGGED_CLS
+ * (0 for a bad batch), 256-byte aligned. Checked on the host before any device work: null pointers, B <= 0, negative
+ * sizes, an image smaller than one patch (the message names the image) and a small or misaligned workspace are
+ * DSS_ERR_BAD_ARG; a batch whose token rows exceed the tensor-map extents (2^31) is DSS_ERR_UNSUPPORTED. The
+ * positional tables are computed on the device per call (the bits of dss_pos_embed_interp_host); the handle's
+ * positional cache is neither read nor written. Both precision modes. */
+enum { DSS_VIT_RAGGED_K = 0, DSS_VIT_RAGGED_CLS = 1 };
+size_t dss_vit_ragged_workspace_bytes(const dss_vit_t* h, const int* dims_host, int B, int mode);
+int dss_vit_forward_k_ragged(dss_vit_t* h, const uint8_t* images_u8, const int* dims_host, int B, int which_block,
+                             float* k_out, void* ws, size_t ws_bytes, dss_stream_t stream);
+int dss_vit_forward_cls_ragged(dss_vit_t* h, const uint8_t* images_u8, const int* dims_host, int B, float* cls_out,
+                               void* ws, size_t ws_bytes, dss_stream_t stream);
+
+/* The positional tables a ragged forward adds (mode DSS_VIT_RAGGED_*): pos_out [sum T_b, d] fp32 (device), image b's
+ * [T_b, d] table at its token rows. Same arguments and workspace as the forwards. */
+int dss_vit_pos_embed_ragged(dss_vit_t* h, const int* dims_host, int B, int mode, float* pos_out, void* ws,
+                             size_t ws_bytes, dss_stream_t stream);
+/* Number of patch grids in the handle's positional cache (the uniform calls fill it, at most 64; -1 for NULL). */
+int dss_vit_pos_cache_entries(const dss_vit_t* h);
+
 /* Interpolated positional embedding [T, d] fp32 for an (Hp x Wp) patch grid, as upstream
  * VisionTransformer.interpolate_pos_encoding computes it (bicubic, scale (Hp+0.1)/grid0). Copied to out (device). */
 int dss_vit_pos_embed(dss_vit_t* h, int Hp, int Wp, float* out, dss_stream_t stream);
