@@ -55,8 +55,6 @@ PROTOTYPES = {
                                          c_void_p]),
     "dss_vit_forward_cls_ragged": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "dss_vit_pos_embed_ragged": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
-    "dss_vit_pos_cache_entries": (c_int, [c_void_p]),
-    "dss_vit_pos_embed": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
     "dss_pos_embed_interp_host": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "dss_op_gemm_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
                                 c_int, c_void_p]),

@@ -97,7 +97,7 @@ extern "C" int dss_profile_read(dss_profile_entry* out, int max_entries) {
 }
 
 extern "C" const char* dss_last_error(void) { return dss::last_error(); }
-extern "C" int dss_version(void) { return 2; }
+extern "C" int dss_version(void) { return 3; }
 extern "C" int dss_device_sm_count(void) {
   const int n = dss::device_sm_count();
   if (n < 0) dss::set_error("no CUDA device available");

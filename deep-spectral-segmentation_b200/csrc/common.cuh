@@ -58,7 +58,6 @@ int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int im
 // ViT kernels (vit_kernels.cu, attention.cu). split: the operand is written in the split-fp16 format of
 // DSS_VIT_PRECISION_FP32 (A order), three groups per value (split_f16 below)
 int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P, int pad, bool split, cudaStream_t st);
-int launch_cls_row(float* x, const float* cls, const float* pos, int B, int T, int d, cudaStream_t st);
 int launch_layernorm(const float* x, const float* g, const float* b, void* y, int M, int d, float eps, bool split,
                      cudaStream_t st);
 // qkv: f16 [B*T, 3d] (f32_keys false) or the fp32 qkv GEMM output of DSS_VIT_PRECISION_FP32 (f32_keys true)
@@ -71,12 +70,11 @@ int launch_attention_split(const void* qkv_split, void* out, int B, int T, int h
 
 // ---- ragged ViT batches: B images of any sizes, packed one after another (vit.cu). Device table entry of image b:
 // its pixels start at pixel px_off of the packed [sum H W, 3] input, its patch rows at patch_off, its T = Hp Wp + 1
-// token rows (CLS first) at tok_off; its positional-interpolation indices and weights at axis_off of the axis tables
-// (Hp y entries, then Wp x entries); stored: the stored positional grid is used unchanged (identity rule).
+// token rows (CLS first) at tok_off; stored: the stored positional grid is used unchanged (identity rule).
 struct RaggedImage {
   long long px_off;
   int H, W, Hp, Wp;
-  int patch_off, tok_off, axis_off, stored;
+  int patch_off, tok_off, stored;
 };
 // the image whose first row off(b) is the last one <= x (off nondecreasing in b, off(0) = 0)
 template <typename Off>
@@ -90,10 +88,6 @@ __device__ __forceinline__ int ragged_find(int B, long long x, Off&& off) {
 }
 int launch_im2col_ragged(const uint8_t* img, void* patches, const RaggedImage* imgs, int B, long long n_patches, int P,
                          bool split, cudaStream_t st);
-int launch_cls_row_ragged(float* x, const float* cls, const float* pos_all, const RaggedImage* imgs, int B, int d,
-                          cudaStream_t st);
-int launch_pos_ragged(const float* pos_src, int grid0, int d, const RaggedImage* imgs, int B, long long M,
-                      const int* axis_idx, const float* axis_w, float* pos_all, cudaStream_t st);
 // tile_prefix [B + 1]: image b's 128-query tiles are CTAs [tile_prefix[b], tile_prefix[b + 1])
 int launch_attention_tc_ragged(const void* qkv, void* out, const RaggedImage* imgs, const int* tile_prefix, int B,
                                long long M, int tiles, int heads, cudaStream_t st);

@@ -16,8 +16,6 @@
 
 #include <algorithm>
 #include <cstring>
-#include <map>
-#include <tuple>
 #include <utility>
 #include <vector>
 
@@ -25,13 +23,36 @@
 
 namespace dss {
 
-// y[b, :] = LayerNorm(x[b * row_stride, :]) * gamma + beta in fp32 (one warp per row): the final norm of the CLS token
+// Where a batch's token rows lie, for the kernels outside attention that see image boundaries (attention.cu has its
+// own tile locators): row0(b) is image b's first (CLS) row of the residual stream, and at(r) names positional-table
+// row r: token t of an image with an Hp x Wp patch grid, stored = the identity rule keeps the stored grid.
+struct PosRow { int t, Hp, Wp, stored; };
+// A uniform batch: image b's T = Hp Wp + 1 rows start at b T; the positional table is the [T, d] one all images share.
+struct UniformRows {
+  int T, Hp, Wp, stored;
+  __device__ __forceinline__ long long row0(int b) const { return (long long)b * T; }
+  __device__ __forceinline__ PosRow at(long long r) const { return {(int)r, Hp, Wp, stored}; }
+};
+// A ragged batch: image b's rows start at imgs[b].tok_off; the positional table is laid out like the residual stream.
+struct RaggedRows {
+  const RaggedImage* imgs;
+  int B;
+  __device__ __forceinline__ long long row0(int b) const { return imgs[b].tok_off; }
+  __device__ __forceinline__ PosRow at(long long r) const {
+    const RaggedImage im = imgs[ragged_find(B, r, [&](int j) { return imgs[j].tok_off; })];
+    return {(int)(r - im.tok_off), im.Hp, im.Wp, im.stored};
+  }
+};
+
+// y[b, :] = LayerNorm(x[row0(b), :]) * gamma + beta in fp32 (one warp per image): the final norm of the CLS token, read
+// where it lies in the residual stream
+template <typename Loc>
 __global__ void __launch_bounds__(128)
-layernorm_rows_f32_kernel(const float* __restrict__ x, long long row_stride, const float* __restrict__ gamma,
+layernorm_rows_f32_kernel(const float* __restrict__ x, Loc loc, const float* __restrict__ gamma,
                           const float* __restrict__ beta, float* __restrict__ y, int rows, int d, float eps) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
   if (row >= rows) return;
-  const float* xr = x + (long long)row * row_stride;
+  const float* xr = x + loc.row0(row) * d;
   float s = 0.f;
   for (int i = lane; i < d; i += 32) s += xr[i];
   const float mean = warp_sum(s) / (float)d;
@@ -39,14 +60,6 @@ layernorm_rows_f32_kernel(const float* __restrict__ x, long long row_stride, con
   for (int i = lane; i < d; i += 32) { const float a = xr[i] - mean; q = fmaf(a, a, q); }
   const float rstd = rsqrtf(warp_sum(q) / (float)d + eps);
   for (int i = lane; i < d; i += 32) y[(long long)row * d + i] = (xr[i] - mean) * rstd * gamma[i] + beta[i];
-}
-
-// a ragged batch's CLS rows x[tok_off_b, :] -> y [B, d] (the input of the final norm)
-__global__ void gather_cls_rows_kernel(const float* __restrict__ x, const RaggedImage* __restrict__ imgs,
-                                       float* __restrict__ y, int B, int d) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * d) return;
-  y[i] = x[(long long)imgs[i / d].tok_off * d + i % d];
 }
 
 __global__ void f32_to_f16_kernel(const float* __restrict__ src, __half* __restrict__ dst, size_t n) {
@@ -72,12 +85,9 @@ struct dss_vit {
   __half* patch_w = nullptr;
   float *patch_b = nullptr, *cls = nullptr;
   float *norm_w = nullptr, *norm_b = nullptr;   // final LayerNorm (only needed by dss_vit_forward_cls)
-  float* pos_dev = nullptr;   // [1 + grid0^2, d] the stored positional grid (ragged batches interpolate it on the device)
+  float* pos_dev = nullptr;   // [1 + grid0^2, d] the stored positional grid (every forward interpolates it on the device)
   CUtensorMap tm_patch;
   std::vector<dss::BlockW> blocks;
-  std::vector<float> pos_host;                        // [1 + grid0^2, d] fp32 host copy
-  std::map<std::tuple<int, int, bool>, float*> pos_cache;   // (Hp, Wp, stored grid) -> device [T, d]
-  std::vector<std::tuple<int, int, bool>> pos_order;        // insertion order: the cache is bounded (oldest evicted)
 };
 
 namespace dss {
@@ -111,7 +121,15 @@ static void interp_axis(int in, int out, double scale_factor, std::vector<int>& 
 // patch multiples first as the reference does before get_intermediate_layers (then Hp == Wp decides).
 static bool pos_is_stored(int g, int Hp, int Wp, bool square) { return Hp == g && Wp == g && square; }
 
-// pos_src [1 + g*g, d] -> pos_out [1 + Hp*Wp, d]; host memory, pure CPU (runs once per distinct image shape)
+// The identity rule for one H x W image with an Hp x Wp patch grid. The model's own forward (the final-norm CLS token
+// and the residual-stream hook) takes the image as is, so its pixel sizes decide; forward_k's and localization's inputs
+// are cropped or padded to patch multiples by the reference before the model sees them, so their patch grid decides.
+static bool image_pos_is_stored(int g, int H, int W, int Hp, int Wp, bool own_forward) {
+  return pos_is_stored(g, Hp, Wp, own_forward ? H == W : Hp == Wp);
+}
+
+// pos_src [1 + g*g, d] -> pos_out [1 + Hp*Wp, d]; host memory, pure CPU: the reference the device tables (pos_cls_kernel)
+// are tested against
 static void interp_pos_host(const float* src, int g, int d, int Hp, int Wp, bool square, float* pos) {
   std::copy(src, src + d, pos);  // CLS slot untouched
   if (pos_is_stored(g, Hp, Wp, square)) {
@@ -140,37 +158,69 @@ static void interp_pos_host(const float* src, int g, int d, int Hp, int Wp, bool
     }
 }
 
-static int get_pos(dss_vit* h, int Hp, int Wp, bool square, cudaStream_t st, float** out) {
-  const int d = h->cfg.dim, g = h->cfg.grid0, T = Hp * Wp + 1;
-  // keyed by the identity decision too: a g x g grid from a non-square input must not get the stored entry
-  const auto key = std::make_tuple(Hp, Wp, pos_is_stored(g, Hp, Wp, square));
-  auto it = h->pos_cache.find(key);
-  if (it != h->pos_cache.end()) {
-    *out = it->second;
-    return DSS_OK;
+// ---- the same interpolation on the device. interp_axis's taps for output cell o of an axis of n cells: the scale, its
+// reciprocal and the cubic coefficients in double and the source coordinate in fp32, every operation rounded on its
+// own as the host code rounds it (no contraction), so the taps are the host's bits. Returns the first source index.
+__device__ __forceinline__ double cubic1_rn(double x, double A) {
+  return __dadd_rn(__dmul_rn(__dmul_rn(__dsub_rn(__dmul_rn(A + 2.0, x), A + 3.0), x), x), 1.0);
+}
+__device__ __forceinline__ double cubic2_rn(double x, double A) {
+  return __dsub_rn(__dmul_rn(__dadd_rn(__dmul_rn(__dsub_rn(__dmul_rn(A, x), 5.0 * A), x), 8.0 * A), x), 4.0 * A);
+}
+__device__ __forceinline__ int pos_taps(int g, int n, int o, float (&w)[4]) {
+  const double A = -0.75;
+  const float rscale = __double2float_rn(__ddiv_rn(1.0, __ddiv_rn(__dadd_rn((double)n, 0.1), (double)g)));
+  const float real = __fsub_rn(__fmul_rn(rscale, __fadd_rn((float)o, 0.5f)), 0.5f);
+  const float fl = floorf(real);
+  const double t = (double)__fsub_rn(real, fl);
+  w[0] = __double2float_rn(cubic2_rn(__dadd_rn(t, 1.0), A));
+  w[1] = __double2float_rn(cubic1_rn(t, A));
+  w[2] = __double2float_rn(cubic1_rn(__dsub_rn(1.0, t), A));
+  w[3] = __double2float_rn(cubic2_rn(__dsub_rn(2.0, t), A));
+  return (int)fl;
+}
+
+// The token embedding's shape-dependent part, before the patch GEMM: the positional table pos [rows, d] (Loc: one
+// shared [T, d] table, or a ragged batch's tables laid out like the residual stream) and every image's CLS row
+// x[row0(b)] = cls + pos[0]. The bicubic resampling of interp_pos_host with the same tap order and every product and
+// sum rounded on its own, so the tables are dss_pos_embed_interp_host's bits; the CLS slot and, under the identity
+// rule, the whole grid are copied. One thread per POS_PC consecutive channels of max(rows, B) rows (d is 384 or 768),
+// so the taps are computed once for POS_PC outputs.
+constexpr int POS_PC = 4;
+template <typename Loc>
+__global__ void pos_cls_kernel(const float* __restrict__ grid, int g, const float* __restrict__ cls, Loc loc, int B,
+                               long long rows, int d, float* __restrict__ pos, float* __restrict__ x) {
+  const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * POS_PC;
+  const long long r = i / d;
+  const int c0 = (int)(i % d);
+  if (r < B) {
+#pragma unroll
+    for (int c = c0; c < c0 + POS_PC; ++c) x[loc.row0((int)r) * d + c] = cls[c] + grid[c];
   }
-  std::vector<float> pos((size_t)T * d);
-  interp_pos_host(h->pos_host.data(), g, d, Hp, Wp, square, pos.data());
-  float* dev = nullptr;
-  DSS_CHECK_CUDA(cudaMalloc(&dev, (size_t)T * d * sizeof(float)));
-  DSS_CHECK_CUDA(cudaMemcpyAsync(dev, pos.data(), (size_t)T * d * sizeof(float), cudaMemcpyHostToDevice, st));
-  DSS_CHECK_CUDA(cudaStreamSynchronize(st));  // `pos` is a pageable temporary
-  // bounded: data sets with hundreds of distinct image sizes must not grow the cache without limit. Eviction happens
-  // after the stream synchronisation above, so no kernel that was given the evicted pointer is still running.
-  constexpr size_t kMaxPosGrids = 64;
-  if (h->pos_order.size() >= kMaxPosGrids) {
-    auto old = h->pos_order.front();
-    h->pos_order.erase(h->pos_order.begin());
-    auto oit = h->pos_cache.find(old);
-    if (oit != h->pos_cache.end()) {
-      cudaFree(oit->second);
-      h->pos_cache.erase(oit);
+  if (r >= rows) return;
+  const PosRow p = loc.at(r);
+  if (p.t == 0 || p.stored) {
+#pragma unroll
+    for (int k = 0; k < POS_PC; ++k) pos[i + k] = grid[(long long)p.t * d + c0 + k];
+    return;
+  }
+  float wy[4], wx[4];
+  const int iy = pos_taps(g, p.Hp, (p.t - 1) / p.Wp, wy), ix = pos_taps(g, p.Wp, (p.t - 1) % p.Wp, wx);
+  float o[POS_PC] = {};
+#pragma unroll
+  for (int a = 0; a < 4; ++a) {
+    const int sy = min(max(iy - 1 + a, 0), g - 1);
+#pragma unroll
+    for (int b = 0; b < 4; ++b) {
+      const int sx = min(max(ix - 1 + b, 0), g - 1);
+      const float wgt = __fmul_rn(wy[a], wx[b]);
+      const float* s = grid + ((long long)(sy * g + sx) + 1) * d + c0;
+#pragma unroll
+      for (int k = 0; k < POS_PC; ++k) o[k] = __fadd_rn(o[k], __fmul_rn(wgt, s[k]));
     }
   }
-  h->pos_cache[key] = dev;
-  h->pos_order.push_back(key);
-  *out = dev;
-  return DSS_OK;
+#pragma unroll
+  for (int k = 0; k < POS_PC; ++k) pos[i + k] = o[k];
 }
 
 // ks = 1 (DSS_VIT_PRECISION_FP16) or 3 (DSS_VIT_PRECISION_FP32, split): patches, xn and attn hold ks fp16 groups per
@@ -185,11 +235,13 @@ struct VitWs {
   __half* qkv;      // [B*T, 3d] (fp16) | [B*T, 9d] (split)
   __half* hid;      // [B*T, ks 4d]
   float* f32;       // split only
+  float* pos;       // [pos_rows, d] positional table(s)
   size_t total;
 };
 
-// n_patches patch rows and M token rows (B Np and B T for a uniform batch)
-static VitWs carve(const dss_vit_config& c, size_t n_patches, size_t M, void* base, int precision) {
+// n_patches patch rows and M token rows (B Np and B T for a uniform batch); pos_rows positional rows (T for a uniform
+// batch, whose images share one table; M for a ragged one)
+static VitWs carve(const dss_vit_config& c, size_t n_patches, size_t M, size_t pos_rows, void* base, int precision) {
   const int d = c.dim;
   const size_t ks = precision == DSS_VIT_PRECISION_FP32 ? 3 : 1;
   uint8_t* p = reinterpret_cast<uint8_t*>(base);
@@ -214,6 +266,7 @@ static VitWs carve(const dss_vit_config& c, size_t n_patches, size_t M, void* ba
     w.hid = reinterpret_cast<__half*>(take(hid_bytes));
     w.f32 = nullptr;
   }
+  w.pos = reinterpret_cast<float*>(take(pos_rows * d * 4));
   w.total = off;
   return w;
 }
@@ -228,29 +281,37 @@ struct Ragged {
   const int* tile_prefix;         // [B + 1]
   const int* patch_rows;          // [n_patches] token row of each patch row
   const int* k_rows;              // [M] feature row of each token row (-1: CLS)
-  float* pos_all;                 // [M, d] positional rows, laid out like the residual stream
 };
 
+// the positional table (pos_rows rows) and every image's CLS row: pos_cls_kernel over batch `loc`
+template <typename Loc>
+static int launch_pos_cls(const dss_vit* h, Loc loc, int B, long long pos_rows, const VitWs& w, cudaStream_t st) {
+  const int d = h->cfg.dim;
+  const long long n = std::max<long long>(pos_rows, B) * (d / POS_PC);
+  LaunchScope scope(st, KC_CLS_ROW);
+  pos_cls_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(h->pos_dev, h->cfg.grid0, h->cls, loc, B, pos_rows, d,
+                                                              w.pos, w.x);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
 // modes 1 and 2 after the blocks: the residual stream, or the final LayerNorm of the CLS rows
-static int vit_tail(const dss_vit* h, const float* x, int mode, float* out, int B, int T, const Ragged* rg,
-                    cudaStream_t st) {
+static int vit_tail(const dss_vit* h, const float* x, int mode, float* out, int B, const UniformRows& uni,
+                    const Ragged* rg, cudaStream_t st) {
   const int d = h->cfg.dim;
   if (mode == 2) {
     // upstream VisionTransformer.forward: x = norm(x); return x[:, 0]  (LayerNorm is row-wise: only the CLS rows)
     DSS_REQUIRE(h->norm_w && h->norm_b, "vit: the final LayerNorm weights (norm.weight / norm.bias) were not loaded");
     LaunchScope scope(st, KC_LAYERNORM);
-    long long stride = (long long)T * d;
-    if (rg) {   // the CLS rows gathered into pos_all, which is free once the tokens are embedded
-      gather_cls_rows_kernel<<<cdiv(B * d, 256), 256, 0, st>>>(x, rg->imgs, rg->pos_all, B, d);
-      DSS_CHECK_CUDA(cudaGetLastError());
-      x = rg->pos_all;
-      stride = d;
-    }
-    layernorm_rows_f32_kernel<<<cdiv(B, 4), 128, 0, st>>>(x, stride, h->norm_w, h->norm_b, out, B, d, h->cfg.ln_eps);
+    if (rg)
+      layernorm_rows_f32_kernel<<<cdiv(B, 4), 128, 0, st>>>(x, RaggedRows{rg->imgs, B}, h->norm_w, h->norm_b, out, B, d,
+                                                            h->cfg.ln_eps);
+    else
+      layernorm_rows_f32_kernel<<<cdiv(B, 4), 128, 0, st>>>(x, uni, h->norm_w, h->norm_b, out, B, d, h->cfg.ln_eps);
     DSS_CHECK_CUDA(cudaGetLastError());
   } else {
     DSS_REQUIRE(!rg, "vit: no residual-stream output for ragged batches");
-    DSS_CHECK_CUDA(cudaMemcpyAsync(out, x, (size_t)B * T * d * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    DSS_CHECK_CUDA(cudaMemcpyAsync(out, x, (size_t)B * uni.T * d * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
   return DSS_OK;
 }
@@ -277,20 +338,13 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   const int M = rg ? (int)rg->M : B * T, n_patches = rg ? (int)rg->n_patches : B * Np;
   const bool split = h->precision == DSS_VIT_PRECISION_FP32;
   const int ks = split ? 3 : 1;   // fp16 values per operand value
-  VitWs w = carve(c, (size_t)n_patches, (size_t)M, ws, h->precision);
+  VitWs w = carve(c, (size_t)n_patches, (size_t)M, rg ? (size_t)M : (size_t)T, ws, h->precision);
   if (ws_bytes < w.total) {
     set_error("vit: workspace too small (%zu < %zu)", ws_bytes, w.total);
     return DSS_ERR_WORKSPACE;
   }
+  const UniformRows uni{T, Hp, Wp, !rg && image_pos_is_stored(c.grid0, H, W, Hp, Wp, mode == 1 || mode == 2)};
   int rc;
-  float* pos = nullptr;
-  if (!rg) {
-    // forward_k's and localization's inputs are cropped or padded to patch multiples by the reference before the model
-    // sees them, so their patch grid decides; the model's own forward (box crops) and the token hook take the image as
-    // is
-    const bool square = (mode == 1 || mode == 2) ? H == W : Hp == Wp;
-    if ((rc = get_pos(h, Hp, Wp, square, st, &pos))) return rc;
-  }
 
   CUtensorMap tm_patches, tm_xn, tm_attn, tm_hid;
   if ((rc = make_tmap_f16(&tm_patches, w.patches, n_patches, ks * Kp, 128))) return rc;
@@ -304,19 +358,19 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   if ((rc = make_tmap_out(&tm_qkv_out, split ? (void*)w.f32 : w.qkv, M, 3 * d, split))) return rc;
   if ((rc = make_tmap_out(&tm_hid_out, split ? (void*)w.f32 : w.hid, M, hd, split))) return rc;
 
-  // tokens: x[b, 1+n, :] = patch_embed + pos ; x[b, 0, :] = cls + pos[0]
+  // tokens: x[b, 0, :] = cls + pos[0] and the positional table, then x[b, 1+n, :] = patch_embed + pos[1+n]
   if (rg) {
     if ((rc = launch_im2col_ragged(img, w.patches, rg->imgs, B, n_patches, P, split, st))) return rc;
+    if ((rc = launch_pos_cls(h, RaggedRows{rg->imgs, B}, B, M, w, st))) return rc;
     if ((rc = gemm_f16_tc_rows(tm_patches, h->tm_patch, h->patch_b, w.x, n_patches, d, ks * Kp, DSS_EPI_PATCH_F32,
-                               rg->pos_all, rg->patch_rows, st, KC_GEMM_PATCH)))
+                               w.pos, rg->patch_rows, st, KC_GEMM_PATCH)))
       return rc;
-    if ((rc = launch_cls_row_ragged(w.x, h->cls, rg->pos_all, rg->imgs, B, d, st))) return rc;
   } else {
     if ((rc = launch_im2col(img, w.patches, B, H, W, P, pad, split, st))) return rc;
+    if ((rc = launch_pos_cls(h, uni, B, T, w, st))) return rc;
     if ((rc = gemm_f16_tc(tm_patches, h->tm_patch, nullptr, h->patch_b, w.x, n_patches, d, ks * Kp, DSS_EPI_PATCH_F32,
-                          pos, Np, T, st, KC_GEMM_PATCH, 128)))
+                          w.pos, Np, T, st, KC_GEMM_PATCH, 128)))
       return rc;
-    if ((rc = launch_cls_row(w.x, h->cls, pos, B, T, d, st))) return rc;
   }
 
   // the full qkv projection: the attention operands (fp16), or the fp32 values they are split from
@@ -352,7 +406,7 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
                           0, st, KC_GEMM_FC2, gemm_tile_n())))
       return rc;
   }
-  if (mode == 1 || mode == 2) return vit_tail(h, w.x, mode, out, B, T, rg, st);
+  if (mode == 1 || mode == 2) return vit_tail(h, w.x, mode, out, B, uni, rg, st);
 
   const BlockW& bw = h->blocks[n_full];
   if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, split, st))) return rc;
@@ -372,16 +426,15 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   return DSS_OK;
 }
 
-// ---- ragged batches: host plan. Workspace = the forward's buffers (carve) | pos_all [M, d] fp32 | one block of tables
-// (RaggedImage [B], tile_prefix [B + 1], patch_rows [n_patches], k_rows [M], axis indices [A] and weights [4 A], A the
-// sum of Hp + Wp over the images whose positional grid is resampled), uploaded with one copy per forward.
+// ---- ragged batches: host plan. Workspace = the forward's buffers (carve, positional tables [M, d] included) | one
+// block of tables (RaggedImage [B], tile_prefix [B + 1], patch_rows [n_patches], k_rows [M]), uploaded with one copy
+// per forward.
 struct RaggedPlan {
   std::vector<RaggedImage> imgs;
-  std::vector<int> tile_prefix, patch_rows, k_rows, axis_idx;
-  std::vector<float> axis_w;
-  long long n_patches = 0, M = 0, axis = 0;
-  size_t vit_bytes = 0, off_pos = 0, off_tables = 0, tables_bytes = 0, total = 0;
-  size_t t_imgs = 0, t_tiles = 0, t_prows = 0, t_krows = 0, t_aidx = 0, t_aw = 0;   // offsets inside the table block
+  std::vector<int> tile_prefix, patch_rows, k_rows;
+  long long n_patches = 0, M = 0;
+  size_t vit_bytes = 0, tables_bytes = 0, total = 0;
+  size_t t_imgs = 0, t_tiles = 0, t_prows = 0, t_krows = 0;   // offsets inside the table block
 };
 
 constexpr int RAGGED_TILE = 128;   // query rows per attention CTA (FA_BM, AS_BM)
@@ -392,16 +445,13 @@ static int ragged_plan(const dss_vit* h, const int* dims, int B, int mode, bool 
   DSS_REQUIRE(B > 0, "vit_ragged: B must be positive (got %d)", B);
   DSS_REQUIRE(mode == DSS_VIT_RAGGED_K || mode == DSS_VIT_RAGGED_CLS, "vit_ragged: unknown mode %d", mode);
   const dss_vit_config& c = h->cfg;
-  const int P = c.patch, g = c.grid0;
-  long long px = 0, np = 0, M = 0, axis = 0, tiles = 0;
+  const int P = c.patch;
+  long long px = 0, np = 0, M = 0, tiles = 0;
   for (int b = 0; b < B; ++b) {
     const int H = dims[2 * b], W = dims[2 * b + 1];
     DSS_REQUIRE(H >= 0 && W >= 0, "vit_ragged: image %d has negative size %dx%d", b, H, W);
     DSS_REQUIRE(H >= P && W >= P, "vit_ragged: image %d (%dx%d) is smaller than one %d-pixel patch", b, H, W, P);
     const long long Hp = H / P, Wp = W / P;
-    // the identity rule of interpolate_pos_encoding: pixel H == W for the model's own forward, Hp == Wp for forward_k
-    const bool square = mode == DSS_VIT_RAGGED_CLS ? H == W : Hp == Wp;
-    if (!pos_is_stored(g, (int)Hp, (int)Wp, square)) axis += Hp + Wp;
     px += (long long)H * W;
     np += Hp * Wp;
     M += Hp * Wp + 1;
@@ -414,49 +464,30 @@ static int ragged_plan(const dss_vit* h, const int* dims, int B, int mode, bool 
   }
   pl.n_patches = np;
   pl.M = M;
-  pl.axis = axis;
   size_t off = 0;
   auto part = [&off](size_t bytes) { const size_t o = off; off += align_up(bytes, 16); return o; };
   pl.t_imgs = part((size_t)B * sizeof(RaggedImage));
   pl.t_tiles = part((size_t)(B + 1) * 4);
   pl.t_prows = part((size_t)np * 4);
   pl.t_krows = part((size_t)M * 4);
-  pl.t_aidx = part((size_t)axis * 4);
-  pl.t_aw = part((size_t)axis * 16);
   pl.tables_bytes = off;
-  pl.vit_bytes = carve(c, (size_t)np, (size_t)M, nullptr, h->precision).total;
-  pl.off_pos = pl.vit_bytes;
-  pl.off_tables = pl.off_pos + align_up((size_t)M * c.dim * 4, 1024);
-  pl.total = pl.off_tables + align_up(pl.tables_bytes, 1024);
+  pl.vit_bytes = carve(c, (size_t)np, (size_t)M, (size_t)M, nullptr, h->precision).total;
+  pl.total = pl.vit_bytes + align_up(pl.tables_bytes, 1024);
   if (!tables) return DSS_OK;
 
   pl.imgs.resize(B);
   pl.tile_prefix.assign(1, 0);
   pl.patch_rows.resize((size_t)np);
   pl.k_rows.resize((size_t)M);
-  pl.axis_idx.clear();
-  pl.axis_w.clear();
   long long pxo = 0, po = 0, to = 0, fo = 0;
-  std::vector<int> iy, ix;
-  std::vector<float> wy, wx;
   for (int b = 0; b < B; ++b) {
     const int H = dims[2 * b], W = dims[2 * b + 1], Hp = H / P, Wp = W / P, Np = Hp * Wp;
-    const bool square = mode == DSS_VIT_RAGGED_CLS ? H == W : Hp == Wp;
     RaggedImage& im = pl.imgs[b];
     im.px_off = pxo;
     im.H = H; im.W = W; im.Hp = Hp; im.Wp = Wp;
     im.patch_off = (int)po;
     im.tok_off = (int)to;
-    im.stored = pos_is_stored(g, Hp, Wp, square) ? 1 : 0;
-    im.axis_off = (int)pl.axis_idx.size();
-    if (!im.stored) {   // the per-axis indices and weights of interp_pos_host
-      interp_axis(g, Hp, ((double)Hp + 0.1) / (double)g, iy, wy);
-      interp_axis(g, Wp, ((double)Wp + 0.1) / (double)g, ix, wx);
-      pl.axis_idx.insert(pl.axis_idx.end(), iy.begin(), iy.end());
-      pl.axis_idx.insert(pl.axis_idx.end(), ix.begin(), ix.end());
-      pl.axis_w.insert(pl.axis_w.end(), wy.begin(), wy.end());
-      pl.axis_w.insert(pl.axis_w.end(), wx.begin(), wx.end());
-    }
+    im.stored = image_pos_is_stored(c.grid0, H, W, Hp, Wp, mode == DSS_VIT_RAGGED_CLS) ? 1 : 0;
     pl.tile_prefix.push_back(pl.tile_prefix.back() + (Np + RAGGED_TILE) / RAGGED_TILE);
     pl.k_rows[(size_t)to] = -1;
     for (int n = 0; n < Np; ++n) {
@@ -471,8 +502,7 @@ static int ragged_plan(const dss_vit* h, const int* dims, int B, int mode, bool 
   return DSS_OK;
 }
 
-// Validates a ragged batch (rmode: DSS_VIT_RAGGED_*), uploads its tables into the workspace and computes its
-// positional tables (rg.pos_all).
+// Validates a ragged batch (rmode: DSS_VIT_RAGGED_*) and uploads its tables into the workspace.
 static int ragged_setup(dss_vit* h, const int* dims, int B, int rmode, void* ws, size_t ws_bytes, cudaStream_t st,
                         RaggedPlan& pl, Ragged& rg) {
   int rc = ragged_plan(h, dims, B, rmode, true, pl);
@@ -488,10 +518,7 @@ static int ragged_setup(dss_vit* h, const int* dims, int B, int rmode, void* ws,
   put(pl.t_tiles, pl.tile_prefix.data(), pl.tile_prefix.size() * 4);
   put(pl.t_prows, pl.patch_rows.data(), pl.patch_rows.size() * 4);
   put(pl.t_krows, pl.k_rows.data(), pl.k_rows.size() * 4);
-  put(pl.t_aidx, pl.axis_idx.data(), pl.axis_idx.size() * 4);
-  put(pl.t_aw, pl.axis_w.data(), pl.axis_w.size() * 4);
-  uint8_t* base = reinterpret_cast<uint8_t*>(ws);
-  uint8_t* tb = base + pl.off_tables;
+  uint8_t* tb = reinterpret_cast<uint8_t*>(ws) + pl.vit_bytes;
   // pageable source: the call returns once the bytes are staged, so `blob` may go out of scope (no stream sync)
   DSS_CHECK_CUDA(cudaMemcpyAsync(tb, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
   rg.B = B;
@@ -502,11 +529,6 @@ static int ragged_setup(dss_vit* h, const int* dims, int B, int rmode, void* ws,
   rg.tile_prefix = reinterpret_cast<const int*>(tb + pl.t_tiles);
   rg.patch_rows = reinterpret_cast<const int*>(tb + pl.t_prows);
   rg.k_rows = reinterpret_cast<const int*>(tb + pl.t_krows);
-  rg.pos_all = reinterpret_cast<float*>(base + pl.off_pos);
-  if ((rc = launch_pos_ragged(h->pos_dev, h->cfg.grid0, h->cfg.dim, rg.imgs, B, pl.M,
-                              reinterpret_cast<const int*>(tb + pl.t_aidx), reinterpret_cast<const float*>(tb + pl.t_aw),
-                              rg.pos_all, st)))
-    return rc;
   return DSS_OK;
 }
 
@@ -540,7 +562,6 @@ extern "C" int dss_vit_create(const dss_vit_config* cfg, dss_vit_t** out) {
 
 extern "C" void dss_vit_destroy(dss_vit_t* h) {
   if (!h) return;
-  for (auto& kv : h->pos_cache) cudaFree(kv.second);
   if (h->arena) cudaFree(h->arena);
   delete h;
 }
@@ -652,13 +673,6 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
     if ((rc = make_tmap_f16(&b.tm_fc1, b.fc1_w, (int)hid, kd, gemm_tile_n() / 2))) return rc;
     if ((rc = make_tmap_f16(&b.tm_fc2, b.fc2_w, (int)d, khid, gemm_tile_n() / 2))) return rc;
   }
-  // host copy of the positional grid for interpolation; drop stale interpolations
-  h->pos_host.resize(npos);
-  DSS_CHECK_CUDA(cudaMemcpyAsync(h->pos_host.data(), w->pos_embed, npos * 4, cudaMemcpyDeviceToHost, st));
-  DSS_CHECK_CUDA(cudaStreamSynchronize(st));
-  for (auto& kv : h->pos_cache) cudaFree(kv.second);
-  h->pos_cache.clear();
-  h->pos_order.clear();
   h->loaded = true;
   return DSS_OK;
 }
@@ -666,7 +680,7 @@ extern "C" int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_
 extern "C" size_t dss_vit_workspace_bytes(const dss_vit_t* h, int B, int H, int W) {
   if (!h || B <= 0 || H < h->cfg.patch || W < h->cfg.patch) return 0;
   const size_t Np = (size_t)(H / h->cfg.patch) * (W / h->cfg.patch);
-  return carve(h->cfg, (size_t)B * Np, (size_t)B * (Np + 1), nullptr, h->precision).total;
+  return carve(h->cfg, (size_t)B * Np, (size_t)B * (Np + 1), Np + 1, nullptr, h->precision).total;
 }
 
 extern "C" size_t dss_vit_forward_last_workspace_bytes(const dss_vit_t* h, int B, int H, int W, int pad) {
@@ -674,7 +688,7 @@ extern "C" size_t dss_vit_forward_last_workspace_bytes(const dss_vit_t* h, int B
   const int P = h->cfg.patch;
   if (!pad) return dss_vit_workspace_bytes(h, B, H, W);
   const size_t Np = (size_t)cdiv(H, P) * cdiv(W, P);
-  return carve(h->cfg, (size_t)B * Np, (size_t)B * (Np + 1), nullptr, h->precision).total;
+  return carve(h->cfg, (size_t)B * Np, (size_t)B * (Np + 1), Np + 1, nullptr, h->precision).total;
 }
 
 extern "C" int dss_vit_forward_last(dss_vit_t* h, const uint8_t* images_u8, int B, int H, int W, int pad, int which,
@@ -740,22 +754,11 @@ extern "C" int dss_vit_pos_embed_ragged(dss_vit_t* h, const int* dims_host, int 
   Ragged rg;
   int rc = ragged_setup(h, dims_host, B, mode, ws, ws_bytes, st, pl, rg);
   if (rc) return rc;
-  DSS_CHECK_CUDA(cudaMemcpyAsync(pos_out, rg.pos_all, (size_t)pl.M * h->cfg.dim * sizeof(float),
-                                 cudaMemcpyDeviceToDevice, st));
-  return DSS_OK;
-}
-
-extern "C" int dss_vit_pos_cache_entries(const dss_vit_t* h) { return h ? (int)h->pos_cache.size() : -1; }
-
-extern "C" int dss_vit_pos_embed(dss_vit_t* h, int Hp, int Wp, float* out, dss_stream_t stream) {
-  DSS_REQUIRE(h && h->loaded && out, "vit_pos_embed: handle not loaded / null out");
-  DSS_REQUIRE(Hp > 0 && Wp > 0, "vit_pos_embed: empty grid");
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  float* pos = nullptr;
-  int rc = get_pos(h, Hp, Wp, Hp == Wp, st, &pos);
-  if (rc) return rc;
-  DSS_CHECK_CUDA(cudaMemcpyAsync(out, pos, ((size_t)Hp * Wp + 1) * h->cfg.dim * sizeof(float),
-                                 cudaMemcpyDeviceToDevice, st));
+  // the forward's first step (it also writes the CLS rows of the workspace's residual stream)
+  const VitWs w = carve(h->cfg, (size_t)pl.n_patches, (size_t)pl.M, (size_t)pl.M, ws, h->precision);
+  if ((rc = launch_pos_cls(h, RaggedRows{rg.imgs, B}, B, pl.M, w, st))) return rc;
+  DSS_CHECK_CUDA(cudaMemcpyAsync(pos_out, w.pos, (size_t)pl.M * h->cfg.dim * sizeof(float), cudaMemcpyDeviceToDevice,
+                                 st));
   return DSS_OK;
 }
 

@@ -1,4 +1,4 @@
-// Non-GEMM kernels of the DINO ViT forward: pixel normalisation + im2col, CLS row, LayerNorm, CLS attention row, and
+// Non-GEMM kernels of the DINO ViT forward: pixel normalisation + im2col, LayerNorm, CLS attention row, and
 // the split-fp16 operand producers of DSS_VIT_PRECISION_FP32. In that mode every value that feeds a tensor-core
 // product is written as the three fp16 groups of split_f16 (common.cuh), so that one fp16 GEMM over K' = 3 K gives the
 // fp32-equivalent product: activations in A order, weights (and K / V of attention) in B order. The fp32 value that is
@@ -139,58 +139,6 @@ __global__ void im2col_ragged_kernel(const uint8_t* __restrict__ img, __half* __
       *reinterpret_cast<uint4*>(out + gp * Kp + (c * P + py) * P + px0) = q;
     }
   }
-}
-
-// Positional tables of a ragged batch: pos_all [M, d] laid out like the residual stream, image b's rows at tok_off its
-// [T_b, d] table. The bicubic resampling of interp_pos_host (vit.cu) with the same per-axis indices and fp32 weights
-// (computed on the host), the same tap order and every product and sum rounded on its own (no contraction), so the
-// tables are the host routine's bits; the CLS row and, under the identity rule, the whole grid are copied.
-__global__ void pos_ragged_kernel(const float* __restrict__ src, int g, int d, const RaggedImage* __restrict__ imgs, int B,
-                                  long long M, const int* __restrict__ axis_idx, const float* __restrict__ axis_w,
-                                  float* __restrict__ pos_all) {
-  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= M * d) return;
-  const long long row = i / d;
-  const int c = (int)(i % d);
-  const int b = ragged_find(B, row, [&](int j) { return imgs[j].tok_off; });
-  const RaggedImage im = imgs[b];
-  const int t = (int)(row - im.tok_off);
-  if (t == 0 || im.stored) {
-    pos_all[i] = src[(long long)t * d + c];
-    return;
-  }
-  const int y = (t - 1) / im.Wp, x = (t - 1) % im.Wp;
-  const int ay = im.axis_off + y, ax = im.axis_off + im.Hp + x;
-  float o = 0.f;
-#pragma unroll
-  for (int a = 0; a < 4; ++a) {
-    const int sy = min(max(axis_idx[ay] - 1 + a, 0), g - 1);
-#pragma unroll
-    for (int bb = 0; bb < 4; ++bb) {
-      const int sx = min(max(axis_idx[ax] - 1 + bb, 0), g - 1);
-      const float wgt = __fmul_rn(axis_w[4 * ay + a], axis_w[4 * ax + bb]);
-      o = __fadd_rn(o, __fmul_rn(wgt, src[((long long)(sy * g + sx) + 1) * d + c]));
-    }
-  }
-  pos_all[i] = o;
-}
-
-// x[b, 0, :] = cls + pos[0, :]
-__global__ void cls_row_kernel(float* __restrict__ x, const float* __restrict__ cls, const float* __restrict__ pos,
-                               int B, int T, int d) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * d) return;
-  const int b = i / d, c = i % d;
-  x[(long long)b * T * d + c] = cls[c] + pos[c];
-}
-
-// ragged: x[tok_off_b, :] = cls + pos_all[tok_off_b, :]
-__global__ void cls_row_ragged_kernel(float* __restrict__ x, const float* __restrict__ cls, const float* __restrict__ pos,
-                                      const RaggedImage* __restrict__ imgs, int B, int d) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= B * d) return;
-  const long long r = (long long)imgs[i / d].tok_off * d + i % d;
-  x[r] = cls[i % d] + pos[r];
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -340,13 +288,6 @@ int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P,
   return DSS_OK;
 }
 
-int launch_cls_row(float* x, const float* cls, const float* pos, int B, int T, int d, cudaStream_t st) {
-  LaunchScope scope(st, KC_CLS_ROW);
-  cls_row_kernel<<<cdiv(B * d, 256), 256, 0, st>>>(x, cls, pos, B, T, d);
-  DSS_CHECK_CUDA(cudaGetLastError());
-  return DSS_OK;
-}
-
 int launch_im2col_ragged(const uint8_t* img, void* patches, const RaggedImage* imgs, int B, long long n_patches, int P,
                          bool split, cudaStream_t st) {
   DSS_REQUIRE(img && patches && imgs && B > 0 && n_patches > 0, "im2col_ragged: bad arguments");
@@ -357,22 +298,6 @@ int launch_im2col_ragged(const uint8_t* img, void* patches, const RaggedImage* i
     im2col_ragged_kernel<true><<<grid_for(n_patches * 3 * P * P, 256), 256, 0, st>>>(img, out, imgs, B, n_patches, P);
   else
     im2col_ragged_kernel<false><<<grid_for(n_patches * P * (P / 8), 256), 256, 0, st>>>(img, out, imgs, B, n_patches, P);
-  DSS_CHECK_CUDA(cudaGetLastError());
-  return DSS_OK;
-}
-
-int launch_pos_ragged(const float* pos_src, int grid0, int d, const RaggedImage* imgs, int B, long long M,
-                      const int* axis_idx, const float* axis_w, float* pos_all, cudaStream_t st) {
-  LaunchScope scope(st, KC_CLS_ROW);
-  pos_ragged_kernel<<<grid_for(M * d, 256), 256, 0, st>>>(pos_src, grid0, d, imgs, B, M, axis_idx, axis_w, pos_all);
-  DSS_CHECK_CUDA(cudaGetLastError());
-  return DSS_OK;
-}
-
-int launch_cls_row_ragged(float* x, const float* cls, const float* pos_all, const RaggedImage* imgs, int B, int d,
-                          cudaStream_t st) {
-  LaunchScope scope(st, KC_CLS_ROW);
-  cls_row_ragged_kernel<<<cdiv(B * d, 256), 256, 0, st>>>(x, cls, pos_all, imgs, B, d);
   DSS_CHECK_CUDA(cudaGetLastError());
   return DSS_OK;
 }

@@ -266,9 +266,15 @@ class DinoViT:
         return out, [(b, b + 1) for b in range(B)]
 
     def pos_embed(self, Hp: int, Wp: int) -> torch.Tensor:
+        """The positional embedding [Hp * Wp + 1, d] fp32 the forwards add for an Hp x Wp patch grid (forward_k's
+        identity rule: the stored grid for a square grid0 x grid0 grid)."""
+        dims = torch.tensor([[Hp * self.patch_size, Wp * self.patch_size]], dtype=torch.int32)
         with torch.cuda.device(self.device):
+            ws = self._ragged_workspace(dims, _lib.VIT_RAGGED_K)
             out = torch.empty(Hp * Wp + 1, self.dim, dtype=torch.float32, device=self.device)
-            _lib.check(self.lib.dss_vit_pos_embed(self._h, Hp, Wp, out.data_ptr(), _lib.stream_ptr(self.device)))
+            _lib.check(self.lib.dss_vit_pos_embed_ragged(self._h, dims.data_ptr(), 1, _lib.VIT_RAGGED_K, out.data_ptr(),
+                                                         ws.data_ptr(), ws.numel(), _lib.stream_ptr(self.device)),
+                       "dss_vit_pos_embed_ragged")
         return out
 
 

@@ -11,7 +11,7 @@
  *     the name ends in _host. The library never synchronises the device and never frees caller memory; all work
  *     is enqueued on the caller's stream (a cudaStream_t passed as void*).
  *   - Scratch memory comes from the caller: query dss_*_workspace_bytes, pass (ws, ws_bytes). Workspaces must be
- *     256-byte aligned. A dss_vit_t handle owns only its packed weights and cached positional embeddings.
+ *     256-byte aligned. A dss_vit_t handle owns only its packed weights.
  *   - Return value: DSS_OK (0) or a negative dss_status; dss_last_error() gives a thread-local message.
  *     Asynchronous numerical outcomes (eigensolver convergence) are reported through device-side info arrays.
  *   - Row-major, C-contiguous tensors; shapes are written [outer, ..., inner].
@@ -97,7 +97,8 @@ void dss_vit_destroy(dss_vit_t* h);
  * DSS_ERR_BAD_ARG. The workspace queries report the size for the handle's mode. */
 enum { DSS_VIT_PRECISION_FP16 = 0, DSS_VIT_PRECISION_FP32 = 1 };
 int dss_vit_set_precision(dss_vit_t* h, int precision);
-/* Packs the weights into the library's fp16 operand layout (synchronises `stream` before returning). */
+/* Packs the weights into the library's fp16 operand layout. The copies run on `stream`: the source buffers must stay
+ * valid until it has run them. */
 int dss_vit_load_weights(dss_vit_t* h, const dss_vit_weights* w, dss_stream_t stream);
 
 size_t dss_vit_workspace_bytes(const dss_vit_t* h, int B, int H, int W);
@@ -132,9 +133,8 @@ int dss_vit_forward_cls(dss_vit_t* h, const uint8_t* images_u8, int B, int H, in
  * Workspace: dss_vit_ragged_workspace_bytes(h, dims_host, B, mode) with mode DSS_VIT_RAGGED_K or DSS_VIT_RAGGED_CLS
  * (0 for a bad batch), 256-byte aligned. Checked on the host before any device work: null pointers, B <= 0, negative
  * sizes, an image smaller than one patch (the message names the image) and a small or misaligned workspace are
- * DSS_ERR_BAD_ARG; a batch whose token rows exceed the tensor-map extents (2^31) is DSS_ERR_UNSUPPORTED. The
- * positional tables are computed on the device per call (the bits of dss_pos_embed_interp_host); the handle's
- * positional cache is neither read nor written. Both precision modes. */
+ * DSS_ERR_BAD_ARG; a batch whose token rows exceed the tensor-map extents (2^31) is DSS_ERR_UNSUPPORTED. Both precision
+ * modes. */
 enum { DSS_VIT_RAGGED_K = 0, DSS_VIT_RAGGED_CLS = 1 };
 size_t dss_vit_ragged_workspace_bytes(const dss_vit_t* h, const int* dims_host, int B, int mode);
 int dss_vit_forward_k_ragged(dss_vit_t* h, const uint8_t* images_u8, const int* dims_host, int B, int which_block,
@@ -143,17 +143,13 @@ int dss_vit_forward_cls_ragged(dss_vit_t* h, const uint8_t* images_u8, const int
                                void* ws, size_t ws_bytes, dss_stream_t stream);
 
 /* The positional tables a ragged forward adds (mode DSS_VIT_RAGGED_*): pos_out [sum T_b, d] fp32 (device), image b's
- * [T_b, d] table at its token rows. Same arguments and workspace as the forwards. */
+ * [T_b, d] table at its token rows, as upstream VisionTransformer.interpolate_pos_encoding computes it (bicubic, scale
+ * (Hp+0.1)/grid0, the identity rule above). Same arguments and workspace as the forwards. Every forward, uniform or
+ * ragged, computes its tables on the device this way, per call: the handle keeps no per-shape state. */
 int dss_vit_pos_embed_ragged(dss_vit_t* h, const int* dims_host, int B, int mode, float* pos_out, void* ws,
                              size_t ws_bytes, dss_stream_t stream);
-/* Number of patch grids in the handle's positional cache (the uniform calls fill it, at most 64; -1 for NULL). */
-int dss_vit_pos_cache_entries(const dss_vit_t* h);
-
-/* Interpolated positional embedding [T, d] fp32 for an (Hp x Wp) patch grid, as upstream
- * VisionTransformer.interpolate_pos_encoding computes it (bicubic, scale (Hp+0.1)/grid0). Copied to out (device). */
-int dss_vit_pos_embed(dss_vit_t* h, int Hp, int Wp, float* out, dss_stream_t stream);
 /* The same interpolation on HOST buffers (pure CPU, no CUDA call): pos_embed_host [1+grid0^2, d] -> out_host
- * [1+Hp*Wp, d]. This is the routine the handle runs once per distinct image shape. */
+ * [1+Hp*Wp, d], with the stored grid for Hp == Wp == grid0. The device tables are this routine's bits. */
 int dss_pos_embed_interp_host(const float* pos_embed_host, int grid0, int d, int Hp, int Wp, float* out_host);
 
 /* ------------------------------------------------------------------------------------------------------------

@@ -102,8 +102,19 @@ def test_workspace_query(handle):
     assert lib.dss_vit_ragged_workspace_bytes(h, _dims(base), 0, 0) == 0
     # at least the uniform call's workspace for the same images; the fp32 mode needs more
     assert ws([(480, 480)] * 4) >= lib.dss_vit_workspace_bytes(h, 4, 480, 480)
+
+    def one_image_tables():
+        # both batch kinds carve the same buffers, positional table included: one image needs the uniform call's
+        # workspace and the ragged tables (RaggedImage, tile prefix, patch -> token and token -> feature rows)
+        for H, W in [(16, 16), (224, 224), (375, 500), (480, 480)]:
+            T = (H // 16) * (W // 16) + 1
+            extra = ws([(H, W)]) - lib.dss_vit_workspace_bytes(h, 1, H, W)
+            assert extra % 1024 == 0 and 8 * T <= extra < 8 * T + 2048, (H, W, extra)
+
+    one_image_tables()
     assert lib.dss_vit_set_precision(h, L.VIT_PRECISION["fp32"]) == 0
     assert ws(base) > w0
+    one_image_tables()
 
 
 def test_pack_images_and_row_ranges():

@@ -4,8 +4,8 @@ Every image's rows from dss_vit_forward_k_ragged / _cls_ragged must be torch.equ
 forward_k / forward_cls, in both precision modes: one-patch and 2 x 2 crops (T = 2, 5), T = 128 and 129 (one row either
 side of a 128-query attention tile), VOC shapes (T = 714), 480^2 (T = 901), ViT-B/8 at 480^2 (T = 3601) next to a T = 2
 crop, a grid0 x grid0 grid from non-square pixels next to a square 224^2 image (the identity rule per image), which_block
-other than -1 and a 264-image batch. Also: rows past the outputs are not written, the device positional tables are
-dss_pos_embed_interp_host's bits for every grid up to 64 x 64, the handle's positional cache is untouched, and
+other than -1 and a 264-image batch. Also: rows past the outputs are not written, the device positional tables of
+ragged and uniform forwards are dss_pos_embed_interp_host's bits (every grid up to 64 x 64 for ragged batches), and
 extract_features / extract_bbox_features write what the per-image uniform forward gives."""
 import ctypes as C
 from concurrent.futures import ThreadPoolExecutor
@@ -125,9 +125,47 @@ def test_no_rows_written_past_the_outputs(cuda, precision):
     assert torch.equal(k[:n], ref)
 
 
+def _host_table(lib, src, g, Hp, Wp):
+    out = torch.empty(Hp * Wp + 1, src.shape[1])
+    assert lib.dss_pos_embed_interp_host(src.data_ptr(), g, src.shape[1], Hp, Wp, out.data_ptr()) == 0
+    return out
+
+
+def _resampled(src, g, Hp, Wp):
+    """interp_pos_host restated in numpy, every operation rounded on its own (taps in double, sums in fp32): the
+    resampled table also for the grid0 x grid0 grid of a non-square image, for which dss_pos_embed_interp_host (the
+    patch-grid rule) returns the stored grid."""
+    f32, A = np.float32, -0.75
+    c1 = lambda x: ((A + 2.0) * x - (A + 3.0)) * x * x + 1.0
+    c2 = lambda x: ((A * x - 5.0 * A) * x + 8.0 * A) * x - 4.0 * A
+
+    def taps(n):
+        rscale = f32(1.0 / ((n + 0.1) / g))
+        for o in range(n):
+            real = rscale * (f32(o) + f32(0.5)) - f32(0.5)
+            fl = np.floor(real)
+            t = float(real - fl)
+            yield int(fl), [f32(c2(t + 1.0)), f32(c1(t)), f32(c1(1.0 - t)), f32(c2(2.0 - t))]
+
+    grid = src[1:].numpy().reshape(g, g, -1)
+    clamp = lambda v: min(max(v, 0), g - 1)
+    rows = [src[0].numpy()]
+    for iy, wy in taps(Hp):
+        for ix, wx in taps(Wp):
+            o = np.zeros(src.shape[1], np.float32)
+            for a in range(4):
+                for b in range(4):
+                    o = o + (wy[a] * wx[b]) * grid[clamp(iy - 1 + a), clamp(ix - 1 + b)]
+            rows.append(o)
+    return torch.from_numpy(np.stack(rows))
+
+
 def test_positional_tables_match_the_host_routine(cuda):
     """Every grid up to 64 x 64 (ViT-S/16, grid0 14) against dss_pos_embed_interp_host, bit for bit: K mode (the
-    identity rule by patch grid). The 14 x 14 grid of a 224 x 232 image in CLS mode is resampled, not the stored grid."""
+    identity rule by patch grid). The 14 x 14 grid of a 224 x 232 image in CLS mode is resampled, not the stored grid.
+    The uniform forwards, ViT-S/16 and ViT-B/8: with zero patch weight and bias, forward_tokens(img, 0) is
+    [cls + pos[0], pos[1:]] for every image of the batch, pos the host routine's table (for a grid0 x grid0 grid of
+    non-square pixels, which the model's own forward resamples, its numpy restatement)."""
     model = _model()
     lib = load_pkg("_lib").load()
     vit = load_pkg("vit")
@@ -136,15 +174,10 @@ def test_positional_tables_match_the_host_routine(cuda):
     grids = [(a, b) for a in range(1, 65) for b in range(1, 65)]
     st = torch.cuda.current_stream().cuda_stream
 
-    def host(g):
-        out = torch.empty(g[0] * g[1] + 1, model.dim)
-        assert lib.dss_pos_embed_interp_host(src.data_ptr(), 14, model.dim, g[0], g[1], out.data_ptr()) == 0
-        return out
-
     with ThreadPoolExecutor(8) as pool:
         for c0 in range(0, len(grids), 256):
             chunk = grids[c0:c0 + 256]
-            want = list(pool.map(host, chunk))
+            want = list(pool.map(lambda g: _host_table(lib, src, 14, *g), chunk))
             dims = torch.tensor([[16 * a, 16 * b] for a, b in chunk], dtype=torch.int32)
             B = len(chunk)
             ws = torch.empty(lib.dss_vit_ragged_workspace_bytes(model._h, dims.data_ptr(), B, 0), dtype=torch.uint8,
@@ -167,22 +200,31 @@ def test_positional_tables_match_the_host_routine(cuda):
         got = got.cpu()
         assert torch.equal(got[197:], src)
         assert torch.equal(got[:197], src) == (mode == 0)
+        assert torch.equal(got[:197], src if mode == 0 else _resampled(src, 14, 14, 14))
         assert torch.equal(got[0], src[0])
 
-
-def test_positional_cache_untouched(cuda):
-    vit = load_pkg("vit")
-    lib = load_pkg("_lib").load()
-    model = vit.DinoViT("dino_vits16", vit.random_state_dict("dino_vits16", 0), device="cuda")
-    assert lib.dss_vit_pos_cache_entries(model._h) == 0
-    shapes = [(16 * (1 + i % 9), 16 * (1 + i % 11)) for i in range(80)]
-    model.forward_k_ragged(_images(shapes))
-    model.forward_cls_ragged(_images(shapes))
-    assert lib.dss_vit_pos_cache_entries(model._h) == 0
-    model.forward_k(_images([(64, 48)])[0][None])
-    assert lib.dss_vit_pos_cache_entries(model._h) == 1
-    model.forward_k_ragged(_images([(96, 96), (64, 48)]))
-    assert lib.dss_vit_pos_cache_entries(model._h) == 1
+    for name in ("dino_vits16", "dino_vitb8"):
+        sd = vit.random_state_dict(name, 0)
+        sd["patch_embed.proj.weight"].zero_()
+        sd["patch_embed.proj.bias"].zero_()
+        m = vit.DinoViT(name, sd, device="cuda")
+        P, g = m.patch_size, vit.TRAIN_IMG // m.patch_size
+        src = sd["pos_embed"].reshape(g * g + 1, m.dim).contiguous()
+        cls = sd["cls_token"].reshape(m.dim)
+        assert torch.equal(_resampled(src, g, g - 1, g + 1), _host_table(lib, src, g, g - 1, g + 1))
+        grids = [(1, 1), (1, 2), (1, g), (1, 3 * g), (2, 1), (g, 1), (3 * g, 1), (g - 1, g - 1), (g, g),
+                 (g + 1, g + 1), (g - 1, g), (g, g + 1), (g + 1, g), (5, 9)]
+        # non-square pixels on square grids: grid0 (resampled, unlike the patch-grid rule) and grid0 - 1
+        sizes = [(P * a, P * b) for a, b in grids] + [(P * g, P * g + P // 2), (P * g + P - 1, P * g),
+                                                      (P * (g - 1), P * (g - 1) + 3)]
+        for H, W in sizes:
+            Hp, Wp = H // P, W // P
+            want = _resampled(src, g, g, g) if (Hp, Wp) == (g, g) and H != W else _host_table(lib, src, g, Hp, Wp)
+            img = torch.randint(0, 256, (3, H, W, 3), dtype=torch.uint8, generator=torch.Generator().manual_seed(H * W))
+            got = m.forward_tokens(img.cuda(), 0).cpu()   # the 1 x 1 grid: B = 3 images of T = 2 rows
+            for b in range(3):
+                assert torch.equal(got[b, 0], cls + want[0]), (name, H, W, b)
+                assert torch.equal(got[b, 1:], want[1:]), (name, H, W, b)
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)

@@ -161,8 +161,8 @@ POS_SIZES_8 = [(224, 231), (224, 224), (8, 640), (640, 15), (216, 216), (232, 23
 @pytest.mark.parametrize("name,sizes", [("dino_vits16", POS_SIZES_16), ("dino_vitb8", POS_SIZES_8)])
 def test_positional_embedding_of_uncropped_inputs(cuda, name, sizes):
     """Zero patch-embedding weight and bias: forward_tokens(img, 0) = [cls + pos[0], pos[1:]] in fp32, exactly the
-    tokens upstream prepare_tokens builds before the first block. Sizes repeat in the list, so the handle's positional
-    cache must hand each call the entry its own pixel sizes need."""
+    tokens upstream prepare_tokens builds before the first block. Sizes repeat in the list, so each call must get the
+    table its own pixel sizes need, whatever the calls before it."""
     from oracle import dino_vit
     vit = load_pkg("vit")
     ref = dino_vit.build(name, seed=11)

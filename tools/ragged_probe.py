@@ -119,7 +119,7 @@ def measure(model, shapes, cls, reps):
     batches = grouped_batches(shapes)
     grouped = lambda: run_grouped(model, ims, batches, cls)
     ragged = lambda: run_ragged(model, packed, dims, offsets, cls)
-    og, _ = timed(grouped)   # warm-up: every shape, the tensor maps, the positional cache
+    og, _ = timed(grouped)   # warm-up: every shape
     orr, _ = timed(ragged)
     tg, tr = [], []
     for _ in range(reps):
