@@ -9,7 +9,9 @@
 //
 // attention_wgmma_kernel (DSS_VIT_PRECISION_FP16): Q / K / V come straight out of the packed qkv activations [B*T, 3d]
 // (box 64 x 128, 128 B swizzle); 128-key tiles, S by wgmma m64 x 128 x 16 (x4), PV by m64 x 64 x 16 (x8); two CTAs per
-// SM. The output leaves through the (then free) Q tile with one 3-D TMA store (rows past T clipped per image).
+// SM. The output leaves through the (then free) Q tile with one 3-D TMA store (rows past T clipped per image). Padding
+// is not computed: an image's last key tile runs on the narrowest wgmma N of 8, 16, 32, 64, 96, 128 that covers its
+// keys, and in an image's last query tile with at most 64 rows only warp group 0 runs.
 //
 // attention_split_kernel (DSS_VIT_PRECISION_FP32): fp32-equivalent accuracy on the fp16 tensor cores. Operands come
 // from qkv_split_kernel (vit_kernels.cu), per head 192 columns of [B*T, 9d]:
@@ -23,23 +25,25 @@
 // GEMM's A operand and is stored straight from registers (rows past T skipped).
 #include <math.h>
 
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace dss {
 
 // mbarriers of an attention CTA: q_full (the Q tile landed) and, per stage s of the K/V ring, kv_full (the stage
-// landed) and kv_empty (both warp groups are done with it)
+// landed) and kv_empty (every warp group that runs the key loop is done with it)
 template <int STAGES>
 struct KvRing {
   uint32_t bar0;
   __device__ __forceinline__ uint32_t q_full() const { return bar0; }
   __device__ __forceinline__ uint32_t full(int s) const { return bar0 + 8u * (1 + s); }
   __device__ __forceinline__ uint32_t empty(int s) const { return bar0 + 8u * (1 + STAGES + s); }
-  __device__ __forceinline__ void init() const {
+  __device__ __forceinline__ void init(uint32_t groups) const {
     mbar_init(q_full(), 1);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full(s), 1);
-      mbar_init(empty(s), 2);   // one arrival per warp group
+      mbar_init(empty(s), groups);   // one arrival per warp group in the key loop
     }
     mbar_fence_init();
   }
@@ -47,7 +51,8 @@ struct KvRing {
     mbar_wait(full(j % STAGES), (j / STAGES) & 1);
     __syncwarp();   // wgmma is warp-aligned: reconverge after the per-thread barrier spin / thread 0's refill
   }
-  // this warp group is done with K_j / V_j; thread 0 refills the slot with tile j + STAGES once both groups are
+  // this warp group is done with K_j / V_j; thread 0 refills the slot with tile j + STAGES once every group in the key
+  // loop is
   template <typename Load>
   __device__ __forceinline__ void release(int j, int nt, Load&& load_kv) const {
     const int s = j % STAGES;
@@ -172,6 +177,8 @@ __device__ __forceinline__ void attention_wgmma_tile(const CUtensorMap& tmQKV, c
   const int T = loc.T;
   const int nt = (T + FA_BN - 1) / FA_BN;
   const int row0 = loc.row0();   // first row of this image in [rows, 3d]
+  // a tile with at most 64 query rows (an image's last) leaves warp group 1 without rows: it skips the key loop
+  const int groups = q0 + 64 >= T ? 1 : 2;
 
   auto load_kv = [&](int j) {
     const int s = j % FA_KV_STAGES;
@@ -182,7 +189,7 @@ __device__ __forceinline__ void attention_wgmma_tile(const CUtensorMap& tmQKV, c
   if (tid == 0) {
     tma_prefetch_desc(&tmQKV);
     tma_prefetch_desc(&tmO);
-    ring.init();
+    ring.init(groups);
     mbar_arrive_expect_tx(ring.q_full(), FA_TILE);
     tma_load_2d(sQ, &tmQKV, ring.q_full(), h * FA_D, row0 + q0);
     for (int j = 0; j < FA_KV_STAGES && j < nt; ++j) load_kv(j);
@@ -195,39 +202,66 @@ __device__ __forceinline__ void attention_wgmma_tile(const CUtensorMap& tmQKV, c
   float o[32];
 #pragma unroll
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
-  const uint64_t qdesc = wgmma_desc_sw128(sQ + wg * 64 * 128);
-  mbar_wait(ring.q_full(), 0);
-  __syncwarp();
+  const uint64_t qdesc0 = wgmma_desc_sw128(sQ + wg * 64 * 128);
 
-  for (int j = 0; j < nt; ++j) {
+  // Key tile j with NB 8-key blocks (keys 128 j + [0, 8 NB)): S on wgmma m64 x 8NB x 16 (x4), the softmax, then
+  // O += P V over ceil(NB / 2) 16-key steps. A narrower tile gives the same bits as the full one: each S element is the
+  // same four k16 products, and the keys it drops are past T, so they would only add -inf to the row max, 0 to the row
+  // sum and exact zeros (P = 0 times finite V rows) to O.
+  auto key_tile = [&](int j, auto nb) {
+    constexpr int NB = decltype(nb)::value, KS = (NB + 1) / 2;
     const int s = j % FA_KV_STAGES;
     ring.wait(j);
-    float sacc[64];
+    float sacc[4 * NB];
+    // opaque per tile, so that the compiler does not hoist the k-step descriptors out of the key loop (and spill them)
+    uint64_t qdesc = qdesc0;
+    asm volatile("" : "+l"(qdesc));
     const uint64_t kdesc = wgmma_desc_sw128(sK + s * FA_TILE);
     wgmma_fence();
 #pragma unroll
-    for (int k = 0; k < FA_D / 16; ++k) wgmma_m64n128_ss(sacc, qdesc + 2u * k, kdesc + 2u * k, k != 0 ? 1u : 0u);
+    for (int k = 0; k < FA_D / 16; ++k) Wgmma<8 * NB>::ss(sacc, qdesc + 2u * k, kdesc + 2u * k, k != 0 ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(sacc);
     // accumulator layout of two adjacent 8-key blocks == register A-operand layout of one 16-key step
-    uint32_t pf[8][4];
-    softmax_tile<16>(sacc, o, m_run, l_run, j * FA_BN, T, fc, [&](int i, float p0, float p1, float p2, float p3) {
+    uint32_t pf[KS][4];
+    if constexpr (NB % 2) pf[KS - 1][2] = pf[KS - 1][3] = 0u;   // the missing block of the last step: P = 0
+    softmax_tile<NB>(sacc, o, m_run, l_run, j * FA_BN, T, fc, [&](int i, float p0, float p1, float p2, float p3) {
       pf[i >> 1][(i & 1) * 2 + 0] = pack_half2(p0, p1);
       pf[i >> 1][(i & 1) * 2 + 1] = pack_half2(p2, p3);
     });
     const uint64_t vdesc = wgmma_desc_sw128(sV + s * FA_TILE);   // +16 key rows = +2048 B
     wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < FA_BN / 16; ++ks) wgmma_m64n64_rs_tb(o, pf[ks], vdesc + 128u * ks);
+    for (int ks = 0; ks < KS; ++ks) wgmma_m64n64_rs_tb(o, pf[ks], vdesc + 128u * ks);
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_acc(o);
     ring.release(j, nt, load_kv);
+  };
+  if (wg < groups) {
+    mbar_wait(ring.q_full(), 0);
+    __syncwarp();
+    for (int j = 0; j < nt - 1; ++j) key_tile(j, std::integral_constant<int, 16>{});
+    // the last key tile holds T - 128 (nt - 1) keys: the narrowest of 8, 16, 32, 64, 96 or 128 keys that covers them
+    const int r = T - FA_BN * (nt - 1);
+    if (r <= 8)
+      key_tile(nt - 1, std::integral_constant<int, 1>{});
+    else if (r <= 16)
+      key_tile(nt - 1, std::integral_constant<int, 2>{});
+    else if (r <= 32)
+      key_tile(nt - 1, std::integral_constant<int, 4>{});
+    else if (r <= 64)
+      key_tile(nt - 1, std::integral_constant<int, 8>{});
+    else if (r <= 96)
+      key_tile(nt - 1, std::integral_constant<int, 12>{});
+    else
+      key_tile(nt - 1, std::integral_constant<int, 16>{});
   }
 
   // finalise: normalise, fp16 into this group's half of the Q tile (swizzled as the output box), one TMA store of the
-  // 128 x 64 box
+  // 128 x 64 box. A group without rows stores nothing: the ragged partial tile skips rows >= T, and the uniform box
+  // store clips them.
   softmax_rowsum(l_run);
   const float inv0 = 1.0f / l_run[0], inv1 = 1.0f / l_run[1];
   const int r0 = 64 * wg + 16 * wi + (lane >> 2);
@@ -245,16 +279,18 @@ __device__ __forceinline__ void attention_wgmma_tile(const CUtensorMap& tmQKV, c
       return;
     }
   }
+  if (wg < groups) {
 #pragma unroll
-  for (int i = 0; i < 8; ++i) {
+    for (int i = 0; i < 8; ++i) {
 #pragma unroll
-    for (int hh = 0; hh < 2; ++hh) {
-      const int row = r0 + 8 * hh;
-      const float inv = hh ? inv1 : inv0;
-      const uint32_t addr = sw128_addr(sQ, row, i) + (lane & 3) * 4;
-      asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr),
-                   "r"(pack_half2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv))
-                   : "memory");
+      for (int hh = 0; hh < 2; ++hh) {
+        const int row = r0 + 8 * hh;
+        const float inv = hh ? inv1 : inv0;
+        const uint32_t addr = sw128_addr(sQ, row, i) + (lane & 3) * 4;
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr),
+                     "r"(pack_half2(o[4 * i + 2 * hh] * inv, o[4 * i + 2 * hh + 1] * inv))
+                     : "memory");
+      }
     }
   }
   fence_proxy_async_smem();
@@ -317,7 +353,7 @@ __device__ __forceinline__ void attention_split_tile(const CUtensorMap& tmQKV, _
   };
   if (tid == 0) {
     tma_prefetch_desc(&tmQKV);
-    ring.init();
+    ring.init(2);
     mbar_arrive_expect_tx(ring.q_full(), AS_Q);
     // Q' group g: rows 0-63 at +0, rows 64-127 at +8 KB, so each group is one 128-row swizzled tile
     for (int g = 0; g < 3; ++g)

@@ -290,6 +290,33 @@ __device__ __forceinline__ uint32_t sw128_addr(uint32_t base, int row, int chunk
 // d[i .. i+7] as read-write asm operands
 #define DSS_ACC8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), \
                     "+f"(d[i + 6]), "+f"(d[i + 7])
+// D[64 x 8] (+)= A(smem) * B(smem), both K-major
+__device__ __forceinline__ void wgmma_m64n8_ss(float (&d)[4], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %6, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n8k16.f32.f16.f16 {%0, %1, %2, %3}, "
+      "%4, %5, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x 16] (+)= A(smem) * B(smem), both K-major
+__device__ __forceinline__ void wgmma_m64n16_ss(float (&d)[8], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7}, "
+      "%8, %9, p, 1, 1, 0, 0;\n\t}"
+      : DSS_ACC8(0)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x 32] (+)= A(smem) * B(smem), both K-major
+__device__ __forceinline__ void wgmma_m64n32_ss(float (&d)[16], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, "
+      "%16, %17, p, 1, 1, 0, 0;\n\t}"
+      : DSS_ACC8(0), DSS_ACC8(8)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
 // D[64 x 64] (+)= A(smem) * B(smem), both K-major
 __device__ __forceinline__ void wgmma_m64n64_ss(float (&d)[32], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
@@ -297,6 +324,15 @@ __device__ __forceinline__ void wgmma_m64n64_ss(float (&d)[32], uint64_t adesc, 
       "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
       "%32, %33, p, 1, 1, 0, 0;\n\t}"
       : DSS_ACC8(0), DSS_ACC8(8), DSS_ACC8(16), DSS_ACC8(24)
+      : "l"(adesc), "l"(bdesc), "r"(accumulate));
+}
+// D[64 x 96] (+)= A(smem) * B(smem), both K-major
+__device__ __forceinline__ void wgmma_m64n96_ss(float (&d)[48], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %50, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47}, "
+      "%48, %49, p, 1, 1, 0, 0;\n\t}"
+      : DSS_ACC8(0), DSS_ACC8(8), DSS_ACC8(16), DSS_ACC8(24), DSS_ACC8(32), DSS_ACC8(40)
       : "l"(adesc), "l"(bdesc), "r"(accumulate));
 }
 // D[64 x 128] (+)= A(smem) * B(smem), both K-major
@@ -336,6 +372,11 @@ __device__ __forceinline__ void wgmma_m64n64_rs_tb(float (&d)[32], const uint32_
 }
 #undef DSS_ACC8
 template <int N> struct Wgmma;
+template <> struct Wgmma<8> { static __device__ __forceinline__ void ss(float (&d)[4], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n8_ss(d, a, b, acc); } };
+template <> struct Wgmma<16> { static __device__ __forceinline__ void ss(float (&d)[8], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n16_ss(d, a, b, acc); } };
+template <> struct Wgmma<32> { static __device__ __forceinline__ void ss(float (&d)[16], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n32_ss(d, a, b, acc); } };
+template <> struct Wgmma<64> { static __device__ __forceinline__ void ss(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n64_ss(d, a, b, acc); } };
+template <> struct Wgmma<96> { static __device__ __forceinline__ void ss(float (&d)[48], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n96_ss(d, a, b, acc); } };
 template <> struct Wgmma<128> { static __device__ __forceinline__ void ss(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n128_ss(d, a, b, acc); } };
 template <> struct Wgmma<192> { static __device__ __forceinline__ void ss(float (&d)[96], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n192_ss(d, a, b, acc); } };
 template <> struct Wgmma<256> { static __device__ __forceinline__ void ss(float (&d)[128], uint64_t a, uint64_t b, uint32_t acc) { wgmma_m64n256_ss(d, a, b, acc); } };
