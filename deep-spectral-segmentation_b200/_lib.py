@@ -54,6 +54,8 @@ PROTOTYPES = {
     "dss_vit_forward_k_ragged": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                          c_void_p]),
     "dss_vit_forward_cls_ragged": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "dss_vit_forward_last_ragged": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p,
+                                            c_void_p, c_size_t, c_void_p]),
     "dss_vit_pos_embed_ragged": (c_int, [c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "dss_pos_embed_interp_host": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "dss_op_gemm_f16": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int,
@@ -114,6 +116,12 @@ PROTOTYPES = {
     "dss_lost_boxes": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p,
                                c_void_p, c_void_p, c_size_t, c_void_p]),
     "dss_dinoseg_boxes": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "dss_lost_ragged_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "dss_lost_boxes_ragged": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p,
+                                      c_void_p, c_size_t, c_void_p]),
+    "dss_dinoseg_ragged_workspace_bytes": (c_size_t, [c_int]),
+    "dss_dinoseg_boxes_ragged": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_int, c_void_p, c_void_p,
+                                         c_void_p, c_size_t, c_void_p]),
     "dss_vit_forward_last_workspace_bytes": (c_size_t, [c_void_p, c_int, c_int, c_int, c_int]),
     "dss_vit_forward_last": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p,
                                      c_size_t, c_void_p]),
@@ -132,7 +140,7 @@ LOC_OK, LOC_NO_GRID, LOC_SEED_IN_BACKGROUND, LOC_EMPTY_COMPONENT = range(4)
 SEGEVAL_SEMANTIC, SEGEVAL_BINARY, SEGEVAL_FIELDS = 0, 1, 13
 DSS_ERR_BAD_ARG, DSS_ERR_UNSUPPORTED = -1, -4
 VIT_PRECISION = {"fp16": 0, "fp32": 1}   # DSS_VIT_PRECISION_FP16 / _FP32
-VIT_RAGGED_K, VIT_RAGGED_CLS = 0, 1          # DSS_VIT_RAGGED_K / _CLS
+VIT_RAGGED_K, VIT_RAGGED_CLS, VIT_RAGGED_PAD = 0, 1, 3   # DSS_VIT_RAGGED_K / _CLS / _PAD
 
 _lib = None
 

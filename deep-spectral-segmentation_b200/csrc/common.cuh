@@ -86,8 +86,38 @@ __device__ __forceinline__ int ragged_find(int B, long long x, Off&& off) {
   }
   return lo;
 }
+
+// Where a batch's token rows lie, for the kernels outside attention that see image boundaries (attention.cu has its
+// own tile locators): row0(b) is image b's first (CLS) row of the residual stream, tokens(b) its token count, and at(r)
+// names positional-table row r: token t of an image with an Hp x Wp patch grid, stored = the identity rule keeps the
+// stored grid.
+struct PosRow { int t, Hp, Wp, stored; };
+// A uniform batch: image b's T = Hp Wp + 1 rows start at b T; the positional table is the [T, d] one all images share.
+struct UniformRows {
+  int T, Hp, Wp, stored;
+  __device__ __forceinline__ long long row0(int b) const { return (long long)b * T; }
+  __device__ __forceinline__ int tokens(int) const { return T; }
+  __device__ __forceinline__ PosRow at(long long r) const { return {(int)r, Hp, Wp, stored}; }
+};
+// A ragged batch: image b's rows start at imgs[b].tok_off; the positional table is laid out like the residual stream.
+struct RaggedRows {
+  const RaggedImage* imgs;
+  int B;
+  __device__ __forceinline__ long long row0(int b) const { return imgs[b].tok_off; }
+  __device__ __forceinline__ int tokens(int b) const { return imgs[b].Hp * imgs[b].Wp + 1; }
+  __device__ __forceinline__ PosRow at(long long r) const {
+    const RaggedImage im = imgs[ragged_find(B, r, [&](int j) { return imgs[j].tok_off; })];
+    return {(int)(r - im.tok_off), im.Hp, im.Wp, im.stored};
+  }
+};
+
+// pad: the zero-padded ceil grid (imgs[b].Hp = ceil(H / P)) instead of the crop
 int launch_im2col_ragged(const uint8_t* img, void* patches, const RaggedImage* imgs, int B, long long n_patches, int P,
-                         bool split, cudaStream_t st);
+                         bool split, bool pad, cudaStream_t st);
+// The CLS attention rows of a ragged batch into out [B, heads, n_out]: image b's N_b = Hp Wp entries, then exact zeros
+// up to n_out (>= every N_b)
+int launch_cls_attention_ragged(const void* qkv, bool f32_keys, const RaggedImage* imgs, int B, int n_out, int heads,
+                                float* out, cudaStream_t st);
 // tile_prefix [B + 1]: image b's 128-query tiles are CTAs [tile_prefix[b], tile_prefix[b + 1])
 int launch_attention_tc_ragged(const void* qkv, void* out, const RaggedImage* imgs, const int* tile_prefix, int B,
                                long long M, int tiles, int heads, cudaStream_t st);

@@ -9,6 +9,7 @@
 // integer atomics, so the result does not depend on thread scheduling.
 #include <stdint.h>
 
+#include <algorithm>
 #include <vector>
 
 #include "common.cuh"
@@ -126,6 +127,14 @@ __device__ int cc_largest(const int* parent, const int* size, int n, int skip, u
 
 struct EigsegImage { int P, gh, gw, H, W, ok; };
 
+// One image of LOST or DINO-seg: N = gh gw cells, n2 = next_pow2(N) sort keys, un-padded size H x W (LOST). A uniform
+// batch passes one descriptor by value (imgs == NULL); a ragged batch a table of B. Image b's rows start at row
+// b * pitch of the inputs (pitch = N, or n_max of a padded ragged batch).
+struct LocImage { int N, n2, gh, gw, H, W; };
+__device__ __forceinline__ LocImage loc_image(const LocImage* imgs, const LocImage& uni, int b) {
+  return imgs ? imgs[b] : uni;
+}
+
 // Shared memory of the box kernels: parent + size (or the sort keys, which they replace), the mask, LOST's list
 __device__ __forceinline__ void loc_carve(int n, int n2, unsigned char* smem, unsigned long long** keys, int** parent,
                                           int** size, uint8_t** mask, int** list) {
@@ -191,32 +200,37 @@ eigseg_box_kernel(const float* __restrict__ evecs, int K, int N, int which, cons
 }
 
 // ---- b) LOST (lost + patch_scoring + detect_box, object_discovery.py:129-227)
-// degree[b, i] = #{j != i : A[b, i, j] > 0}: one warp per row
+// degree[b, i] = #{j != i : A[b, i, j] > 0} over image b's N cells: one warp per row
 __global__ void __launch_bounds__(256)
-lost_degree_kernel(const float* __restrict__ A, int N, int ldw, int* __restrict__ degree) {
+lost_degree_kernel(const float* __restrict__ A, const LocImage* __restrict__ imgs, LocImage uni, int pitch, int ldw,
+                   int* __restrict__ degree) {
   const int b = blockIdx.y, row = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  const int N = loc_image(imgs, uni, b).N;
   if (row >= N) return;
-  const float* a = A + ((long long)b * N + row) * ldw;
+  const float* a = A + ((long long)b * pitch + row) * ldw;
   int c = 0;
   for (int j = lane; j < N; j += 32) c += (j != row) && (a[j] > 0.f);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if (lane == 0) degree[(long long)b * N + row] = c;
+  if (lane == 0) degree[(long long)b * pitch + row] = c;
 }
 
 __global__ void __launch_bounds__(LOC_THREADS)
-lost_box_kernel(const float* __restrict__ A, int N, int n2, int ldw, const int* __restrict__ degree, int gh, int gw, int H,
-                int W, int P, int k_patches, int* __restrict__ boxes, int* __restrict__ seeds, int* __restrict__ status) {
+lost_box_kernel(const float* __restrict__ A, const LocImage* __restrict__ imgs, LocImage uni, int pitch, int ldw,
+                const int* __restrict__ degree, int P, int k_patches, int* __restrict__ boxes, int* __restrict__ seeds,
+                int* __restrict__ status) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ int sbox[4];
   __shared__ int snsim;
   const int b = blockIdx.x;
+  const LocImage im = loc_image(imgs, uni, b);
+  const int N = im.N, n2 = im.n2, gh = im.gh, gw = im.gw, H = im.H, W = im.W;
   unsigned long long* keys; int *parent, *size, *list; uint8_t* mask;
   loc_carve(N, n2, smem, &keys, &parent, &size, &mask, &list);
-  const float* Ab = A + (long long)b * N * ldw;
+  const float* Ab = A + (long long)b * pitch * ldw;
   // ascending degree, ties by patch index (a stable order; torch.argsort(stable=False) leaves ties unspecified)
   for (int i = threadIdx.x; i < n2; i += blockDim.x)
-    keys[i] = i < N ? ((unsigned long long)degree[(long long)b * N + i] << 32) | (unsigned)i : ~0ull;
+    keys[i] = i < N ? ((unsigned long long)degree[(long long)b * pitch + i] << 32) | (unsigned)i : ~0ull;
   __syncthreads();
   bitonic_sort_u64(keys, n2);
   const int seed = (int)(keys[0] & 0xffffffffu);
@@ -275,8 +289,8 @@ __device__ __forceinline__ unsigned f32_order_key(float x) {
 }
 
 __global__ void __launch_bounds__(LOC_THREADS)
-dinoseg_box_kernel(const float* __restrict__ attn, int heads, int N, int n2, int head, int gh, int gw, int P,
-                   int* __restrict__ boxes, int* __restrict__ status) {
+dinoseg_box_kernel(const float* __restrict__ attn, int heads, const LocImage* __restrict__ imgs, LocImage uni, int pitch,
+                   int head, int P, int* __restrict__ boxes, int* __restrict__ status) {
   extern __shared__ __align__(16) unsigned char smem[];
   __shared__ int sbox[4];
   __shared__ int smaxroot, scomp;
@@ -284,9 +298,11 @@ dinoseg_box_kernel(const float* __restrict__ attn, int heads, int N, int n2, int
   __shared__ unsigned long long sbest;
   __shared__ double red[LOC_THREADS / 32];
   const int b = blockIdx.x;
+  const LocImage im = loc_image(imgs, uni, b);
+  const int N = im.N, n2 = im.n2, gh = im.gh, gw = im.gw;
   unsigned long long* keys; int *parent, *size, *list; uint8_t* mask;
   loc_carve(N, n2, smem, &keys, &parent, &size, &mask, &list);
-  const float* a = attn + ((long long)b * heads + head) * N;
+  const float* a = attn + ((long long)b * heads + head) * pitch;
   // torch.sort ascending (ties by index), val /= sum(val), cumsum, keep where the cumulative mass > 1 - 0.6
   double part = 0.0;
   for (int i = threadIdx.x; i < n2; i += blockDim.x) {
@@ -360,6 +376,62 @@ static EigsegImage eigseg_grid(int N, int H, int W) {
   return e;
 }
 
+static LocImage loc_image_host(int gh, int gw, int H, int W) {
+  const int N = gh * gw;
+  return {N, next_pow2(N), gh, gw, H, W};
+}
+
+// LOST over B images (imgs: device table, or NULL and every image `uni`); shared memory for max_n cells
+static int launch_lost(const float* A, int B, int pitch, int ldw, const LocImage* imgs, const LocImage& uni, int max_n,
+                       int P, int k_patches, int* boxes, int* seeds, int* status, int* degree, cudaStream_t st) {
+  {
+    LaunchScope scope(st, KC_MISC);
+    lost_degree_kernel<<<dim3(cdiv(max_n, 8), B), 256, 0, st>>>(A, imgs, uni, pitch, ldw, degree);
+    DSS_CHECK_CUDA(cudaGetLastError());
+  }
+  const size_t smem = loc_smem_bytes(max_n, next_pow2(max_n), true);
+  int rc;
+  if ((rc = loc_set_smem((const void*)lost_box_kernel, smem))) return rc;
+  LaunchScope scope(st, KC_MISC);
+  lost_box_kernel<<<B, LOC_THREADS, smem, st>>>(A, imgs, uni, pitch, ldw, degree, P, k_patches, boxes, seeds, status);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
+static int launch_dinoseg(const float* attn, int B, int heads, int pitch, int head, const LocImage* imgs,
+                          const LocImage& uni, int max_n, int P, int* boxes, int* status, cudaStream_t st) {
+  const size_t smem = loc_smem_bytes(max_n, next_pow2(max_n), false);
+  int rc;
+  if ((rc = loc_set_smem((const void*)dinoseg_box_kernel, smem))) return rc;
+  LaunchScope scope(st, KC_MISC);
+  dinoseg_box_kernel<<<B, LOC_THREADS, smem, st>>>(attn, heads, imgs, uni, pitch, head, P, boxes, status);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
+// The descriptors of a ragged batch from dims_host [B, per] = {gh, gw[, H, W]}: every grid non-empty, at most n_max
+// and LOC_MAX_CELLS cells. Returns the largest N_b in *max_n.
+static int ragged_loc_images(const char* name, const int* dims, int B, int per, int n_max, std::vector<LocImage>& imgs,
+                             int* max_n) {
+  imgs.resize(B);
+  *max_n = 0;
+  for (int b = 0; b < B; ++b) {
+    const int* d = dims + (size_t)b * per;
+    const int gh = d[0], gw = d[1], H = per == 4 ? d[2] : 1, W = per == 4 ? d[3] : 1;
+    DSS_REQUIRE(gh > 0 && gw > 0 && H > 0 && W > 0, "%s: image %d has grid %dx%d, size %dx%d", name, b, gh, gw, H, W);
+    const long long N = (long long)gh * gw;
+    DSS_REQUIRE(N <= n_max, "%s: image %d's %dx%d grid has more than n_max = %d cells", name, b, gh, gw, n_max);
+    if (N > LOC_MAX_CELLS) {
+      set_error("%s: image %d's %lld cells exceed the %d (128 x 128) a CTA holds in shared memory", name, b, N,
+                LOC_MAX_CELLS);
+      return DSS_ERR_UNSUPPORTED;
+    }
+    imgs[b] = loc_image_host(gh, gw, H, W);
+    *max_n = std::max(*max_n, (int)N);
+  }
+  return DSS_OK;
+}
+
 }  // namespace dss
 
 using namespace dss;
@@ -419,22 +491,35 @@ extern "C" int dss_lost_boxes(const float* A, int B, int N, int ldw, int grid_h,
     set_error("lost_boxes: workspace too small (%zu < %zu)", ws_bytes, dss_lost_workspace_bytes(B, N));
     return DSS_ERR_WORKSPACE;
   }
-  cudaStream_t st = static_cast<cudaStream_t>(stream);
-  int* degree = reinterpret_cast<int*>(ws);
-  {
-    LaunchScope scope(st, KC_MISC);
-    lost_degree_kernel<<<dim3(cdiv(N, 8), B), 256, 0, st>>>(A, N, ldw, degree);
-    DSS_CHECK_CUDA(cudaGetLastError());
+  return launch_lost(A, B, N, ldw, nullptr, loc_image_host(grid_h, grid_w, H, W), N, P, k_patches, boxes, seeds, status,
+                     reinterpret_cast<int*>(ws), static_cast<cudaStream_t>(stream));
+}
+
+extern "C" size_t dss_lost_ragged_workspace_bytes(int B, int n_max) {
+  return (B > 0 && n_max > 0) ? align_up((size_t)B * n_max * sizeof(int), 256) + align_up(B * sizeof(LocImage), 256)
+                              : 0;
+}
+
+extern "C" int dss_lost_boxes_ragged(const float* A, int B, int n_max, int ldw, const int* dims_host, int P,
+                                     int k_patches, int* boxes, int* seeds, int* status, void* ws, size_t ws_bytes,
+                                     dss_stream_t stream) {
+  DSS_REQUIRE(A && dims_host && boxes && status && ws, "lost_boxes_ragged: null pointer");
+  DSS_REQUIRE(B > 0 && n_max > 0 && ldw >= n_max, "lost_boxes_ragged: bad shape (B=%d n_max=%d ldw=%d)", B, n_max, ldw);
+  DSS_REQUIRE(P > 0 && k_patches > 0, "lost_boxes_ragged: bad patch / k_patches");
+  std::vector<LocImage> imgs;
+  int max_n, rc;
+  if ((rc = ragged_loc_images("lost_boxes_ragged", dims_host, B, 4, n_max, imgs, &max_n))) return rc;
+  const size_t need = dss_lost_ragged_workspace_bytes(B, n_max), deg_bytes = align_up((size_t)B * n_max * 4, 256);
+  if (ws_bytes < need) {
+    set_error("lost_boxes_ragged: workspace too small (%zu < %zu)", ws_bytes, need);
+    return DSS_ERR_WORKSPACE;
   }
-  const int n2 = next_pow2(N);
-  const size_t smem = loc_smem_bytes(N, n2, true);
-  int rc;
-  if ((rc = loc_set_smem((const void*)lost_box_kernel, smem))) return rc;
-  LaunchScope scope(st, KC_MISC);
-  lost_box_kernel<<<B, LOC_THREADS, smem, st>>>(A, N, n2, ldw, degree, grid_h, grid_w, H, W, P, k_patches, boxes, seeds,
-                                                status);
-  DSS_CHECK_CUDA(cudaGetLastError());
-  return DSS_OK;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  uint8_t* tab = reinterpret_cast<uint8_t*>(ws) + deg_bytes;
+  // pageable source: the copy is staged before cudaMemcpyAsync returns, so `imgs` may go out of scope
+  DSS_CHECK_CUDA(cudaMemcpyAsync(tab, imgs.data(), (size_t)B * sizeof(LocImage), cudaMemcpyHostToDevice, st));
+  return launch_lost(A, B, n_max, ldw, reinterpret_cast<const LocImage*>(tab), imgs[0], max_n, P, k_patches, boxes,
+                     seeds, status, reinterpret_cast<int*>(ws), st);
 }
 
 extern "C" int dss_dinoseg_boxes(const float* cls_attn, int B, int heads, int N, int head, int grid_h, int grid_w, int P,
@@ -448,13 +533,31 @@ extern "C" int dss_dinoseg_boxes(const float* cls_attn, int B, int heads, int N,
     set_error("dinoseg_boxes: %d cells exceed the %d (128 x 128) a CTA holds in shared memory", N, LOC_MAX_CELLS);
     return DSS_ERR_UNSUPPORTED;
   }
+  return launch_dinoseg(cls_attn, B, heads, N, head, nullptr, loc_image_host(grid_h, grid_w, 1, 1), N, P, boxes, status,
+                        static_cast<cudaStream_t>(stream));
+}
+
+extern "C" size_t dss_dinoseg_ragged_workspace_bytes(int B) {
+  return B > 0 ? align_up((size_t)B * sizeof(LocImage), 256) : 0;
+}
+
+extern "C" int dss_dinoseg_boxes_ragged(const float* cls_attn, int B, int heads, int n_max, int head,
+                                        const int* dims_host, int P, int* boxes, int* status, void* ws, size_t ws_bytes,
+                                        dss_stream_t stream) {
+  DSS_REQUIRE(cls_attn && dims_host && boxes && status && ws, "dinoseg_boxes_ragged: null pointer");
+  DSS_REQUIRE(B > 0 && heads > 0 && n_max > 0, "dinoseg_boxes_ragged: bad shape (B=%d heads=%d n_max=%d)", B, heads,
+              n_max);
+  DSS_REQUIRE(head >= 0 && head < heads, "dinoseg_boxes_ragged: head %d not in [0, %d)", head, heads);
+  DSS_REQUIRE(P > 0, "dinoseg_boxes_ragged: bad patch size %d", P);
+  std::vector<LocImage> imgs;
+  int max_n, rc;
+  if ((rc = ragged_loc_images("dinoseg_boxes_ragged", dims_host, B, 2, n_max, imgs, &max_n))) return rc;
+  if (ws_bytes < dss_dinoseg_ragged_workspace_bytes(B)) {
+    set_error("dinoseg_boxes_ragged: workspace too small (%zu < %zu)", ws_bytes, dss_dinoseg_ragged_workspace_bytes(B));
+    return DSS_ERR_WORKSPACE;
+  }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const int n2 = next_pow2(N);
-  const size_t smem = loc_smem_bytes(N, n2, false);
-  int rc;
-  if ((rc = loc_set_smem((const void*)dinoseg_box_kernel, smem))) return rc;
-  LaunchScope scope(st, KC_MISC);
-  dinoseg_box_kernel<<<B, LOC_THREADS, smem, st>>>(cls_attn, heads, N, n2, head, grid_h, grid_w, P, boxes, status);
-  DSS_CHECK_CUDA(cudaGetLastError());
-  return DSS_OK;
+  DSS_CHECK_CUDA(cudaMemcpyAsync(ws, imgs.data(), (size_t)B * sizeof(LocImage), cudaMemcpyHostToDevice, st));
+  return launch_dinoseg(cls_attn, B, heads, n_max, head, reinterpret_cast<const LocImage*>(ws), imgs[0], max_n, P, boxes,
+                        status, st);
 }

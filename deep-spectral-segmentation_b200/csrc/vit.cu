@@ -23,27 +23,6 @@
 
 namespace dss {
 
-// Where a batch's token rows lie, for the kernels outside attention that see image boundaries (attention.cu has its
-// own tile locators): row0(b) is image b's first (CLS) row of the residual stream, and at(r) names positional-table
-// row r: token t of an image with an Hp x Wp patch grid, stored = the identity rule keeps the stored grid.
-struct PosRow { int t, Hp, Wp, stored; };
-// A uniform batch: image b's T = Hp Wp + 1 rows start at b T; the positional table is the [T, d] one all images share.
-struct UniformRows {
-  int T, Hp, Wp, stored;
-  __device__ __forceinline__ long long row0(int b) const { return (long long)b * T; }
-  __device__ __forceinline__ PosRow at(long long r) const { return {(int)r, Hp, Wp, stored}; }
-};
-// A ragged batch: image b's rows start at imgs[b].tok_off; the positional table is laid out like the residual stream.
-struct RaggedRows {
-  const RaggedImage* imgs;
-  int B;
-  __device__ __forceinline__ long long row0(int b) const { return imgs[b].tok_off; }
-  __device__ __forceinline__ PosRow at(long long r) const {
-    const RaggedImage im = imgs[ragged_find(B, r, [&](int j) { return imgs[j].tok_off; })];
-    return {(int)(r - im.tok_off), im.Hp, im.Wp, im.stored};
-  }
-};
-
 // y[b, :] = LayerNorm(x[row0(b), :]) * gamma + beta in fp32 (one warp per image): the final norm of the CLS token, read
 // where it lies in the residual stream
 template <typename Loc>
@@ -281,6 +260,7 @@ struct Ragged {
   const int* tile_prefix;         // [B + 1]
   const int* patch_rows;          // [n_patches] token row of each patch row
   const int* k_rows;              // [M] feature row of each token row (-1: CLS)
+  int n_out;                      // feature rows per image of a padded output [B, n_out, d] (0: packed output)
 };
 
 // the positional table (pos_rows rows) and every image's CLS row: pos_cls_kernel over batch `loc`
@@ -322,8 +302,10 @@ static int vit_tail(const dss_vit* h, const float* x, int mode, float* out, int 
 // DSS_VIT_PRECISION_FP32 runs the same sequence on split operands: every GEMM runs the fp16 path's kernel and epilogue
 // at K' = 3 K; the qkv and fc1 GEMMs write fp32 (DSS_EPI_BIAS_F32), which qkv_split_kernel / gelu_split_kernel turn
 // into the next product's split operands.
-// rg: a ragged batch (modes 0 and 2; H, W unused). Only the token embedding, attention, the K projection's CLS drop and
-// the final-norm rows depend on image boundaries; they read rg's tables, every other step is row-wise over M rows.
+// rg: a ragged batch (modes 0, 2 and 3; H, W unused). Only the token embedding, attention, the projection's CLS drop,
+// the CLS attention row and the final-norm rows depend on image boundaries; they read rg's tables, every other step is
+// row-wise over M rows. Mode 3 writes rg's padded layout: out [B, n_out, d] and cls_attn [B, heads, n_out], the rows
+// past an image's N_b exact zeros.
 static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_full, int mode, float* out, void* ws,
                    size_t ws_bytes, cudaStream_t st, int pad = 0, int which = 1, float* cls_attn = nullptr,
                    const Ragged* rg = nullptr) {
@@ -360,7 +342,7 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
 
   // tokens: x[b, 0, :] = cls + pos[0] and the positional table, then x[b, 1+n, :] = patch_embed + pos[1+n]
   if (rg) {
-    if ((rc = launch_im2col_ragged(img, w.patches, rg->imgs, B, n_patches, P, split, st))) return rc;
+    if ((rc = launch_im2col_ragged(img, w.patches, rg->imgs, B, n_patches, P, split, pad, st))) return rc;
     if ((rc = launch_pos_cls(h, RaggedRows{rg->imgs, B}, B, M, w, st))) return rc;
     if ((rc = gemm_f16_tc_rows(tm_patches, h->tm_patch, h->patch_b, w.x, n_patches, d, ks * Kp, DSS_EPI_PATCH_F32,
                                w.pos, rg->patch_rows, st, KC_GEMM_PATCH)))
@@ -412,6 +394,8 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
   if ((rc = launch_layernorm(w.x, bw.ln1_w, bw.ln1_b, w.xn, M, d, c.ln_eps, split, st))) return rc;
   if (out) {   // qkv[b, 1+n, which*d : (which+1)*d] in fp32, CLS rows dropped (which = 1: the K features)
     const CUtensorMap& tm = which == 0 ? bw.tm_q : (which == 1 ? bw.tm_k : bw.tm_v);
+    // the rows of a padded output that no token row maps to
+    if (rg && rg->n_out) DSS_CHECK_CUDA(cudaMemsetAsync(out, 0, (size_t)B * rg->n_out * d * sizeof(float), st));
     rc = rg ? gemm_f16_tc_rows(tm_xn, tm, bw.qkv_b + (size_t)which * d, out, M, d, ks * d, DSS_EPI_DROPCLS_F32, nullptr,
                                rg->k_rows, st, KC_GEMM_KPROJ)
             : gemm_f16_tc(tm_xn, tm, nullptr, bw.qkv_b + (size_t)which * d, out, M, d, ks * d, DSS_EPI_DROPCLS_F32,
@@ -419,16 +403,19 @@ static int vit_run(dss_vit* h, const uint8_t* img, int B, int H, int W, int n_fu
     if (rc) return rc;
   }
   if (cls_attn) {   // the full qkv projection the attention kernels read, then the CLS row of the softmax
-    DSS_REQUIRE(!rg, "vit: no CLS attention output for ragged batches");
     if ((rc = qkv_gemm(bw))) return rc;
-    if ((rc = launch_cls_attention(split ? (const void*)w.f32 : w.qkv, split, B, T, c.heads, cls_attn, st))) return rc;
+    const void* keys = split ? (const void*)w.f32 : w.qkv;
+    rc = rg ? launch_cls_attention_ragged(keys, split, rg->imgs, B, rg->n_out, c.heads, cls_attn, st)
+            : launch_cls_attention(keys, split, B, T, c.heads, cls_attn, st);
+    if (rc) return rc;
   }
   return DSS_OK;
 }
 
 // ---- ragged batches: host plan. Workspace = the forward's buffers (carve, positional tables [M, d] included) | one
 // block of tables (RaggedImage [B], tile_prefix [B + 1], patch_rows [n_patches], k_rows [M]), uploaded with one copy
-// per forward.
+// per forward. Mode DSS_VIT_RAGGED_PAD runs the zero-padded ceil grid of forward_last(pad = 1), so an image may be
+// smaller than one patch; the others crop.
 struct RaggedPlan {
   std::vector<RaggedImage> imgs;
   std::vector<int> tile_prefix, patch_rows, k_rows;
@@ -440,26 +427,38 @@ struct RaggedPlan {
 constexpr int RAGGED_TILE = 128;   // query rows per attention CTA (FA_BM, AS_BM)
 
 // Validates the batch and lays out its workspace; with `tables`, also fills the host tables. mode: DSS_VIT_RAGGED_*.
-static int ragged_plan(const dss_vit* h, const int* dims, int B, int mode, bool tables, RaggedPlan& pl) {
+// n_out > 0: the features go to a padded [B, n_out, d] output (image b's row n at b n_out + n), which must hold every
+// image's N_b rows; 0: packed.
+static int ragged_plan(const dss_vit* h, const int* dims, int B, int mode, int n_out, bool tables, RaggedPlan& pl) {
   DSS_REQUIRE(h && dims, "vit_ragged: null pointer");
   DSS_REQUIRE(B > 0, "vit_ragged: B must be positive (got %d)", B);
-  DSS_REQUIRE(mode == DSS_VIT_RAGGED_K || mode == DSS_VIT_RAGGED_CLS, "vit_ragged: unknown mode %d", mode);
+  DSS_REQUIRE(mode == DSS_VIT_RAGGED_K || mode == DSS_VIT_RAGGED_CLS || mode == DSS_VIT_RAGGED_PAD,
+              "vit_ragged: unknown mode %d", mode);
+  DSS_REQUIRE(n_out >= 0, "vit_ragged: negative n_max %d", n_out);
   const dss_vit_config& c = h->cfg;
   const int P = c.patch;
+  const bool pad = mode == DSS_VIT_RAGGED_PAD;
   long long px = 0, np = 0, M = 0, tiles = 0;
   for (int b = 0; b < B; ++b) {
     const int H = dims[2 * b], W = dims[2 * b + 1];
     DSS_REQUIRE(H >= 0 && W >= 0, "vit_ragged: image %d has negative size %dx%d", b, H, W);
-    DSS_REQUIRE(H >= P && W >= P, "vit_ragged: image %d (%dx%d) is smaller than one %d-pixel patch", b, H, W, P);
-    const long long Hp = H / P, Wp = W / P;
+    if (pad)
+      DSS_REQUIRE(H > 0 && W > 0, "vit_ragged: image %d (%dx%d) has no pixels", b, H, W);
+    else
+      DSS_REQUIRE(H >= P && W >= P, "vit_ragged: image %d (%dx%d) is smaller than one %d-pixel patch", b, H, W, P);
+    const long long Hp = pad ? cdiv(H, P) : H / P, Wp = pad ? cdiv(W, P) : W / P;
+    DSS_REQUIRE(!n_out || Hp * Wp <= n_out, "vit_ragged: image %d (%dx%d) has %lld patches, more than n_max = %d", b, H,
+                W, Hp * Wp, n_out);
     px += (long long)H * W;
     np += Hp * Wp;
     M += Hp * Wp + 1;
     tiles += (Hp * Wp + RAGGED_TILE) / RAGGED_TILE;
   }
-  // row counts are the extents of the tensor maps and GEMM problems (int); tile counts a grid dimension
-  if (M > INT_MAX - 2 * RAGGED_TILE || tiles > INT_MAX) {
-    set_error("vit_ragged: %lld token rows do not fit the tensor-map extents", M);
+  // row counts are the extents of the tensor maps and GEMM problems (int); tile counts a grid dimension; a padded
+  // output's rows are int table entries
+  if (M > INT_MAX - 2 * RAGGED_TILE || tiles > INT_MAX || (long long)B * n_out > INT_MAX) {
+    set_error("vit_ragged: %lld token rows (%lld output rows) do not fit the tensor-map extents", M,
+              (long long)B * n_out);
     return DSS_ERR_UNSUPPORTED;
   }
   pl.n_patches = np;
@@ -481,7 +480,9 @@ static int ragged_plan(const dss_vit* h, const int* dims, int B, int mode, bool 
   pl.k_rows.resize((size_t)M);
   long long pxo = 0, po = 0, to = 0, fo = 0;
   for (int b = 0; b < B; ++b) {
-    const int H = dims[2 * b], W = dims[2 * b + 1], Hp = H / P, Wp = W / P, Np = Hp * Wp;
+    const int H = dims[2 * b], W = dims[2 * b + 1], Hp = pad ? cdiv(H, P) : H / P, Wp = pad ? cdiv(W, P) : W / P;
+    const int Np = Hp * Wp;
+    if (n_out) fo = (long long)b * n_out;
     RaggedImage& im = pl.imgs[b];
     im.px_off = pxo;
     im.H = H; im.W = W; im.Hp = Hp; im.Wp = Wp;
@@ -502,10 +503,10 @@ static int ragged_plan(const dss_vit* h, const int* dims, int B, int mode, bool 
   return DSS_OK;
 }
 
-// Validates a ragged batch (rmode: DSS_VIT_RAGGED_*) and uploads its tables into the workspace.
-static int ragged_setup(dss_vit* h, const int* dims, int B, int rmode, void* ws, size_t ws_bytes, cudaStream_t st,
-                        RaggedPlan& pl, Ragged& rg) {
-  int rc = ragged_plan(h, dims, B, rmode, true, pl);
+// Validates a ragged batch (rmode: DSS_VIT_RAGGED_*, n_out: as ragged_plan) and uploads its tables into the workspace.
+static int ragged_setup(dss_vit* h, const int* dims, int B, int rmode, int n_out, void* ws, size_t ws_bytes,
+                        cudaStream_t st, RaggedPlan& pl, Ragged& rg) {
+  int rc = ragged_plan(h, dims, B, rmode, n_out, true, pl);
   if (rc) return rc;
   DSS_REQUIRE(ws, "vit_ragged: null workspace");
   DSS_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 255) == 0, "vit_ragged: workspace must be 256-byte aligned");
@@ -529,6 +530,7 @@ static int ragged_setup(dss_vit* h, const int* dims, int B, int rmode, void* ws,
   rg.tile_prefix = reinterpret_cast<const int*>(tb + pl.t_tiles);
   rg.patch_rows = reinterpret_cast<const int*>(tb + pl.t_prows);
   rg.k_rows = reinterpret_cast<const int*>(tb + pl.t_krows);
+  rg.n_out = n_out;
   return DSS_OK;
 }
 
@@ -538,7 +540,7 @@ static int vit_ragged(dss_vit* h, const uint8_t* img, const int* dims, int B, in
   DSS_REQUIRE(img && out, "vit_ragged: null pointer");
   RaggedPlan pl;
   Ragged rg;
-  int rc = ragged_setup(h, dims, B, mode == 0 ? DSS_VIT_RAGGED_K : DSS_VIT_RAGGED_CLS, ws, ws_bytes, st, pl, rg);
+  int rc = ragged_setup(h, dims, B, mode == 0 ? DSS_VIT_RAGGED_K : DSS_VIT_RAGGED_CLS, 0, ws, ws_bytes, st, pl, rg);
   if (rc) return rc;
   return vit_run(h, img, B, 0, 0, n_full, mode, out, ws, pl.vit_bytes, st, 0, 1, nullptr, &rg);
 }
@@ -726,7 +728,7 @@ extern "C" int dss_vit_forward_cls(dss_vit_t* h, const uint8_t* images_u8, int B
 
 extern "C" size_t dss_vit_ragged_workspace_bytes(const dss_vit_t* h, const int* dims_host, int B, int mode) {
   RaggedPlan pl;
-  return ragged_plan(h, dims_host, B, mode, false, pl) == DSS_OK ? pl.total : 0;
+  return ragged_plan(h, dims_host, B, mode, 0, false, pl) == DSS_OK ? pl.total : 0;
 }
 
 extern "C" int dss_vit_forward_k_ragged(dss_vit_t* h, const uint8_t* images_u8, const int* dims_host, int B,
@@ -746,13 +748,31 @@ extern "C" int dss_vit_forward_cls_ragged(dss_vit_t* h, const uint8_t* images_u8
                     static_cast<cudaStream_t>(stream));
 }
 
+extern "C" int dss_vit_forward_last_ragged(dss_vit_t* h, const uint8_t* images_u8, const int* dims_host, int B,
+                                           int pad, int which, float* feats_out, int n_max, float* cls_attn_out,
+                                           void* ws, size_t ws_bytes, dss_stream_t stream) {
+  DSS_REQUIRE(h, "vit_forward_last_ragged: null handle");
+  DSS_REQUIRE(pad == 0 || pad == 1, "vit_forward_last_ragged: pad must be 0 or 1, got %d", pad);
+  DSS_REQUIRE(which >= 0 && which <= 2, "vit_forward_last_ragged: which must be 0 (q), 1 (k) or 2 (v), got %d", which);
+  DSS_REQUIRE(images_u8 && (feats_out || cls_attn_out), "vit_forward_last_ragged: null pointer");
+  DSS_REQUIRE(n_max > 0, "vit_forward_last_ragged: n_max must be positive (got %d)", n_max);
+  DSS_REQUIRE(!cls_attn_out || B <= 65535, "vit_forward_last_ragged: B = %d CLS attention rows exceed one grid column", B);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  RaggedPlan pl;
+  Ragged rg;
+  int rc = ragged_setup(h, dims_host, B, pad ? DSS_VIT_RAGGED_PAD : DSS_VIT_RAGGED_K, n_max, ws, ws_bytes, st, pl, rg);
+  if (rc) return rc;
+  return vit_run(h, images_u8, B, 0, 0, h->cfg.depth - 1, 3, feats_out, ws, pl.vit_bytes, st, pad, which,
+                 cls_attn_out, &rg);
+}
+
 extern "C" int dss_vit_pos_embed_ragged(dss_vit_t* h, const int* dims_host, int B, int mode, float* pos_out, void* ws,
                                          size_t ws_bytes, dss_stream_t stream) {
   DSS_REQUIRE(h && pos_out, "vit_pos_embed_ragged: null pointer");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   RaggedPlan pl;
   Ragged rg;
-  int rc = ragged_setup(h, dims_host, B, mode, ws, ws_bytes, st, pl, rg);
+  int rc = ragged_setup(h, dims_host, B, mode, 0, ws, ws_bytes, st, pl, rg);
   if (rc) return rc;
   // the forward's first step (it also writes the CLS rows of the workspace's residual stream)
   const VitWs w = carve(h->cfg, (size_t)pl.n_patches, (size_t)pl.M, (size_t)pl.M, ws, h->precision);

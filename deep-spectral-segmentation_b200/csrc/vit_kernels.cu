@@ -107,8 +107,9 @@ __global__ void im2col_split_kernel(const uint8_t* __restrict__ img, __half* __r
 
 // im2col of a ragged batch (vit.cu): imgs[b] gives image b's pixel offset, size, patch grid and first patch row.
 // One thread = 8 consecutive pixels of one patch row, all three channels (the values and stores of im2col_f16_kernel,
-// patch-major thread order); the split form writes one patch element per thread as im2col_split_kernel does.
-template <bool SPLIT>
+// patch-major thread order); the split form writes one patch element per thread as im2col_split_kernel does. PAD: the
+// ceil grid, a pixel outside the image is 0 (the values of im2col_f16_kernel<true> / im2col_split_kernel).
+template <bool SPLIT, bool PAD>
 __global__ void im2col_ragged_kernel(const uint8_t* __restrict__ img, __half* __restrict__ out,
                                      const RaggedImage* __restrict__ imgs, int B, long long n_patches, int P) {
   const int Kp = 3 * P * P, per_patch = SPLIT ? Kp : P * (P / 8);
@@ -120,9 +121,26 @@ __global__ void im2col_ragged_kernel(const uint8_t* __restrict__ img, __half* __
   const RaggedImage im = imgs[b];
   const int n = (int)(gp - im.patch_off), ph = n / im.Wp, pw = n % im.Wp;
   if constexpr (SPLIT) {
-    const int c = r / (P * P), py = (r / P) % P, px = r % P;
-    const float v = pixel_value(img[(im.px_off + (long long)(ph * P + py) * im.W + pw * P + px) * 3 + c], c);
+    const int c = r / (P * P), y = ph * P + (r / P) % P, x = pw * P + r % P;
+    const float v = (!PAD || (y < im.H && x < im.W)) ? pixel_value(img[(im.px_off + (long long)y * im.W + x) * 3 + c], c)
+                                                      : 0.f;
     store_split(out + gp * 3 * Kp + r, Kp, 0, v);
+  } else if constexpr (PAD) {
+    const int py = r / (P / 8), px0 = (r % (P / 8)) * 8, y = ph * P + py, x0 = pw * P + px0;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float v[8];
+#pragma unroll
+      for (int t = 0; t < 8; ++t)
+        v[t] = (y < im.H && x0 + t < im.W)
+                   ? pixel_value(__ldg(img + (im.px_off + (long long)y * im.W + x0 + t) * 3 + c), c) : 0.f;
+      uint4 q;
+      q.x = pack_half2(v[0], v[1]);
+      q.y = pack_half2(v[2], v[3]);
+      q.z = pack_half2(v[4], v[5]);
+      q.w = pack_half2(v[6], v[7]);
+      *reinterpret_cast<uint4*>(out + gp * Kp + (c * P + py) * P + px0) = q;
+    }
   } else {
     const int py = r / (P / 8), px0 = (r % (P / 8)) * 8;
     const uint8_t* src = img + (im.px_off + (long long)(ph * P + py) * im.W + pw * P + px0) * 3;
@@ -191,7 +209,9 @@ layernorm_kernel(const float* __restrict__ x, const float* __restrict__ gamma, c
 // CLS row of the last block's attention (get_last_selfattention(...)[:, :, 0, 1:], the input of dino_seg):
 // s_j = (q_0 . k_j) / 8 over all T tokens, softmax in fp32. One CTA per (head, image); the 64-term dot products are
 // recomputed in each of the three passes (max, sum, output) rather than kept in scratch memory. KeyT: the qkv
-// activations [B*T, 3d] of the fp16 path, or the fp32 qkv GEMM output of DSS_VIT_PRECISION_FP32.
+// activations [M, 3d] of the fp16 path, or the fp32 qkv GEMM output of DSS_VIT_PRECISION_FP32. Loc (UniformRows /
+// RaggedRows, common.cuh) says where image b's T_b tokens lie; its row of out is n_out long, the T_b - 1 patch entries
+// and then exact zeros (n_out = T - 1 for a uniform batch).
 constexpr int CLSATT_THREADS = 256;
 __device__ __forceinline__ float to_f32(__half v) { return __half2float(v); }
 __device__ __forceinline__ float to_f32(float v) { return v; }
@@ -214,13 +234,13 @@ __device__ __forceinline__ float cls_block_reduce(float v, float* red, bool is_m
   __syncthreads();
   return red[CLSATT_THREADS / 32];
 }
-template <typename KeyT>
+template <typename KeyT, typename Loc>
 __global__ void __launch_bounds__(CLSATT_THREADS)
-cls_attention_kernel(const KeyT* __restrict__ qkv, int T, int heads, float* __restrict__ out) {
+cls_attention_kernel(const KeyT* __restrict__ qkv, Loc loc, int heads, int n_out, float* __restrict__ out) {
   __shared__ float q0[64];
   __shared__ float red[CLSATT_THREADS / 32 + 1];
-  const int h = blockIdx.x, b = blockIdx.y, d = heads * 64, tid = threadIdx.x;
-  const KeyT* base = qkv + (long long)b * T * 3 * d;
+  const int h = blockIdx.x, b = blockIdx.y, d = heads * 64, tid = threadIdx.x, T = loc.tokens(b);
+  const KeyT* base = qkv + loc.row0(b) * 3 * d;
   const KeyT* kbase = base + d + h * 64;
   if (tid < 64) q0[tid] = to_f32(base[h * 64 + tid]);
   __syncthreads();
@@ -230,8 +250,9 @@ cls_attention_kernel(const KeyT* __restrict__ qkv, int T, int heads, float* __re
   float sum = 0.f;
   for (int j = tid; j < T; j += CLSATT_THREADS) sum += expf(cls_score(q0, kbase + (long long)j * 3 * d) - mx);
   sum = cls_block_reduce(sum, red, false);
-  float* o = out + ((long long)b * heads + h) * (T - 1);
+  float* o = out + ((long long)b * heads + h) * n_out;
   for (int j = tid + 1; j < T; j += CLSATT_THREADS) o[j - 1] = expf(cls_score(q0, kbase + (long long)j * 3 * d) - mx) / sum;
+  for (int j = T - 1 + tid; j < n_out; j += CLSATT_THREADS) o[j] = 0.f;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -289,15 +310,20 @@ int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P,
 }
 
 int launch_im2col_ragged(const uint8_t* img, void* patches, const RaggedImage* imgs, int B, long long n_patches, int P,
-                         bool split, cudaStream_t st) {
+                         bool split, bool pad, cudaStream_t st) {
   DSS_REQUIRE(img && patches && imgs && B > 0 && n_patches > 0, "im2col_ragged: bad arguments");
   DSS_REQUIRE(P > 0 && P % 8 == 0, "im2col_ragged: patch must be a multiple of 8 (got %d)", P);
   __half* out = reinterpret_cast<__half*>(patches);
+  const unsigned g_split = grid_for(n_patches * 3 * P * P, 256), g_f16 = grid_for(n_patches * P * (P / 8), 256);
   LaunchScope scope(st, KC_IM2COL);
-  if (split)
-    im2col_ragged_kernel<true><<<grid_for(n_patches * 3 * P * P, 256), 256, 0, st>>>(img, out, imgs, B, n_patches, P);
+  if (split && pad)
+    im2col_ragged_kernel<true, true><<<g_split, 256, 0, st>>>(img, out, imgs, B, n_patches, P);
+  else if (split)
+    im2col_ragged_kernel<true, false><<<g_split, 256, 0, st>>>(img, out, imgs, B, n_patches, P);
+  else if (pad)
+    im2col_ragged_kernel<false, true><<<g_f16, 256, 0, st>>>(img, out, imgs, B, n_patches, P);
   else
-    im2col_ragged_kernel<false><<<grid_for(n_patches * P * (P / 8), 256), 256, 0, st>>>(img, out, imgs, B, n_patches, P);
+    im2col_ragged_kernel<false, false><<<g_f16, 256, 0, st>>>(img, out, imgs, B, n_patches, P);
   DSS_CHECK_CUDA(cudaGetLastError());
   return DSS_OK;
 }
@@ -323,11 +349,29 @@ int launch_layernorm(const float* x, const float* g, const float* b, void* y, in
 
 int launch_cls_attention(const void* qkv, bool f32_keys, int B, int T, int heads, float* out, cudaStream_t st) {
   DSS_REQUIRE(B > 0 && T >= 2 && heads > 0, "cls_attention: bad shape (B=%d T=%d heads=%d)", B, T, heads);
+  const UniformRows loc{T, 0, 0, 0};
   LaunchScope scope(st, KC_ATTENTION);
   if (f32_keys)
-    cls_attention_kernel<<<dim3(heads, B), CLSATT_THREADS, 0, st>>>(static_cast<const float*>(qkv), T, heads, out);
+    cls_attention_kernel<<<dim3(heads, B), CLSATT_THREADS, 0, st>>>(static_cast<const float*>(qkv), loc, heads, T - 1,
+                                                                      out);
   else
-    cls_attention_kernel<<<dim3(heads, B), CLSATT_THREADS, 0, st>>>(static_cast<const __half*>(qkv), T, heads, out);
+    cls_attention_kernel<<<dim3(heads, B), CLSATT_THREADS, 0, st>>>(static_cast<const __half*>(qkv), loc, heads, T - 1,
+                                                                      out);
+  DSS_CHECK_CUDA(cudaGetLastError());
+  return DSS_OK;
+}
+
+int launch_cls_attention_ragged(const void* qkv, bool f32_keys, const RaggedImage* imgs, int B, int n_out, int heads,
+                                float* out, cudaStream_t st) {
+  DSS_REQUIRE(qkv && imgs && out && B > 0 && n_out > 0 && heads > 0, "cls_attention_ragged: bad arguments");
+  const RaggedRows loc{imgs, B};
+  LaunchScope scope(st, KC_ATTENTION);
+  if (f32_keys)
+    cls_attention_kernel<<<dim3(heads, B), CLSATT_THREADS, 0, st>>>(static_cast<const float*>(qkv), loc, heads, n_out,
+                                                                      out);
+  else
+    cls_attention_kernel<<<dim3(heads, B), CLSATT_THREADS, 0, st>>>(static_cast<const __half*>(qkv), loc, heads, n_out,
+                                                                      out);
   DSS_CHECK_CUDA(cudaGetLastError());
   return DSS_OK;
 }

@@ -120,7 +120,8 @@ class ImagePrefetcher:
 
 class PackedRing:
     """Ring of page-locked uint8 buffers that each hold one batch of images of ANY sizes packed one after another
-    ([sum H*W, 3], the input layout of the ragged ViT forwards). ``stage`` copies decoded images into the next slot
+    ([sum H*W, 3], the input layout of the ragged ViT forwards). ``stage`` copies decoded uint8 [H, W, 3] images (torch
+    or numpy) into the next slot
     (host memcpy; a slot grows when a batch does not fit) and returns the packed view and the dims [B, 2];
     ``to_device`` starts the asynchronous H2D copy and returns the device batch. A slot is reused only after the copy
     that read it has completed (tracked with a CUDA event)."""
@@ -151,7 +152,7 @@ class PackedRing:
         offs = np.cumsum([0] + sizes)
 
         def copy(j):
-            np.copyto(dst[offs[j]:offs[j + 1]], images[j].numpy().reshape(-1, 3))
+            np.copyto(dst[offs[j]:offs[j + 1]], np.asarray(images[j]).reshape(-1, 3))
         # numpy's copy loop releases the interpreter lock (torch's Tensor.copy_ on CPU tensors does not), so a few threads
         # copy in parallel
         if self._pool is None or len(images) < 2 * self.copy_threads:

@@ -2,8 +2,10 @@
 from the eigenvectors (eigen-segmentation), and the LOST and DINO-seg baselines, scored by CorLoc on Pascal VOC.
 
 Device work: csrc/localize.cu (the three box kernels, one CTA per image) and the last-block ViT outputs of csrc/vit.cu
-(zero-padded grid, q / k / v features, the CLS attention row). The host reads VOC annotations with ElementTree, JPEG
-sizes from their headers and images on reader threads, and keeps the reference's output files:
+(zero-padded grid, q / k / v features, the CLS attention row). LOST and DINO-seg run ``--batch_size`` images per ViT
+forward in list order whatever their sizes (a ragged forward with outputs padded to the batch's largest grid, then one
+box kernel over the batch); eigen-segmentation from images batches images of one size. The host reads VOC annotations
+with ElementTree, JPEG sizes from their headers and images on reader threads, and keeps the reference's output files:
 ``{output_dir}/{dataset}/{exp_name}/preds.pkl``, ``gt.pkl`` (dict image file name -> int64 boxes [xmin, ymin, xmax,
 ymax]) and ``results.txt``. Single process: there is no multi-GPU sharding of this command."""
 from __future__ import annotations
@@ -13,6 +15,7 @@ import os
 import pickle
 import sys
 import xml.etree.ElementTree as ET
+from collections import deque
 from concurrent.futures import ThreadPoolExecutor
 from pathlib import Path
 from pprint import pprint
@@ -83,6 +86,52 @@ def dinoseg_boxes(cls_attn: torch.Tensor, grid: Tuple[int, int], patch: int, hea
         _lib.check(_lib.load().dss_dinoseg_boxes(a.data_ptr(), B, heads, N, int(head), int(grid[0]), int(grid[1]),
                                                  int(patch), boxes.data_ptr(), status.data_ptr(),
                                                  _lib.stream_ptr(a.device)), "dss_dinoseg_boxes")
+    return boxes.cpu().numpy().astype(np.int64), status.cpu().numpy()
+
+
+@torch.no_grad()
+def lost_boxes_ragged(feats: torch.Tensor, grids: Sequence[Tuple[int, int]], sizes: Sequence[Tuple[int, int]],
+                      patch: int, k_patches: int = 100):
+    """LOST for a batch of images of any sizes: feats [B, n_max, d] fp32 CUDA in the padded layout of
+    DinoViT.forward_last_ragged (image b's gh_b * gw_b rows first, then zero rows), grids[b] = (gh_b, gw_b), sizes[b] =
+    the un-padded (H_b, W_b). One affinity over the padded batch: the zero rows leave each image's block as the image
+    alone gives it. Returns (boxes int64 [B, 4], seeds int32 [B], status int32 [B]) as numpy, each image's as
+    lost_boxes gives for that image alone."""
+    _lib.require_cuda(feats, "feats")
+    B, n_max, _ = feats.shape
+    assert len(grids) == B and len(sizes) == B
+    A = spectral.affinity(feats, normalize=False, threshold_at_zero=False, scale_by_max=False)
+    lib = _lib.load()
+    dims = torch.tensor([[int(g[0]), int(g[1]), int(s[0]), int(s[1])] for g, s in zip(grids, sizes)], dtype=torch.int32)
+    with torch.cuda.device(A.device):
+        boxes = torch.empty(B, 4, dtype=torch.int32, device=A.device)
+        seeds = torch.empty(B, dtype=torch.int32, device=A.device)
+        status = torch.empty(B, dtype=torch.int32, device=A.device)
+        ws = spectral._scratch.get("lost", int(lib.dss_lost_ragged_workspace_bytes(B, n_max)), A.device)
+        _lib.check(lib.dss_lost_boxes_ragged(A.data_ptr(), B, n_max, A.shape[2], dims.data_ptr(), int(patch),
+                                             int(k_patches), boxes.data_ptr(), seeds.data_ptr(), status.data_ptr(),
+                                             ws.data_ptr(), ws.numel(), _lib.stream_ptr(A.device)),
+                   "dss_lost_boxes_ragged")
+    return boxes.cpu().numpy().astype(np.int64), seeds.cpu().numpy(), status.cpu().numpy()
+
+
+@torch.no_grad()
+def dinoseg_boxes_ragged(cls_attn: torch.Tensor, grids: Sequence[Tuple[int, int]], patch: int, head: int = 4):
+    """dino_seg for a batch of images of any sizes: cls_attn [B, heads, n_max] fp32 CUDA in the padded layout of
+    DinoViT.forward_last_ragged, grids[b] = (gh_b, gw_b). Returns (boxes int64 [B, 4], status int32 [B]) as numpy."""
+    _lib.require_cuda(cls_attn, "cls_attn")
+    a = cls_attn.to(torch.float32).contiguous()
+    B, heads, n_max = a.shape
+    assert len(grids) == B
+    lib = _lib.load()
+    dims = torch.tensor([[int(g[0]), int(g[1])] for g in grids], dtype=torch.int32)
+    with torch.cuda.device(a.device):
+        boxes = torch.empty(B, 4, dtype=torch.int32, device=a.device)
+        status = torch.empty(B, dtype=torch.int32, device=a.device)
+        ws = spectral._scratch.get("dinoseg", int(lib.dss_dinoseg_ragged_workspace_bytes(B)), a.device)
+        _lib.check(lib.dss_dinoseg_boxes_ragged(a.data_ptr(), B, heads, n_max, int(head), dims.data_ptr(), int(patch),
+                                                boxes.data_ptr(), status.data_ptr(), ws.data_ptr(), ws.numel(),
+                                                _lib.stream_ptr(a.device)), "dss_dinoseg_boxes_ragged")
     return boxes.cpu().numpy().astype(np.int64), status.cpu().numpy()
 
 
@@ -223,7 +272,9 @@ def parse_args(argv=None):
                              "dino_deitsmall8_pretrain.pth: pass it here to reproduce its numbers.")
     parser.add_argument("--random_init", action="store_true", help="Use randomly initialised weights (tests only).")
     parser.add_argument("--seed", type=int, default=None, help="Seed of the random weights (implies --random_init).")
-    parser.add_argument("--batch_size", type=int, default=16, help="Images per ViT batch (images of one size).")
+    parser.add_argument("--batch_size", type=int, default=16,
+                        help="Images per ViT batch: LOST and DINO-seg take them in list order whatever their sizes; "
+                             "--eigenseg from images batches images of one size.")
     parser.add_argument("--precision", type=str, default="fp16", choices=["fp16", "fp32"],
                         help="ViT arithmetic: fp16 operands (fast) or split-fp16 operands with the fp32 model's results.")
     args = parser.parse_args(argv)
@@ -325,6 +376,23 @@ def _eigseg_precomputed(args, items) -> Dict[str, np.ndarray]:
     return preds
 
 
+def _list_batches(items, batch_size: int, load=None, ahead: int = 2):
+    """Decode on reader threads in list order; yields (indices, [uint8 [H, W, 3] numpy]) of batch_size consecutive
+    items whatever their sizes. At most ``ahead`` batches past the one yielded are decoded or queued, so host memory
+    stays bounded by the batches in flight."""
+    load = load or (lambda it: load_rgb(it.path))
+    window = batch_size * (ahead + 1)
+    futs = deque()
+    with ThreadPoolExecutor(max_workers=io_pipeline.default_workers()) as ex:
+        nxt = 0
+        for start in range(0, len(items), batch_size):
+            while nxt < min(len(items), start + window):
+                futs.append(ex.submit(load, items[nxt]))
+                nxt += 1
+            idx = list(range(start, min(start + batch_size, len(items))))
+            yield idx, [futs.popleft().result() for _ in idx]
+
+
 def _image_batches(items, batch_size: int):
     """Decode on reader threads, group images by (H, W); yields (indices, uint8 [B, H, W, 3] numpy)."""
     pending: Dict[Tuple[int, int], List[Tuple[int, np.ndarray]]] = {}
@@ -339,27 +407,44 @@ def _image_batches(items, batch_size: int):
         yield [g[0] for g in group], np.stack([g[1] for g in group])
 
 
-def _from_images(args, items, model) -> Dict[str, np.ndarray]:
+def _from_images_ragged(args, items, model, load=None) -> Dict[str, np.ndarray]:
+    """LOST and DINO-seg: batch_size images per ragged forward in list order, staged in one page-locked packed buffer;
+    the first failing image in list order raises."""
     P = model.patch_size
+    ring = io_pipeline.PackedRing(model.device)
+    preds = {}
+    for idx, imgs in _list_batches(items, max(1, args.batch_size), load):
+        slot, host, dims = ring.stage(imgs)
+        x = ring.to_device(slot, host)
+        if args.dinoseg:
+            _, attn, grids = model.forward_last_ragged(x, dims, "k", pad=True, feats=False, cls_attn=True)
+            if not 0 <= args.dinoseg_head < model.num_heads:
+                raise ValueError(f"--dinoseg_head {args.dinoseg_head} not in [0, {model.num_heads})")
+            boxes, status = dinoseg_boxes_ragged(attn, [g[1:] for g in grids], P, args.dinoseg_head)
+        else:
+            feats, _, grids = model.forward_last_ragged(x, dims, args.which_features, pad=True)
+            boxes, _, status = lost_boxes_ragged(feats, [g[1:] for g in grids], dims.tolist(), P, args.k_patches)
+        for t, j in enumerate(idx):
+            raise_for_status(int(status[t]), items[j].name)
+            preds[items[j].name] = boxes[t]
+    return preds
+
+
+def _from_images(args, items, model) -> Dict[str, np.ndarray]:
+    if not args.eigenseg:
+        return _from_images_ragged(args, items, model)
+    # eigen-segmentation keeps batches of one size: the reference crops to whole patches on this route
+    # (main.py:220-226), and zero pad rows would change the Laplacian's degrees
     preds = {}
     for idx, imgs in _image_batches(items, max(1, args.batch_size)):
         x = torch.from_numpy(imgs).pin_memory().to(model.device, non_blocking=True)
         B, H, W, _ = x.shape
-        if args.dinoseg:
-            _, attn = model.forward_last(x, "k", pad=True, feats=False, cls_attn=True)
-            if not 0 <= args.dinoseg_head < model.num_heads:
-                raise ValueError(f"--dinoseg_head {args.dinoseg_head} not in [0, {model.num_heads})")
-            boxes, status = dinoseg_boxes(attn, (-(-H // P), -(-W // P)), P, args.dinoseg_head)
-        elif args.eigenseg:   # the reference crops to whole patches on this route (main.py:220-226)
-            feats, _ = model.forward_last(x, args.which_features, pad=False)
-            if args.which_matrix == "laplacian":
-                _, evecs, _, _ = spectral.laplacian_eigs(feats, 2, normalize=False, threshold_at_zero=True, lapnorm=True)
-            else:
-                _, evecs, _ = spectral.affinity_eigs(feats, 2, "affinity", normalize=False, threshold_at_zero=False)
-            boxes, status = eigseg_boxes(evecs, SEGMENT_INDEX[args.which_matrix], [(H, W)] * B)
+        feats, _ = model.forward_last(x, args.which_features, pad=False)
+        if args.which_matrix == "laplacian":
+            _, evecs, _, _ = spectral.laplacian_eigs(feats, 2, normalize=False, threshold_at_zero=True, lapnorm=True)
         else:
-            feats, _ = model.forward_last(x, args.which_features, pad=True)
-            boxes, _, status = lost_boxes(feats, (-(-H // P), -(-W // P)), (H, W), P, args.k_patches)
+            _, evecs, _ = spectral.affinity_eigs(feats, 2, "affinity", normalize=False, threshold_at_zero=False)
+        boxes, status = eigseg_boxes(evecs, SEGMENT_INDEX[args.which_matrix], [(H, W)] * B)
         for t, j in enumerate(idx):
             raise_for_status(int(status[t]), items[j].name)
             preds[items[j].name] = boxes[t]

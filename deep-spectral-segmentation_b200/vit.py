@@ -265,6 +265,30 @@ class DinoViT:
                                                            _lib.stream_ptr(self.device)), "dss_vit_forward_cls_ragged")
         return out, [(b, b + 1) for b in range(B)]
 
+    @torch.no_grad()
+    def forward_last_ragged(self, images, dims=None, which: str = "k", pad: bool = True, feats: bool = True,
+                            cls_attn: bool = False, n_max: Optional[int] = None):
+        """forward_last over images of different sizes in one forward (images / dims as forward_k_ragged). Outputs are
+        padded to n_max rows per image (default: the batch's largest N_b): (features [B, n_max, d] fp32 or None, CLS
+        attention [B, heads, n_max] fp32 or None, grids) with grids[b] = (N_b, gh_b, gw_b). Image b's first N_b rows are
+        the bits forward_last gives for that image alone; the rows after them are +0.0."""
+        w = {"q": 0, "k": 1, "v": 2}.get(which)
+        if w is None:
+            raise ValueError(f"which must be 'q', 'k' or 'v' (got {which!r})")
+        packed, dims = self._ragged_args(images, dims)
+        B = dims.shape[0]
+        grids = ragged_grids(dims.tolist(), self.patch_size, pad)
+        n = max(1, *(g[0] for g in grids)) if n_max is None else int(n_max)
+        with torch.cuda.device(self.device):
+            ws = self._ragged_workspace(dims, _lib.VIT_RAGGED_PAD if pad else _lib.VIT_RAGGED_K)
+            f = torch.empty(B, n, self.dim, dtype=torch.float32, device=self.device) if feats else None
+            a = torch.empty(B, self.num_heads, n, dtype=torch.float32, device=self.device) if cls_attn else None
+            _lib.check(self.lib.dss_vit_forward_last_ragged(self._h, packed.data_ptr(), dims.data_ptr(), B,
+                                                            1 if pad else 0, w, _lib.ptr(f), n, _lib.ptr(a),
+                                                            ws.data_ptr(), ws.numel(), _lib.stream_ptr(self.device)),
+                       "dss_vit_forward_last_ragged")
+        return f, a, grids
+
     def pos_embed(self, Hp: int, Wp: int) -> torch.Tensor:
         """The positional embedding [Hp * Wp + 1, d] fp32 the forwards add for an Hp x Wp patch grid (forward_k's
         identity rule: the stored grid for a square grid0 x grid0 grid)."""
@@ -299,6 +323,16 @@ def ragged_rows(dims, patch_size: int) -> List[Tuple[int, int]]:
         rows.append((r, r + n))
         r += n
     return rows
+
+
+def ragged_grids(dims, patch_size: int, pad: bool) -> List[Tuple[int, int, int]]:
+    """(N_b, gh_b, gw_b) of each image of forward_last_ragged: the ceil grid with pad, else the crop."""
+    out = []
+    for H, W in dims:
+        H, W = int(H), int(W)
+        gh, gw = (-(-H // patch_size), -(-W // patch_size)) if pad else (H // patch_size, W // patch_size)
+        out.append((gh * gw, gh, gw))
+    return out
 
 
 def pos_embed_interp_host(pos_embed: torch.Tensor, grid0: int, Hp: int, Wp: int) -> torch.Tensor:

@@ -135,7 +135,7 @@ int dss_vit_forward_cls(dss_vit_t* h, const uint8_t* images_u8, int B, int H, in
  * sizes, an image smaller than one patch (the message names the image) and a small or misaligned workspace are
  * DSS_ERR_BAD_ARG; a batch whose token rows exceed the tensor-map extents (2^31) is DSS_ERR_UNSUPPORTED. Both precision
  * modes. */
-enum { DSS_VIT_RAGGED_K = 0, DSS_VIT_RAGGED_CLS = 1 };
+enum { DSS_VIT_RAGGED_K = 0, DSS_VIT_RAGGED_CLS = 1, DSS_VIT_RAGGED_PAD = 3 };
 size_t dss_vit_ragged_workspace_bytes(const dss_vit_t* h, const int* dims_host, int B, int mode);
 int dss_vit_forward_k_ragged(dss_vit_t* h, const uint8_t* images_u8, const int* dims_host, int B, int which_block,
                              float* k_out, void* ws, size_t ws_bytes, dss_stream_t stream);
@@ -146,6 +146,19 @@ int dss_vit_forward_cls_ragged(dss_vit_t* h, const uint8_t* images_u8, const int
  * [T_b, d] table at its token rows, as upstream VisionTransformer.interpolate_pos_encoding computes it (bicubic, scale
  * (Hp+0.1)/grid0, the identity rule above). Same arguments and workspace as the forwards. Every forward, uniform or
  * ragged, computes its tables on the device this way, per call: the handle keeps no per-shape state. */
+/* dss_vit_forward_last over a ragged batch (images_u8 and dims_host as above). pad = 1: every image on its zero-padded
+ * ceil(H_b/P) x ceil(W_b/P) grid, so an image may be smaller than one patch (workspace mode DSS_VIT_RAGGED_PAD);
+ * pad = 0: the crop (mode DSS_VIT_RAGGED_K). The identity rule goes by the patch grid, as dss_vit_forward_last's.
+ * Outputs are PADDED, not packed: feats_out [B, n_max, d] fp32 (image b's N_b rows at b * n_max) and cls_attn_out
+ * [B, heads, n_max] fp32, either may be NULL; n_max >= every N_b. Every row is written: an image's N_b rows are the bits
+ * dss_vit_forward_last gives for that image alone, the rows past N_b are +0.0. All checks run on the host before any
+ * device work: those of the ragged forwards, pad and which, n_max below an image's N_b (the message names the image),
+ * B > 65535 with cls_attn_out (DSS_ERR_BAD_ARG), and B * n_max past 2^31 (DSS_ERR_UNSUPPORTED). Both precision
+ * modes. */
+int dss_vit_forward_last_ragged(dss_vit_t* h, const uint8_t* images_u8, const int* dims_host, int B, int pad, int which,
+                                float* feats_out, int n_max, float* cls_attn_out, void* ws, size_t ws_bytes,
+                                dss_stream_t stream);
+
 int dss_vit_pos_embed_ragged(dss_vit_t* h, const int* dims_host, int B, int mode, float* pos_out, void* ws,
                              size_t ws_bytes, dss_stream_t stream);
 /* The same interpolation on HOST buffers (pure CPU, no CUDA call): pos_embed_host [1+grid0^2, d] -> out_host
@@ -434,6 +447,21 @@ int dss_lost_boxes(const float* A, int B, int N, int ldw, int grid_h, int grid_w
  * not clipped. */
 int dss_dinoseg_boxes(const float* cls_attn, int B, int heads, int N, int head, int grid_h, int grid_w, int P,
                       int* boxes, int* status, dss_stream_t stream);
+/* The same two methods on a ragged batch in the padded layout of dss_vit_forward_last_ragged: image b has its own
+ * grid and N_b = gh_b gw_b <= n_max cells, and its rows start at b * n_max. Each image's boxes, seeds and status are
+ * those of the uniform call on that image alone.
+ * LOST: A [B, n_max, ldw] = dss_affinity of the padded features [B, n_max, d] at N = n_max with DSS_AFF_NO_MAX_SCALE
+ * (the pad rows are zero, so image b's N_b x N_b block is the affinity of the image alone); dims_host [B, 4] = {gh, gw,
+ * H, W} per image (host). DINO-seg: cls_attn [B, heads, n_max]; dims_host [B, 2] = {gh, gw}. Checked on the host
+ * before any device work: null pointers, shapes, a grid larger than n_max or with no cells, a small workspace
+ * (DSS_ERR_BAD_ARG / DSS_ERR_WORKSPACE) and a grid past 16384 cells (DSS_ERR_UNSUPPORTED); the message names the
+ * image. */
+size_t dss_lost_ragged_workspace_bytes(int B, int n_max);
+int dss_lost_boxes_ragged(const float* A, int B, int n_max, int ldw, const int* dims_host, int P, int k_patches,
+                          int* boxes, int* seeds, int* status, void* ws, size_t ws_bytes, dss_stream_t stream);
+size_t dss_dinoseg_ragged_workspace_bytes(int B);
+int dss_dinoseg_boxes_ragged(const float* cls_attn, int B, int heads, int n_max, int head, const int* dims_host, int P,
+                             int* boxes, int* status, void* ws, size_t ws_bytes, dss_stream_t stream);
 
 /* Last-block ViT outputs for localization. pad != 0 zero-pads the NORMALISED image up to multiples of P
  * (object-localization/main.py:227-235) and runs on the ceil(H/P) x ceil(W/P) grid; pad == 0 crops like
