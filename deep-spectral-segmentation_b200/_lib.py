@@ -78,6 +78,8 @@ PROTOTYPES = {
     "dss_affinity_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
     "dss_affinity": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p, c_int, c_void_p,
                              c_void_p, c_size_t, c_void_p]),
+    "dss_debug_affinity_trace": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_float, c_void_p, c_int,
+                                         c_void_p, c_void_p, c_size_t, c_void_p, c_size_t, c_void_p]),
     "dss_knn_workspace_bytes": (c_size_t, [c_int, c_int]),
     "dss_knn_color_counts": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "dss_eigsh_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),

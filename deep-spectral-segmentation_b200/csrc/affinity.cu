@@ -131,9 +131,11 @@ extern "C" size_t dss_affinity_workspace_bytes(int B, int N, int d) {
          align_up((size_t)B * N * sizeof(float), 256);   // + degree output when the caller does not ask for it
 }
 
-extern "C" int dss_affinity(const float* feats, int B, int N, int d, int flags, const uint8_t* color_counts,
-                            float color_lambda, float* Wmat, int ldw, float* degree, void* ws, size_t ws_bytes,
-                            dss_stream_t stream) {
+namespace dss {
+// dss_affinity; `trace` (if not null) selects the phase-traced GEMM (dss_debug_affinity_trace)
+static int affinity_run(const float* feats, int B, int N, int d, int flags, const uint8_t* color_counts,
+                        float color_lambda, float* Wmat, int ldw, float* degree, void* ws, size_t ws_bytes,
+                        dss_stream_t stream, unsigned long long* trace, size_t trace_bytes) {
   DSS_REQUIRE(feats && Wmat && ws, "affinity: null pointer");
   DSS_REQUIRE(B > 0 && N > 0 && d > 0, "affinity: empty problem B=%d N=%d d=%d", B, N, d);
   DSS_REQUIRE(ldw >= N && ldw % 4 == 0, "affinity: ldw must be >= N and a multiple of 4 (N=%d ldw=%d)", N, ldw);
@@ -179,7 +181,7 @@ extern "C" int dss_affinity(const float* feats, int B, int N, int d, int flags, 
   if ((rc = affinity_gemm_tc(tmS, tmS_half, B, N, dpad, Wmat, ldw, ncols, img_max, normalize ? nullptr : img_absmax,
                              color_counts, color_lambda,
                              ((flags & DSS_AFF_THRESHOLD_AT_ZERO) ? 1 : 0) | ((flags & DSS_AFF_NO_MAX_SCALE) ? 2 : 0),
-                             deg_part, ld_part, st)))
+                             deg_part, ld_part, st, trace, trace_bytes)))
     return rc;
   {
     LaunchScope scope(st, KC_ROWNORM);
@@ -187,6 +189,23 @@ extern "C" int dss_affinity(const float* feats, int B, int N, int d, int flags, 
     DSS_CHECK_CUDA(cudaGetLastError());
   }
   return DSS_OK;
+}
+}  // namespace dss
+
+extern "C" int dss_affinity(const float* feats, int B, int N, int d, int flags, const uint8_t* color_counts,
+                            float color_lambda, float* Wmat, int ldw, float* degree, void* ws, size_t ws_bytes,
+                            dss_stream_t stream) {
+  return affinity_run(feats, B, N, d, flags, color_counts, color_lambda, Wmat, ldw, degree, ws, ws_bytes, stream,
+                      nullptr, 0);
+}
+
+extern "C" int dss_debug_affinity_trace(const float* feats, int B, int N, int d, int flags, const uint8_t* color_counts,
+                                        float color_lambda, float* Wmat, int ldw, float* degree, void* ws,
+                                        size_t ws_bytes, unsigned long long* trace, size_t trace_bytes,
+                                        dss_stream_t stream) {
+  DSS_REQUIRE(trace != nullptr, "debug_affinity_trace: null trace");
+  return affinity_run(feats, B, N, d, flags, color_counts, color_lambda, Wmat, ldw, degree, ws, ws_bytes, stream,
+                      trace, trace_bytes);
 }
 
 extern "C" int dss_normalize_rows(const float* feats, int rows, int d, float* out, dss_stream_t stream) {

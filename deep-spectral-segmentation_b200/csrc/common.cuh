@@ -54,7 +54,8 @@ int gemm_f16_tc_rows(const CUtensorMap& tmA, const CUtensorMap& tmB, const float
                      int epi, const float* aux, const int* row_map, cudaStream_t st, int kclass);
 int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int images, int Nimg, int d, float* Wout, int ldw,
                      int ncols, const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts,
-                     float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st);
+                     float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st,
+                     unsigned long long* trace = nullptr, size_t trace_bytes = 0);
 // ViT kernels (vit_kernels.cu, attention.cu). split: the operand is written in the split-fp16 format of
 // DSS_VIT_PRECISION_FP32 (A order), three groups per value (split_f16 below)
 int launch_im2col(const uint8_t* img, void* patches, int B, int H, int W, int P, int pad, bool split, cudaStream_t st);

@@ -89,7 +89,8 @@ struct EpiParams {
   int tri;
   float* deg_part;
   int ld_part;
-  // phase trace (dss_debug_gemm_trace only; read by the TRACE instantiations, layout at trace_stride)
+  // phase trace (dss_debug_gemm_trace / dss_debug_affinity_trace only; read by the TRACE instantiations, layout at
+  // trace_stride)
   unsigned long long* trace;
   // destination row per GEMM row (EPI_PATCH_ROWS_F32 / EPI_DROPCLS_ROWS_F32)
   const int* row_map;
@@ -162,7 +163,8 @@ template <int BN>
 __device__ __forceinline__ TileCoord decode_tile(int t, int pairs_m, int tiles_n, int rank, int tri = 0) {
   if (tri) {
     // symmetric output (BN == BM): row pair p only visits n-tiles j >= 2p. Tile (2p+1, 2p) of the odd CTA lies below the
-    // diagonal: it is computed (the pair runs in lock step on the shared B tile) but never stored.
+    // diagonal: its slabs are waited for and released (the pair runs in lock step on the shared B tile), but no wgmma
+    // is issued for it and nothing is stored.
     int per_img = 0;
     for (int p = 0; p < pairs_m; ++p) per_img += max(tiles_n - 2 * p, 0);
     const int z = t / per_img;
@@ -177,6 +179,24 @@ __device__ __forceinline__ TileCoord decode_tile(int t, int pairs_m, int tiles_n
   const int per_img = pairs_m * tiles_n;
   const int z = t / per_img, rem = t - z * per_img;
   return TileCoord{((rem / tiles_n) * 2 + rank) * BM, (rem % tiles_n) * BN, z};
+}
+
+// The k-steps of one slab on the first w columns of a 128-wide tile, w in {0, 8, 16, 32, 64, 96, 128} (0: no wgmma).
+// The accumulators of a narrow wgmma are a prefix of the wide one's, and each output element is the same four k16
+// products whatever the width; the registers past the prefix keep stale values.
+__device__ __forceinline__ void mma_slab_cols(float (&acc)[64], int w, uint64_t adesc, uint64_t bdesc, bool first) {
+  switch (w) {
+    case 8: mma_slab<8>(*reinterpret_cast<float (*)[4]>(&acc), adesc, bdesc, first); break;
+    case 16: mma_slab<16>(*reinterpret_cast<float (*)[8]>(&acc), adesc, bdesc, first); break;
+    case 32: mma_slab<32>(*reinterpret_cast<float (*)[16]>(&acc), adesc, bdesc, first); break;
+    case 64: mma_slab<64>(*reinterpret_cast<float (*)[32]>(&acc), adesc, bdesc, first); break;
+    case 96: mma_slab<96>(*reinterpret_cast<float (*)[48]>(&acc), adesc, bdesc, first); break;
+    case 128: mma_slab<128>(acc, adesc, bdesc, first); break;
+  }
+}
+// Narrowest of those widths that covers r >= 1 columns
+__device__ __forceinline__ int mma_cols(int r) {
+  return r <= 8 ? 8 : r <= 16 ? 16 : r <= 32 ? 32 : r <= 64 ? 64 : r <= 96 ? 96 : 128;
 }
 
 // Accumulator fragment helpers. Warp group wg, warp wi (0..3 inside the group), lane l hold for each 8-column block i
@@ -232,7 +252,7 @@ __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                       const __grid_constant__ CUtensorMap tmC, int M, int N, int K, int pairs_m, int tiles_n,
                       int total_items, EpiParams p) {
-  static_assert(!TRACE || (epi_uses_tma_store(EPI) && EPI != EPI_AFFINITY_F32), "traced: the four ViT epilogues only");
+  static_assert(!TRACE || epi_uses_tma_store(EPI), "traced: the TMA-store epilogues only");
   using Cfg = TileCfg<EPI, BN>;
   constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES;
   extern __shared__ uint8_t smem_raw[];
@@ -282,19 +302,31 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
     if constexpr (TRACE) trec = p.trace + blockIdx.x * trace_stride(total_items, ncl) + 4 + 4 * wg * ((total_items + ncl - 1) / ncl);
     const bool tracer = TRACE && (ct & 127) == 0;
     const NamedBar<1, EPI_THREADS> epi_bar;
+    [[maybe_unused]] int mw = BN;   // affinity: columns of the tile this group's wgmmas compute (0: none)
     // each group computes 64 rows of the tile against the whole B slab
     auto mma = [&](int s, int kb) {
       const uint32_t sa = base + s * STAGE_BYTES;
-      mma_slab<BN>(acc, wgmma_desc_sw128(sa + wg * 64 * 128), wgmma_desc_sw128(sa + A_ATOM_BYTES), kb == 0);
+      const uint64_t adesc = wgmma_desc_sw128(sa + wg * 64 * 128), bdesc = wgmma_desc_sw128(sa + A_ATOM_BYTES);
+      if constexpr (EPI == EPI_AFFINITY_F32) mma_slab_cols(acc, mw, adesc, bdesc, kb == 0);
+      else mma_slab<BN>(acc, adesc, bdesc, kb == 0);
     };
+    // the slab was only read by wgmmas that have retired (wgmma_wait): nothing to publish, no release fence
     auto release = [&](int s) {
       if ((ct & 127) == 0) {
-        mbar_arrive_cluster(bars.empty(s), 0);
-        mbar_arrive_cluster(bars.empty(s), 1);
+        mbar_arrive_cluster_relaxed(bars.empty(s), 0);
+        mbar_arrive_cluster_relaxed(bars.empty(s), 1);
       }
     };
     for (int t = cid; t < total_items; t += ncl) {
       const TileCoord tc = decode_tile<BN>(t, pairs_m, tiles_n, rank, p.tri);
+      if constexpr (EPI == EPI_AFFINITY_F32) {
+        // No wgmma for what no output reads; the group still waits for and releases every slab, so the ring and the
+        // pair's multicast run exactly as for a computed tile. The odd CTA's tile below the diagonal is discarded, a
+        // group whose 64 rows all lie past the image computes nothing, and the image's last column tile runs on the
+        // narrowest wgmma that covers its columns: the epilogue zeroes every column >= M and masks every row >= M,
+        // so the stale accumulators past them reach no output.
+        mw = (p.tri && tc.m0 > tc.n0) || tc.m0 + 64 * wg >= M ? 0 : mma_cols(min(N - tc.n0, BN));
+      }
       if (tracer) trec[0] = globaltimer();
       const int last = consume_slabs(pos, bars, num_kb, tracer ? trec + 1 : nullptr, mma, release);
       wgmma_wait<0>();
@@ -310,8 +342,14 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_cons
         constexpr int BOXC = OUT16 ? 64 : 32;          // columns per 128-byte-wide store box
         constexpr int NBOX = BN / BOXC;
         if constexpr (EPI == EPI_AFFINITY_F32) {
-          // the odd CTA's tile below the diagonal (computed only to keep the pair in lock step on the shared B tile)
-          if (p.tri && tc.m0 > tc.n0) continue;
+          // the odd CTA's tile below the diagonal (its slabs only waited for and released, in step with the pair)
+          if (p.tri && tc.m0 > tc.n0) {
+            if (tracer) {   // no epilogue
+              trec[3] = trec[2];
+              trec += 4;
+            }
+            continue;
+          }
         }
 #pragma unroll
         for (int b = 0; b < NBOX; ++b) {
@@ -922,19 +960,31 @@ int gemm_f16_tc_rows(const CUtensorMap& tmA, const CUtensorMap& tmB, const float
 // Batched Gram product for the affinity build: per image z, W[z] = epilogue(S[z] S'[z]^T) with S = split-fp16 rows
 // [images*Nimg, 3d] (see affinity.cu). The GEMM's ncols output columns (Nimg <= ncols <= ldw) are the first ncols of
 // the row pitch ldw; they also set the column tiles, and with them the layout of the degree partial slots
-// [images, 8 * cdiv(ncols, 128), ld_part] that degree_reduce_kernel reads back.
+// [images, 8 * cdiv(ncols, 128), ld_part] that degree_reduce_kernel reads back. With `trace` (dss_debug_affinity_trace)
+// the phase-traced instantiation runs; trace_bytes must hold trace_stride(items, clusters) words per CTA.
 int affinity_gemm_tc(const CUtensorMap& tmS, const CUtensorMap& tmS_half, int images, int Nimg, int d, float* Wout, int ldw,
                      int ncols, const unsigned int* img_max, const unsigned int* img_absmax, const uint8_t* counts,
-                     float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st) {
+                     float lambda, int threshold, float* deg_part, int ld_part, cudaStream_t st,
+                     unsigned long long* trace, size_t trace_bytes) {
   EpiParams p{Wout, nullptr, nullptr, ldw, 0, 0, Nimg, img_max, img_absmax, counts, lambda, threshold, d / BK,
-              1, deg_part, ld_part};
+              1, deg_part, ld_part, trace};
   DSS_REQUIRE(d % BK == 0, "affinity: feature dim must be a multiple of %d for the tensor-core path (got %d)", BK, d);
   DSS_REQUIRE(ncols >= Nimg && ncols <= ldw, "affinity: bad GEMM column count %d (N=%d ldw=%d)", ncols, Nimg, ldw);
   DSS_REQUIRE(deg_part != nullptr && ld_part >= cdiv(ncols, 128) * 128, "affinity: bad degree partial buffer");
   CUtensorMap tmW;
   int rc = make_tmap_out3d_f32(&tmW, Wout, images, Nimg, ldw);
   if (rc) return rc;
-  return launch_tc<EPI_AFFINITY_F32>(tmS, tmS_half, &tmW, Nimg, ncols, 3 * d, p, st, KC_AFFINITY, 128, images);
+  if (trace == nullptr)
+    return launch_tc<EPI_AFFINITY_F32>(tmS, tmS_half, &tmW, Nimg, ncols, 3 * d, p, st, KC_AFFINITY, 128, images);
+  const int tiles = cdiv(ncols, 128);
+  int items = 0;
+  for (int q = 0; q < cdiv(cdiv(Nimg, BM), 2); ++q) items += tiles - 2 * q > 0 ? tiles - 2 * q : 0;
+  items *= images;
+  const int clusters = gemm_clusters(items);
+  const size_t need = (size_t)(2 * clusters) * trace_stride(items, clusters) * sizeof(unsigned long long);
+  DSS_REQUIRE(trace_bytes >= need, "debug_affinity_trace: the trace needs %zu bytes", need);
+  DSS_CHECK_CUDA(cudaMemsetAsync(trace, 0, need, st));
+  return launch_tc<EPI_AFFINITY_F32, true>(tmS, tmS_half, &tmW, Nimg, ncols, 3 * d, p, st, KC_AFFINITY, 128, images);
 }
 
 template <int EPI>

@@ -248,6 +248,11 @@ size_t dss_affinity_workspace_bytes(int B, int N, int d);
  * dss_eigsh_laplacian. A colour term added AFTER this call (dss_rw_affinity_add) updates `degree` itself. */
 int dss_affinity(const float* feats, int B, int N, int d, int flags, const uint8_t* color_counts, float color_lambda,
                  float* Wmat, int ldw, float* degree, void* ws, size_t ws_bytes, dss_stream_t stream);
+/* Tuning probe (not used by the product path): dss_affinity with the affinity GEMM's phase trace, in the layout of
+ * dss_debug_gemm_trace, items = B * (sum over row-tile pairs p of max(ceil(N / 128) - 2 p, 0)). Tiles the pair discards record an epilogue of zero length. */
+int dss_debug_affinity_trace(const float* feats, int B, int N, int d, int flags, const uint8_t* color_counts,
+                             float color_lambda, float* Wmat, int ldw, float* degree, void* ws, size_t ws_bytes,
+                             unsigned long long* trace, size_t trace_bytes, dss_stream_t stream);
 
 /* Colour KNN affinity (extract_utils.py:151-188): rgb [B, Hl*Wl, 3] fp32 in [0,1] (the /255 low-res image of
  * extract.py:199-204). Two exact-KNN passes (k=20, w=2.0) and (k=10, w=0.1) over points (r,g,b,w*x,w*y),
