@@ -131,6 +131,9 @@ PROTOTYPES = {
     "dss_op_im2col_pad_f16": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_int, c_void_p]),
     "dss_upsample_bilinear": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p]),
     "dss_normalize_rows": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "dss_resize_workspace_bytes": (c_size_t, [c_int, c_int, c_int, c_int]),
+    "dss_resize_bilinear": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_void_p,
+                                    c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
     "dss_segeval_workspace_bytes": (c_size_t, [c_int, C.c_longlong]),
     "dss_segeval_counts": (c_int, [c_void_p, C.c_longlong, c_void_p, C.c_longlong, c_void_p, c_int, c_void_p,
                                    C.c_longlong, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),

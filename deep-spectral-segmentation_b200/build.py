@@ -15,7 +15,7 @@ HERE = Path(__file__).resolve().parent
 CSRC = HERE / "csrc"
 LIB = HERE / "libdss_b200.so"
 SOURCES = ["api.cu", "gemm.cu", "vit_kernels.cu", "attention.cu", "vit.cu", "affinity.cu", "eigsh.cu", "knn.cu", "segment.cu",
-           "cluster.cu", "crf.cu", "localize.cu", "segeval.cu"]
+           "cluster.cu", "crf.cu", "localize.cu", "segeval.cu", "resize.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
               "-DDSS_BUILD", "-Xptxas", "-v", *os.environ.get("DSS_EXTRA_NVCC_FLAGS", "").split()]
 

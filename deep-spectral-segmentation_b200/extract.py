@@ -22,7 +22,7 @@ from typing import Dict, List, Optional, Tuple
 import numpy as np
 import torch
 
-from . import _lib, cluster, io_pipeline, segment, spectral
+from . import _lib, cluster, io_pipeline, resize, segment, spectral
 from . import extract_utils as utils
 from . import vit as vit_mod
 
@@ -207,6 +207,13 @@ def _color_inputs(images_root, image_ids, W_lr, H_lr, which_color_matrix, dev):
     if which_color_matrix == "rw":
         return torch.from_numpy(np.ascontiguousarray(lr)).to(dev)
     return torch.from_numpy((lr / 255.0).astype(np.float32)).to(dev)
+
+
+def _device_color_inputs(images_d: torch.Tensor, files: List[str], H_lr: int, W_lr: int, which_color_matrix: str):
+    """extract_all's _color_inputs: the same tensors from the decoded batch [B, H, W, 3] already on the device, resized
+    by Pillow's bilinear rule on the GPU (resize.py). ``files`` names the images (unused here; a caller that swaps in
+    another route may need them)."""
+    return resize.resize(images_d, H_lr, W_lr, "u8" if which_color_matrix == "rw" else "f32")
 
 
 def _bad_rows(evals: torch.Tensor, evecs: torch.Tensor, info: torch.Tensor) -> List[int]:
@@ -791,6 +798,29 @@ def extract_crf_segmentations(images_list: str, images_root: str, segmentations_
 
 
 # ---------------------------------------------------------------------------------------------------------------
+def _extract_all_options(model_name, which_matrix, image_downsample_factor, image_color_lambda, which_color_matrix,
+                         single_region: bool, multi_region: bool) -> Tuple[bool, bool, int]:
+    """extract_all's checks of extract_eigs' options, before any device work -> (Laplacian mode, colour terms, factor).
+    The Laplacian modes solve on the (H_pad // factor) x (W_pad // factor) grid (extract.py:175-188; factor = the patch
+    size by default); the affinity modes always on the patch grid. The segmentation commands read eigenvectors on the
+    patch grid (single region), or on it and the grid twice as fine (multi region); other grids are refused."""
+    _check_supported(which_matrix, which_color_matrix, image_color_lambda)
+    patch_size = vit_mod.arch(model_name)[0]
+    laplacian = which_matrix in ("laplacian", "matting_laplacian")
+    factor = patch_size if (image_downsample_factor is None or not laplacian) else int(image_downsample_factor)
+    if factor <= 0:
+        raise ValueError(f"image_downsample_factor={image_downsample_factor} must be a positive integer")
+    if single_region and factor != patch_size:
+        raise ValueError(f"single_region_dir: with image_downsample_factor={factor} the eigenvectors have "
+                         f"(H // {factor}) x (W // {factor}) entries, which the single-region segmentation cannot "
+                         f"reshape to the {patch_size}-pixel patch grid")
+    if multi_region and 2 * factor != patch_size and factor != patch_size:
+        raise ValueError(f"multi_region_dir: with image_downsample_factor={factor} the eigenvectors have "
+                         f"(H // {factor}) x (W // {factor}) entries; the multi-region segmentation labels only the "
+                         f"{patch_size}-pixel patch grid or the grid twice as fine (factor {patch_size // 2})")
+    return laplacian, laplacian and image_color_lambda > 0, factor
+
+
 def extract_all(images_list: str, images_root: Optional[str], model_name: str, features_dir: Optional[str],
                 eigs_dir: str, K: int = 20, batch_size: int = 64, which_block: int = -1, normalize: bool = True,
                 threshold_at_zero: bool = True, lapnorm: bool = True, image_color_lambda: float = 0.0,
@@ -798,18 +828,29 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
                 random_init: bool = False, yes: Optional[bool] = None, single_region_dir: Optional[str] = None,
                 multi_region_dir: Optional[str] = None, non_adaptive_num_segments: int = 4, adaptive: bool = False,
                 infer_bg_index: bool = True, threshold: float = 0.0, num_workers: Optional[int] = None,
-                num_workers_out: int = 4, writer: str = "process", precision: str = "fp16"):
+                num_workers_out: int = 4, writer: str = "process", precision: str = "fp16",
+                which_matrix: str = "laplacian", image_downsample_factor: Optional[int] = None):
     """Fused extract_features + extract_eigs (+ the two segmentation commands): features and eigenvectors never leave
     the GPU between the stages. Writes the eigs files and, if the directories are given, the features files and the
     single- / multi-region segmentation PNGs, all in the reference's layouts. Decoding, pinned staging and the file
-    writers run on threads (io_pipeline.py). ``precision``: ViT arithmetic, as in extract_features."""
+    writers run on threads (io_pipeline.py). ``precision``: ViT arithmetic, as in extract_features.
+
+    ``which_matrix``, ``image_downsample_factor``, ``image_color_lambda`` and ``which_color_matrix`` are extract_eigs'
+    options with its defaults, and every file equals what extract_features followed by extract_eigs writes. The colour
+    image is the decoded image already on the device, resized by Pillow's bilinear rule on the GPU (resize.py), so no
+    file is read twice; files that are not 3-channel RGB images are refused by name in colour mode. With a Laplacian
+    grid other than the patch grid (image_downsample_factor other than the patch size), ``single_region_dir`` is
+    refused, as extract_single_region_segmentations cannot reshape such eigenvectors; ``multi_region_dir`` is accepted
+    only at half the patch size, whose 2x finer grid extract_multi_region_segmentations also labels."""
     vit_mod.check_precision(precision)
+    model_name = model_name.lower()
+    laplacian, colour, factor = _extract_all_options(model_name, which_matrix, image_downsample_factor,
+                                                     image_color_lambda, which_color_matrix, bool(single_region_dir),
+                                                     bool(multi_region_dir))
     for dname in (features_dir, eigs_dir, single_region_dir, multi_region_dir):
         if dname:
             utils.make_output_dir(dname, assume_yes=yes)
     wr = io_pipeline.make_writer(writer, num_workers_out)   # first: writer processes import torch while the model is set up
-    model_name = model_name.lower()
-    _check_supported("laplacian", which_color_matrix, image_color_lambda)
     dev = _device()
     model, _, patch_size, _ = utils.get_model(model_name, checkpoint=checkpoint, seed=seed, device=dev,
                                               random_init=random_init, precision=precision)
@@ -829,17 +870,19 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
             h["event"].synchronize()
             assembler.release(h["batch"])     # its host->device copy is long done: the decode threads may refill it
             tb = time.perf_counter()
-            items, H, W, Hp, Wp = h["items"], h["H"], h["W"], h["Hp"], h["Wp"]
+            items, H, W, Hp, Wp, grid = h["items"], h["H"], h["W"], h["Hp"], h["Wp"], h["grid"]
             evals, evecs, info = h["evals"], h["evecs"], h["info"]
-            n_img = len(items)
             # rare: the largest Krylov space that fits for the images that did not reach the tolerance
-            failed = _retry_bad_rows(h["solve"], evals, evecs, info, Hp * Wp)
+            failed = _retry_bad_rows(h["solve"], evals, evecs, info, grid[0] * grid[1])
             all_failed.extend(items[j][1] for j in failed)
+            if which_matrix == "affinity" and bool((info[:, 2] != 0).any()):
+                print("Warning: a negative eigenvalue exceeds the K-th largest in magnitude; eigsh(which='LM') would pick it")
             if features_dir:
                 wr.submit_batch({"k": h["k"].numpy()}, [it_ for j, it_ in enumerate(_feature_items(
                     features_dir, [(it[1], it[2]) for it in items], model_name, patch_size, H, W)) if j not in failed])
-            wr.submit_batch({"evals": evals.numpy(), "evecs": evecs.numpy()},
-                            _eigs_items(eigs_dir, [it[1][:-4] for it in items], skip=failed))
+            ev = evals.flip(1) if which_matrix == "affinity" else evals
+            wr.submit_batch({"evals": ev.numpy(), "evecs": evecs.numpy()},
+                            _eigs_items(eigs_dir, [it[1][:-4] for it in items], which_matrix, skip=failed))
             for j, (_, file, index) in enumerate(items):
                 if j in failed:
                     continue
@@ -847,7 +890,7 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
                     png_pool.submit(_save_png, h["masks"][j].numpy().reshape(Hp, Wp).copy(),
                                     str(Path(single_region_dir) / f"{Path(file).stem}.png"))
                 if h["labels"] is not None:
-                    png_pool.submit(_save_png, h["labels"][j].numpy().reshape(Hp, Wp).copy(),
+                    png_pool.submit(_save_png, h["labels"][j].numpy().reshape(grid).copy(),
                                     str(Path(multi_region_dir) / f"{Path(file).stem}.png"))
             tm["wait_gpu"] += tb - ta
             tm["submit"] += time.perf_counter() - tb
@@ -859,28 +902,42 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
             tb = time.perf_counter()
             items = [(None, file, index) for file, index in batch.items]
             host = batch.host[:len(items)]
-            k = model.forward_k(host.to(dev, non_blocking=True), which_block=which_block)
+            images_d = host.to(dev, non_blocking=True)
+            k = model.forward_k(images_d, which_block=which_block)
             Hp, Wp = H // patch_size, W // patch_size
-            rgb_lr, lr_size = None, None
-            if image_color_lambda > 0:
-                rgb_lr = _color_inputs(images_root, [it[1][:-4] for it in items], Wp, Hp, which_color_matrix, dev)
-                lr_size = (Hp, Wp)
+            # _eigs_for_group's grid (extract.py:175-188): the Laplacian modes solve on the low-resolution grid
+            H_lr, W_lr = Hp * patch_size // factor, Wp * patch_size // factor
+            feats, norm = k, normalize
+            if (H_lr, W_lr) != (Hp, Wp):
+                if norm:     # normalise first, then up-sample (no re-normalisation afterwards)
+                    feats, norm = spectral.normalize_rows(feats), False
+                feats = spectral.upsample_bilinear(feats, Hp, Wp, H_lr, W_lr)
+            rgb_lr = None
+            if colour:
+                rgb_lr = _device_color_inputs(images_d, [it[1] for it in items], H_lr, W_lr, which_color_matrix)
 
-            def solve(sel, max_steps):
-                f = k if sel is None else k[sel]
-                rgb = rgb_lr if (sel is None or rgb_lr is None) else rgb_lr[sel]
-                return spectral.laplacian_eigs(f, K, normalize, threshold_at_zero, lapnorm, rgb, lr_size, image_color_lambda,
-                                               max_steps=max_steps, which_color_matrix=which_color_matrix)[:3]
+            if laplacian:
+                def solve(sel, max_steps):
+                    f = feats if sel is None else feats[sel]
+                    rgb = rgb_lr if (sel is None or rgb_lr is None) else rgb_lr[sel]
+                    return spectral.laplacian_eigs(f, K, norm, threshold_at_zero, lapnorm, rgb, (H_lr, W_lr),
+                                                   image_color_lambda, max_steps=max_steps,
+                                                   which_color_matrix=which_color_matrix)[:3]
+            else:
+                def solve(sel, max_steps):
+                    f = feats if sel is None else feats[sel]
+                    return spectral.affinity_eigs(f, K, which_matrix, normalize, threshold_at_zero, max_steps=max_steps)
             evals_d, evecs_d, info_d = solve(None, 0)
             masks_d = labels_d = None
             if single_region_dir:
                 masks_d = segment.threshold_masks(evecs_d, threshold, which=1)
             if multi_region_dir:
                 if adaptive:   # the per-image cluster count comes from the eigenvalues (host arithmetic on K numbers)
-                    ks = [segment.adaptive_num_clusters(e.numpy()) for e in evals_d.cpu()]
+                    saved = evals_d.flip(1) if which_matrix == "affinity" else evals_d   # what the eigs file holds
+                    ks = [segment.adaptive_num_clusters(e.numpy()) for e in saved.cpu()]
                 else:
                     ks = [non_adaptive_num_segments] * len(items)
-                labels_d = segment.kmeans_labels(evecs_d[:, 1:], ks, (Hp, Wp), infer_bg_index,
+                labels_d = segment.kmeans_labels(evecs_d[:, 1:], ks, (H_lr, W_lr), infer_bg_index,
                                                  image_keys=[it[2] for it in items])[0]
 
             def to_host(t):
@@ -889,7 +946,7 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
                 h_ = torch.empty(t.shape, dtype=t.dtype, pin_memory=True)
                 h_.copy_(t, non_blocking=True)
                 return h_
-            h = {"items": items, "H": H, "W": W, "Hp": Hp, "Wp": Wp, "solve": solve, "evals": to_host(evals_d),
+            h = {"items": items, "H": H, "W": W, "Hp": Hp, "Wp": Wp, "grid": (H_lr, W_lr), "solve": solve, "evals": to_host(evals_d),
                  "evecs": to_host(evecs_d), "info": to_host(info_d), "masks": to_host(masks_d), "labels": to_host(labels_d),
                  "k": to_host(k) if features_dir else None, "keep": (k, evals_d, evecs_d, info_d, masks_d, labels_d),
                  "batch": batch}
@@ -911,7 +968,7 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
         # The decode threads group the images by shape and write them straight into page-locked batches
         # (io_pipeline.BatchAssembler); this thread only sees completed batches.
         if dataset.transform is None:
-            load = dataset.load_raw
+            load = dataset.load_raw_rgb_file if colour else dataset.load_raw
         else:
             def load(i):
                 image, file, index = dataset[i]

@@ -45,6 +45,27 @@ def read_image_raw(path):
         return np.asarray(Image.open(str(path)).convert("RGB")), False
 
 
+def read_image_raw_rgb_file(path):
+    """read_image_raw for callers that also need the file itself to be a 3-channel RGB image (the colour affinities
+    resize the file's own pixels, extract.py:199-204, which fail on grayscale or CMYK files). The file is read once:
+    its PIL mode comes from the header in memory, and a mode other than 'RGB' is refused with the file's name before
+    the same decoder as read_image_raw runs on the bytes."""
+    import io
+    from PIL import Image
+    data = Path(path).read_bytes()
+    mode = Image.open(io.BytesIO(data)).mode
+    if mode != "RGB":
+        raise ValueError(f"{path}: colour affinities need a 3-channel RGB image, this file is PIL mode {mode!r}")
+    try:
+        import cv2
+    except ImportError:
+        return np.asarray(Image.open(io.BytesIO(data)).convert("RGB")), False
+    img = cv2.imdecode(np.frombuffer(data, np.uint8), cv2.IMREAD_COLOR)
+    if img is None:
+        raise IOError(f"cannot decode {path}")
+    return img, True
+
+
 class ImagesDataset:
     """De-duplicated, sorted list of image files; items are (uint8 RGB HWC tensor, path, index).
 
@@ -73,6 +94,14 @@ class ImagesDataset:
         full_path = Path(path) if self.root is None else self.root / path
         assert full_path.is_file(), f"Not a file: {full_path}"
         pixels, is_bgr = read_image_raw(full_path)
+        return pixels, is_bgr, path, index
+
+    def load_raw_rgb_file(self, index: int):
+        """load_raw that refuses files which are not 3-channel RGB images (read_image_raw_rgb_file)."""
+        path = self.filenames[index]
+        full_path = Path(path) if self.root is None else self.root / path
+        assert full_path.is_file(), f"Not a file: {full_path}"
+        pixels, is_bgr = read_image_raw_rgb_file(full_path)
         return pixels, is_bgr, path, index
 
     def __len__(self) -> int:

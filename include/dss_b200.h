@@ -495,6 +495,21 @@ int dss_upsample_bilinear(const float* feats, int B, int Hp, int Wp, int d, int 
 /* Row-wise L2 normalisation x / max(||x||, 1e-12) (F.normalize, extract.py:148): feats [rows, d] -> out [rows, d]. */
 int dss_normalize_rows(const float* feats, int rows, int d, float* out, dss_stream_t stream);
 
+/* Pillow's Image.resize((W_out, H_out), Image.BILINEAR) of whole images, bit for bit (the low-resolution colour image
+ * of extract.py:199-204): images [B, H, W, 3] uint8 RGB, all of one size -> out [B, H_out * W_out, 3],
+ *   DSS_RESIZE_U8:       uint8 pixels (which_color_matrix='rw');
+ *   DSS_RESIZE_UNIT_F32: fp32 float(pixel / 255.0), the double division rounded once ('knn').
+ * Per axis the caller builds (host, int32) bounds [out, 2] = {first input index, count} and weights [out, taps] in
+ * fixed point with 22 fractional bits, zero past count (resize.py restates Pillow's arithmetic). Downscaling only:
+ * H_out <= H and W_out <= W. Null pointers, empty sizes, a larger output, an unknown kind and windows or weights
+ * outside their ranges are DSS_ERR_BAD_ARG; B or H_out above 65535 is DSS_ERR_UNSUPPORTED. All checks run before any
+ * device work. Workspace: dss_resize_workspace_bytes(H_out, W_out, taps_y, taps_x). */
+enum { DSS_RESIZE_U8 = 0, DSS_RESIZE_UNIT_F32 = 1 };
+size_t dss_resize_workspace_bytes(int H_out, int W_out, int taps_y, int taps_x);
+int dss_resize_bilinear(const uint8_t* images, int B, int H, int W, int H_out, int W_out, const int* bounds_y_host,
+                        const int* weights_y_host, int taps_y, const int* bounds_x_host, const int* weights_x_host,
+                        int taps_x, int kind, void* out, void* ws, size_t ws_bytes, dss_stream_t stream);
+
 /* Segmentation evaluation counts of a ragged batch of (prediction, target) uint8 label maps (the pixel loops of the
  * reference's semantic-segmentation/eval.py and object-segmentation/main.py). images_host [B, DSS_SEGEVAL_FIELDS] int64
  * per image: {pred_offset, pred_h, pred_w, target_offset, target_h, target_w, top, left, h, w, block_h, block_w,
