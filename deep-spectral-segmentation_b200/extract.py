@@ -17,7 +17,8 @@ from __future__ import annotations
 
 from collections import defaultdict
 from pathlib import Path
-from typing import Dict, List, Optional, Tuple
+from dataclasses import dataclass
+from typing import Callable, Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -56,41 +57,34 @@ def _device():
     return torch.device("cuda", torch.cuda.current_device())
 
 
-def _feature_dict(k: torch.Tensor, index: int, file: str, model_name: str, patch_size: int, H: int, W: int) -> dict:
-    """The dict the reference saves at extract.py:98-110 (k is (1, N, d) fp32 on the CPU; shape is un-cropped)."""
-    return {"k": k, "indices": torch.tensor(index), "file": file, "id": Path(file).stem, "model_name": model_name,
-            "patch_size": patch_size, "shape": (1, 3, H, W)}
-
-
-def _feature_items(output_dir, files_indices, model_name, patch_size, H, W):
-    """Writer items (io_pipeline) for the feature dicts of one batch: extract.py:98-110, k taken from arrays['k']."""
-    items = []
-    for j, (file, index) in enumerate(files_indices):
-        extra = {"file": file, "id": Path(file).stem, "model_name": model_name, "patch_size": patch_size, "shape": (1, 3, H, W)}
-        items.append((str(Path(output_dir) / f"{Path(file).stem}.pth"), j, extra,
-                      {"k": ("slice1", "k"), "indices": ("tensor0d", index)}))
-    return items
-
-
-def _eigs_items(output_dir, image_ids, which_matrix="laplacian", skip=()):
-    """Writer items for the eigs dicts of one batch (extract.py:242). The 'affinity' branch of the reference keeps
-    `eigenvalues` as the ascending numpy array eigsh returned while the eigenvectors are flipped (extract.py:171-172):
-    the caller passes arrays['evals'] already flipped and it is saved as numpy."""
-    how = "np_slice" if which_matrix == "affinity" else "slice"
-    return [(str(Path(output_dir) / f"{image_id}.pth"), j, {}, {"eigenvalues": (how, "evals"), "eigenvectors": ("slice", "evecs")})
-            for j, image_id in enumerate(image_ids) if j not in skip]
-
-
-def _feature_items_ragged(output_dir, items, rows, model_name, patch_size):
-    """Writer items for the feature dicts of one ragged batch: image j = (image, file, index) has the k rows
-    rows[j] = (r0, r1) of arrays['k'], saved as [1, N, d] like _feature_items."""
+def _feature_files(output_dir, images, rows, model_name, patch_size):
+    """Writer items (io_pipeline) for the feature dicts of one batch, the dict the reference saves at extract.py:98-110:
+    image j = (file, index, H, W) has the k rows rows[j] = (r0, r1) of arrays['k'], saved as [1, N, d] fp32; its shape
+    is the un-cropped (1, 3, H, W)."""
     out = []
-    for (image, file, index), (r0, r1) in zip(items, rows):
-        H, W = int(image.shape[0]), int(image.shape[1])
+    for (file, index, H, W), (r0, r1) in zip(images, rows):
         extra = {"file": file, "id": Path(file).stem, "model_name": model_name, "patch_size": patch_size, "shape": (1, 3, H, W)}
         out.append((str(Path(output_dir) / f"{Path(file).stem}.pth"), r0, extra,
                     {"k": ("rows1", ("k", r1 - r0)), "indices": ("tensor0d", index)}))
     return out
+
+
+def _feature_dict(k: torch.Tensor, index: int, file: str, model_name: str, patch_size: int, H: int, W: int) -> dict:
+    """The features file the writers save for one image (k is [1, N, d] fp32 on the CPU)."""
+    return io_pipeline._materialise({"k": k[0].numpy()}, *_feature_files("", [(file, index, H, W)], [(0, k.shape[1])],
+                                                                          model_name, patch_size)[0][1:])
+
+
+def _eigs_content(which_matrix: str, evals: torch.Tensor, evecs: Optional[torch.Tensor] = None):
+    """The eigs files of a batch (extract.py:242) from descending CPU eigenvalues [B, K] (and eigenvectors [B, K, N]) ->
+    (writer arrays, fields of each file's dict; io_pipeline._materialise). The reference's 'affinity' branch keeps the
+    ascending numpy eigenvalues eigsh returned beside eigenvectors flipped to descending order (extract.py:171-172)."""
+    affinity = which_matrix == "affinity"
+    arrays = {"evals": (evals.flip(1) if affinity else evals).numpy()}
+    fields = {"eigenvalues": ("np_slice" if affinity else "slice", "evals")}
+    if evecs is not None:
+        arrays["evecs"], fields["eigenvectors"] = evecs.numpy(), ("slice", "evecs")
+    return arrays, fields
 
 
 class _Batcher:
@@ -159,7 +153,8 @@ def extract_features(images_list: str, images_root: Optional[str], model_name: s
         def flush(items):
             slot, host, dims = ring.stage([it[0] for it in items])
             k, rows = model.forward_k_ragged(ring.to_device(slot, host), dims, which_block=which_block)
-            wr.submit_batch({"k": k.cpu().numpy()}, _feature_items_ragged(output_dir, items, rows, model_name, patch_size))
+            images = [(file, index, int(image.shape[0]), int(image.shape[1])) for image, file, index in items]
+            wr.submit_batch({"k": k.cpu().numpy()}, _feature_files(output_dir, images, rows, model_name, patch_size))
 
         batch = []
         todo = []
@@ -186,19 +181,44 @@ def _load_image_lr_u8(images_root: str, image_id: str, W_lr: int, H_lr: int) -> 
     return np.array(Image.open(image_file).resize((W_lr, H_lr), Image.BILINEAR))
 
 
-def _load_image_lr(images_root: str, image_id: str, W_lr: int, H_lr: int) -> np.ndarray:
-    """extract.py:199-204: the low-resolution image / 255 -> float64 (H_lr, W_lr, 3)."""
-    return _load_image_lr_u8(images_root, image_id, W_lr, H_lr) / 255.0
+@dataclass(frozen=True)
+class _EigOptions:
+    """extract_eigs' options of the eigen stage (extract.py:119-132), checked when made: every command that runs the
+    stage refuses unsupported options before any file or device work."""
+    K: int
+    which_matrix: str
+    which_color_matrix: str
+    normalize: bool
+    threshold_at_zero: bool
+    lapnorm: bool
+    image_downsample_factor: Optional[int]
+    image_color_lambda: float
 
+    def __post_init__(self):
+        if self.which_matrix == "affinity_torch":
+            raise RuntimeError("which_matrix='affinity_torch' calls torch.eig, which PyTorch removed (dead in the reference)")
+        if self.which_matrix not in ("laplacian", "matting_laplacian", "affinity", "affinity_svd"):
+            raise ValueError(f"unknown which_matrix={self.which_matrix!r}")
+        if self.colour and self.which_color_matrix not in ("knn", "rw"):
+            raise ValueError(f"unknown which_color_matrix={self.which_color_matrix!r} (the reference knows 'knn' and 'rw')")
+        if self.laplacian and self.image_downsample_factor is not None and int(self.image_downsample_factor) <= 0:
+            raise ValueError(f"image_downsample_factor={self.image_downsample_factor} must be a positive integer")
 
-def _check_supported(which_matrix, which_color_matrix, image_color_lambda):
-    if which_matrix == "affinity_torch":
-        raise RuntimeError("which_matrix='affinity_torch' calls torch.eig, which PyTorch removed (dead in the reference)")
-    if which_matrix not in ("laplacian", "matting_laplacian", "affinity", "affinity_svd"):
-        raise ValueError(f"unknown which_matrix={which_matrix!r}")
-    if which_matrix in ("laplacian", "matting_laplacian") and image_color_lambda > 0 \
-            and which_color_matrix not in ("knn", "rw"):
-        raise ValueError(f"unknown which_color_matrix={which_color_matrix!r} (the reference knows 'knn' and 'rw')")
+    @property
+    def laplacian(self) -> bool:
+        return self.which_matrix in ("laplacian", "matting_laplacian")
+
+    @property
+    def colour(self) -> bool:
+        """Colour terms in the affinity: only the Laplacian modes have them (extract.py:190-214)."""
+        return self.laplacian and self.image_color_lambda > 0
+
+    def factor(self, patch_size: int) -> int:
+        """The Laplacian modes solve on the (H_pad // factor) x (W_pad // factor) grid (extract.py:175-188; factor = the
+        patch size by default); the affinity modes always on the patch grid."""
+        if self.image_downsample_factor is None or not self.laplacian:
+            return patch_size
+        return int(self.image_downsample_factor)
 
 
 def _color_inputs(images_root, image_ids, W_lr, H_lr, which_color_matrix, dev):
@@ -209,11 +229,44 @@ def _color_inputs(images_root, image_ids, W_lr, H_lr, which_color_matrix, dev):
     return torch.from_numpy((lr / 255.0).astype(np.float32)).to(dev)
 
 
-def _device_color_inputs(images_d: torch.Tensor, files: List[str], H_lr: int, W_lr: int, which_color_matrix: str):
-    """extract_all's _color_inputs: the same tensors from the decoded batch [B, H, W, 3] already on the device, resized
-    by Pillow's bilinear rule on the GPU (resize.py). ``files`` names the images (unused here; a caller that swaps in
-    another route may need them)."""
-    return resize.resize(images_d, H_lr, W_lr, "u8" if which_color_matrix == "rw" else "f32")
+def _eigen_stage(feats: torch.Tensor, grid: Tuple[int, int], patch_size: int, opts: _EigOptions,
+                 colour: Callable[[int, int], torch.Tensor]):
+    """extract.py:148-240 for device features [B, Hp*Wp, d] fp32 of one patch grid (Hp, Wp) -> (solve, (H_lr, W_lr)):
+    ``solve(sel, max_steps)`` enqueues the eigensolve of batch rows ``sel`` (None: all) -> device (eigenvalues [B, K],
+    eigenvectors [B, K, H_lr * W_lr], info), as _solve_with_retry / _retry_bad_rows call it. Affinity modes solve on the
+    patch grid; Laplacian modes on opts.factor's grid, features normalised, then up-sampled (extract.py:179-188), with
+    ``colour(H_lr, W_lr)`` the low-resolution image of the colour terms. Nothing here waits for the device."""
+    Hp, Wp = grid
+    if not opts.laplacian:
+        def solve(sel, max_steps):
+            f = feats if sel is None else feats[sel]
+            return spectral.affinity_eigs(f, opts.K, opts.which_matrix, opts.normalize, opts.threshold_at_zero,
+                                          max_steps=max_steps)
+        return solve, grid
+    factor = opts.factor(patch_size)
+    lr_size = (Hp * patch_size // factor, Wp * patch_size // factor)
+    normalize = opts.normalize
+    if lr_size != grid:
+        if normalize:
+            feats, normalize = spectral.normalize_rows(feats), False
+        feats = spectral.upsample_bilinear(feats, Hp, Wp, *lr_size)
+    rgb_lr = colour(*lr_size) if opts.colour else None
+
+    def solve(sel, max_steps):
+        f = feats if sel is None else feats[sel]
+        rgb = rgb_lr if (sel is None or rgb_lr is None) else rgb_lr[sel]
+        return spectral.laplacian_eigs(f, opts.K, normalize, opts.threshold_at_zero, opts.lapnorm, rgb, lr_size,
+                                       opts.image_color_lambda, max_steps=max_steps,
+                                       which_color_matrix=opts.which_color_matrix)[:3]
+    return solve, lr_size
+
+
+def _warn_eigs(which_matrix: str, info: torch.Tensor, failed: List[str]):
+    """A solved and retried batch's warnings: images without a file; an 'affinity' eigenvalue eigsh('LM') would pick."""
+    if failed:
+        print(f"Warning: eigensolver did not converge for {failed}; no file is written for them")
+    if which_matrix == "affinity" and bool((info[:, 2] != 0).any()):
+        print("Warning: a negative eigenvalue exceeds the K-th largest in magnitude; eigsh(which='LM') would pick it")
 
 
 def _bad_rows(evals: torch.Tensor, evecs: torch.Tensor, info: torch.Tensor) -> List[int]:
@@ -255,56 +308,20 @@ def _solve_with_retry(solve, n_images: int, N: int):
     return evals, evecs, info, failed
 
 
-def _eigs_for_group(data_dicts: List[dict], K: int, images_root, which_features, normalize, lapnorm, threshold_at_zero,
-                    image_downsample_factor, image_color_lambda, dev, which_matrix="laplacian", which_color_matrix="knn"
+def _eigs_for_group(data_dicts: List[dict], opts: _EigOptions, images_root, which_features, dev
                     ) -> Tuple[torch.Tensor, torch.Tensor, List[int]]:
     """One GPU batch: feature dicts whose patch grids have the same size -> (eigenvalues [B,K], eigenvectors [B,K,N],
-    rows whose solve failed even after the retry) on the CPU."""
+    rows whose solve failed even after the retry) on the CPU. The colour images are read from the image files."""
     feats = torch.stack([d[which_features].squeeze() for d in data_dicts]).to(torch.float32)
     feats = feats.pin_memory().to(dev, non_blocking=True)
-    if which_matrix in ("affinity", "affinity_svd"):
-        def solve(sel, max_steps):
-            f = feats if sel is None else feats[sel]
-            return spectral.affinity_eigs(f, K, which_matrix, normalize, threshold_at_zero, max_steps=max_steps)
-    else:
-        rgb_lr, lr_size = None, None
-        sizes = utils.get_image_sizes(data_dicts[0])
-        P, H_patch, W_patch, H_pad, W_pad = sizes[4:]
-        factor = P if image_downsample_factor is None else image_downsample_factor
-        H_lr, W_lr = H_pad // factor, W_pad // factor
-        if (H_patch, W_patch) != (H_lr, W_lr):
-            # extract.py:148,179-188: normalise first, then bilinear up-sampling (no re-normalisation afterwards)
-            if normalize:
-                feats = spectral.normalize_rows(feats)
-                normalize = False
-            feats = spectral.upsample_bilinear(feats, H_patch, W_patch, H_lr, W_lr)
-        if image_color_lambda > 0:
-            rgb_lr = _color_inputs(images_root, [d["file"][:-4] for d in data_dicts], W_lr, H_lr, which_color_matrix, dev)
-            lr_size = (H_lr, W_lr)
-
-        def solve(sel, max_steps):
-            f = feats if sel is None else feats[sel]
-            rgb = rgb_lr if (sel is None or rgb_lr is None) else rgb_lr[sel]
-            return spectral.laplacian_eigs(f, K, normalize, threshold_at_zero, lapnorm, rgb, lr_size, image_color_lambda,
-                                           max_steps=max_steps, which_color_matrix=which_color_matrix)[:3]
-    evals, evecs, info, failed = _solve_with_retry(solve, len(data_dicts), feats.shape[1])
-    if failed:
-        print(f"Warning: eigensolver did not converge for {[data_dicts[i]['id'] for i in failed]}; no file is written for them")
-    if which_matrix == "affinity" and bool((info[:, 2] != 0).any()):
-        print("Warning: a negative eigenvalue exceeds the K-th largest in magnitude; eigsh(which='LM') would pick it")
+    P, H_patch, W_patch = utils.get_image_sizes(data_dicts[0])[4:7]
+    image_ids = [d["file"][:-4] for d in data_dicts]
+    solve, (H_lr, W_lr) = _eigen_stage(
+        feats, (H_patch, W_patch), P, opts,
+        lambda h, w: _color_inputs(images_root, image_ids, w, h, opts.which_color_matrix, dev))
+    evals, evecs, info, failed = _solve_with_retry(solve, len(data_dicts), H_lr * W_lr)
+    _warn_eigs(opts.which_matrix, info, [data_dicts[i]["id"] for i in failed])
     return evals, evecs, failed
-
-
-def _eigs_dict(which_matrix, evals_k: torch.Tensor, evecs_k: torch.Tensor) -> dict:
-    """extract.py:242. The 'affinity' branch of the reference keeps `eigenvalues` as the ascending numpy array eigsh
-    returned while the eigenvectors are flipped to descending order (extract.py:171-172); mirrored here."""
-    eigenvalues = evals_k.flip(0).numpy().copy() if which_matrix == "affinity" else evals_k.clone()
-    return {"eigenvalues": eigenvalues, "eigenvectors": evecs_k.clone()}
-
-
-def _save_eigs(output_file, which_matrix, evals_k: torch.Tensor, evecs_k: torch.Tensor):
-    Path(output_file).parent.mkdir(parents=True, exist_ok=True)
-    torch.save(_eigs_dict(which_matrix, evals_k, evecs_k), str(output_file))
 
 
 def _extract_eig(inp: Tuple[int, str], K: int, images_root: str, output_dir: str, which_matrix: str = "laplacian",
@@ -312,20 +329,22 @@ def _extract_eig(inp: Tuple[int, str], K: int, images_root: str, output_dir: str
                  which_color_matrix: str = "knn", threshold_at_zero: bool = True,
                  image_downsample_factor: Optional[int] = None, image_color_lambda: float = 10):
     """Single-image worker with the reference's signature (extract.py:119-132); writes {output_dir}/{image_id}.pth."""
+    opts = _EigOptions(K=K, which_matrix=which_matrix, which_color_matrix=which_color_matrix, normalize=normalize,
+                       threshold_at_zero=threshold_at_zero, lapnorm=lapnorm,
+                       image_downsample_factor=image_downsample_factor, image_color_lambda=image_color_lambda)
     index, features_file = inp
     data_dict = torch.load(features_file, map_location="cpu")
     image_id = data_dict["file"][:-4]
-    output_file = str(Path(output_dir) / f"{image_id}.pth")
-    if Path(output_file).is_file():
+    output_file = Path(output_dir) / f"{image_id}.pth"
+    if output_file.is_file():
         print(f"Skipping existing file {str(output_file)}")
         return
-    _check_supported(which_matrix, which_color_matrix, image_color_lambda)
-    evals, evecs, failed = _eigs_for_group([data_dict], K, images_root, which_features, normalize, lapnorm,
-                                           threshold_at_zero, image_downsample_factor, image_color_lambda, _device(),
-                                           which_matrix, which_color_matrix)
+    evals, evecs, failed = _eigs_for_group([data_dict], opts, images_root, which_features, _device())
     if failed:
         raise _lib.DssError(f"eigensolver did not converge for {image_id}")
-    _save_eigs(output_file, which_matrix, evals[0], evecs[0])
+    arrays, fields = _eigs_content(which_matrix, evals, evecs)
+    output_file.parent.mkdir(parents=True, exist_ok=True)
+    torch.save(io_pipeline._materialise(arrays, 0, {}, fields), str(output_file))
 
 
 def extract_eigs(images_root: str, features_dir: str, output_dir: str, which_matrix: str = "laplacian",
@@ -345,6 +364,9 @@ def extract_eigs(images_root: str, features_dir: str, output_dir: str, which_mat
             --output_dir "./data/VOC2012/eigs/laplacian" \
             --K 5
     """
+    opts = _EigOptions(K=K, which_matrix=which_matrix, which_color_matrix=which_color_matrix, normalize=normalize,
+                       threshold_at_zero=threshold_at_zero, lapnorm=lapnorm,
+                       image_downsample_factor=image_downsample_factor, image_color_lambda=image_color_lambda)
     utils.make_output_dir(output_dir, assume_yes=yes)
     kwargs = dict(K=K, which_matrix=which_matrix, which_features=which_features, which_color_matrix=which_color_matrix,
                   normalize=normalize, threshold_at_zero=threshold_at_zero, images_root=images_root,
@@ -354,7 +376,6 @@ def extract_eigs(images_root: str, features_dir: str, output_dir: str, which_mat
     if multiprocessing:
         print(f"Note: multiprocessing={multiprocessing} is ignored: images are batched inside the GPU kernels "
               f"({batch_size} per launch) instead of forked CPU workers")
-    _check_supported(which_matrix, which_color_matrix, image_color_lambda)
     dev = _device()
     inputs = _my_share(list(enumerate(sorted(Path(features_dir).iterdir()))))
     import time
@@ -363,13 +384,11 @@ def extract_eigs(images_root: str, features_dir: str, output_dir: str, which_mat
 
     with io_pipeline.make_writer(writer, num_workers_out) as wr:
         def flush(key, dds):
-            evals, evecs, failed = _eigs_for_group(dds, K, images_root, which_features, normalize, lapnorm,
-                                                   threshold_at_zero, image_downsample_factor, image_color_lambda, dev,
-                                                   which_matrix, which_color_matrix)
+            evals, evecs, failed = _eigs_for_group(dds, opts, images_root, which_features, dev)
             all_failed.extend(dds[j]["id"] for j in failed)
-            ev = evals.flip(1) if which_matrix == "affinity" else evals
-            wr.submit_batch({"evals": ev.numpy(), "evecs": evecs.numpy()},
-                            _eigs_items(output_dir, [d["file"][:-4] for d in dds], which_matrix, skip=failed))
+            arrays, fields = _eigs_content(which_matrix, evals, evecs)
+            wr.submit_batch(arrays, [(str(Path(output_dir) / f"{d['file'][:-4]}.pth"), j, {}, fields)
+                                     for j, d in enumerate(dds) if j not in failed])
 
         batcher = _Batcher(batch_size, flush)
         load = lambda i: torch.load(str(inputs[i][1]), map_location="cpu")   # noqa: E731  (file reads overlap on threads)
@@ -798,18 +817,11 @@ def extract_crf_segmentations(images_list: str, images_root: str, segmentations_
 
 
 # ---------------------------------------------------------------------------------------------------------------
-def _extract_all_options(model_name, which_matrix, image_downsample_factor, image_color_lambda, which_color_matrix,
-                         single_region: bool, multi_region: bool) -> Tuple[bool, bool, int]:
-    """extract_all's checks of extract_eigs' options, before any device work -> (Laplacian mode, colour terms, factor).
-    The Laplacian modes solve on the (H_pad // factor) x (W_pad // factor) grid (extract.py:175-188; factor = the patch
-    size by default); the affinity modes always on the patch grid. The segmentation commands read eigenvectors on the
-    patch grid (single region), or on it and the grid twice as fine (multi region); other grids are refused."""
-    _check_supported(which_matrix, which_color_matrix, image_color_lambda)
+def _extract_all_options(model_name, opts: _EigOptions, single_region: bool, multi_region: bool):
+    """extract_all's own refusals, before any device work. The segmentation commands read eigenvectors on the patch grid
+    (single region), or on it and the grid twice as fine (multi region); other grids are refused."""
     patch_size = vit_mod.arch(model_name)[0]
-    laplacian = which_matrix in ("laplacian", "matting_laplacian")
-    factor = patch_size if (image_downsample_factor is None or not laplacian) else int(image_downsample_factor)
-    if factor <= 0:
-        raise ValueError(f"image_downsample_factor={image_downsample_factor} must be a positive integer")
+    factor = opts.factor(patch_size)
     if single_region and factor != patch_size:
         raise ValueError(f"single_region_dir: with image_downsample_factor={factor} the eigenvectors have "
                          f"(H // {factor}) x (W // {factor}) entries, which the single-region segmentation cannot "
@@ -818,7 +830,6 @@ def _extract_all_options(model_name, which_matrix, image_downsample_factor, imag
         raise ValueError(f"multi_region_dir: with image_downsample_factor={factor} the eigenvectors have "
                          f"(H // {factor}) x (W // {factor}) entries; the multi-region segmentation labels only the "
                          f"{patch_size}-pixel patch grid or the grid twice as fine (factor {patch_size // 2})")
-    return laplacian, laplacian and image_color_lambda > 0, factor
 
 
 def extract_all(images_list: str, images_root: Optional[str], model_name: str, features_dir: Optional[str],
@@ -844,9 +855,10 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
     only at half the patch size, whose 2x finer grid extract_multi_region_segmentations also labels."""
     vit_mod.check_precision(precision)
     model_name = model_name.lower()
-    laplacian, colour, factor = _extract_all_options(model_name, which_matrix, image_downsample_factor,
-                                                     image_color_lambda, which_color_matrix, bool(single_region_dir),
-                                                     bool(multi_region_dir))
+    opts = _EigOptions(K=K, which_matrix=which_matrix, which_color_matrix=which_color_matrix, normalize=normalize,
+                       threshold_at_zero=threshold_at_zero, lapnorm=lapnorm,
+                       image_downsample_factor=image_downsample_factor, image_color_lambda=image_color_lambda)
+    _extract_all_options(model_name, opts, bool(single_region_dir), bool(multi_region_dir))
     for dname in (features_dir, eigs_dir, single_region_dir, multi_region_dir):
         if dname:
             utils.make_output_dir(dname, assume_yes=yes)
@@ -874,15 +886,18 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
             evals, evecs, info = h["evals"], h["evecs"], h["info"]
             # rare: the largest Krylov space that fits for the images that did not reach the tolerance
             failed = _retry_bad_rows(h["solve"], evals, evecs, info, grid[0] * grid[1])
-            all_failed.extend(items[j][1] for j in failed)
-            if which_matrix == "affinity" and bool((info[:, 2] != 0).any()):
-                print("Warning: a negative eigenvalue exceeds the K-th largest in magnitude; eigsh(which='LM') would pick it")
+            failed_files = [items[j][1] for j in failed]
+            all_failed.extend(failed_files)
+            _warn_eigs(which_matrix, info, failed_files)
             if features_dir:
-                wr.submit_batch({"k": h["k"].numpy()}, [it_ for j, it_ in enumerate(_feature_items(
-                    features_dir, [(it[1], it[2]) for it in items], model_name, patch_size, H, W)) if j not in failed])
-            ev = evals.flip(1) if which_matrix == "affinity" else evals
-            wr.submit_batch({"evals": ev.numpy(), "evecs": evecs.numpy()},
-                            _eigs_items(eigs_dir, [it[1][:-4] for it in items], which_matrix, skip=failed))
+                k = h["k"].numpy()
+                N = k.shape[1]
+                wr.submit_batch({"k": k.reshape(-1, k.shape[2])}, [it_ for j, it_ in enumerate(_feature_files(
+                    features_dir, [(file, index, H, W) for _, file, index in items],
+                    [(j * N, (j + 1) * N) for j in range(len(items))], model_name, patch_size)) if j not in failed])
+            arrays, fields = _eigs_content(which_matrix, evals, evecs)
+            wr.submit_batch(arrays, [(str(Path(eigs_dir) / f"{file[:-4]}.pth"), j, {}, fields)
+                                     for j, (_, file, _) in enumerate(items) if j not in failed])
             for j, (_, file, index) in enumerate(items):
                 if j in failed:
                     continue
@@ -905,36 +920,18 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
             images_d = host.to(dev, non_blocking=True)
             k = model.forward_k(images_d, which_block=which_block)
             Hp, Wp = H // patch_size, W // patch_size
-            # _eigs_for_group's grid (extract.py:175-188): the Laplacian modes solve on the low-resolution grid
-            H_lr, W_lr = Hp * patch_size // factor, Wp * patch_size // factor
-            feats, norm = k, normalize
-            if (H_lr, W_lr) != (Hp, Wp):
-                if norm:     # normalise first, then up-sample (no re-normalisation afterwards)
-                    feats, norm = spectral.normalize_rows(feats), False
-                feats = spectral.upsample_bilinear(feats, Hp, Wp, H_lr, W_lr)
-            rgb_lr = None
-            if colour:
-                rgb_lr = _device_color_inputs(images_d, [it[1] for it in items], H_lr, W_lr, which_color_matrix)
-
-            if laplacian:
-                def solve(sel, max_steps):
-                    f = feats if sel is None else feats[sel]
-                    rgb = rgb_lr if (sel is None or rgb_lr is None) else rgb_lr[sel]
-                    return spectral.laplacian_eigs(f, K, norm, threshold_at_zero, lapnorm, rgb, (H_lr, W_lr),
-                                                   image_color_lambda, max_steps=max_steps,
-                                                   which_color_matrix=which_color_matrix)[:3]
-            else:
-                def solve(sel, max_steps):
-                    f = feats if sel is None else feats[sel]
-                    return spectral.affinity_eigs(f, K, which_matrix, normalize, threshold_at_zero, max_steps=max_steps)
+            # the colour images: the decoded batch already on the device, resized by Pillow's bilinear rule (resize.py)
+            solve, (H_lr, W_lr) = _eigen_stage(
+                k, (Hp, Wp), patch_size, opts,
+                lambda h, w: resize.resize(images_d, h, w, "u8" if which_color_matrix == "rw" else "f32"))
             evals_d, evecs_d, info_d = solve(None, 0)
             masks_d = labels_d = None
             if single_region_dir:
                 masks_d = segment.threshold_masks(evecs_d, threshold, which=1)
             if multi_region_dir:
                 if adaptive:   # the per-image cluster count comes from the eigenvalues (host arithmetic on K numbers)
-                    saved = evals_d.flip(1) if which_matrix == "affinity" else evals_d   # what the eigs file holds
-                    ks = [segment.adaptive_num_clusters(e.numpy()) for e in saved.cpu()]
+                    saved, _ = _eigs_content(which_matrix, evals_d.cpu())   # what the eigs file holds
+                    ks = [segment.adaptive_num_clusters(e) for e in saved["evals"]]
                 else:
                     ks = [non_adaptive_num_segments] * len(items)
                 labels_d = segment.kmeans_labels(evecs_d[:, 1:], ks, (H_lr, W_lr), infer_bg_index,
@@ -968,7 +965,7 @@ def extract_all(images_list: str, images_root: Optional[str], model_name: str, f
         # The decode threads group the images by shape and write them straight into page-locked batches
         # (io_pipeline.BatchAssembler); this thread only sees completed batches.
         if dataset.transform is None:
-            load = dataset.load_raw_rgb_file if colour else dataset.load_raw
+            load = dataset.load_raw_rgb_file if opts.colour else dataset.load_raw
         else:
             def load(i):
                 image, file, index = dataset[i]

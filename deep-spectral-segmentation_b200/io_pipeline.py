@@ -424,8 +424,6 @@ def _materialise(arrays, j, extra, fields):
     for key, (how, val) in fields.items():
         if how == "slice":            # tensor arrays[val][j]
             obj[key] = torch.from_numpy(np.array(arrays[val][j]))
-        elif how == "slice1":         # tensor arrays[val][j:j+1] (keeps the leading batch dimension of 1)
-            obj[key] = torch.from_numpy(np.array(arrays[val][j:j + 1]))
         elif how == "rows1":          # tensor arrays[name][j:j+n] as [1, n, ...] (val = (name, n))
             name, n = val
             obj[key] = torch.from_numpy(np.array(arrays[name][j:j + n]).reshape(1, n, *arrays[name].shape[1:]))
@@ -470,7 +468,7 @@ def _writer_process_main(q, errq, doneq):
 class ProcessWriter:
     """Writer processes for the per-image .pth files. ``submit_batch(arrays, items)``: ``arrays`` maps names to numpy
     arrays with a leading batch dimension (sent once per batch), ``items`` is a list of (path, row j, extra dict, fields)
-    where fields maps dict keys to ("slice" | "slice1" | "np_slice", array name), ("rows1", (array name, rows)) or
+    where fields maps dict keys to ("slice" | "np_slice", array name), ("rows1", (array name, rows)) or
     ("tensor0d", int); the worker builds
     each dict and torch.saves it. Started with the 'spawn' method (no fork of a process that holds a CUDA context and
     running threads). Importing torch in the children takes a second or two, so the pool is PERSISTENT: make_writer()

@@ -146,7 +146,7 @@ def test_writer_rows_items_split_over_processes():
     spans = [(0, 1), (1, 7), (7, 10)]
     items = [(f"f{i}", r0, {}, {"k": ("rows1", ("k", r1 - r0))}) for i, (r0, r1) in enumerate(spans)]
     assert [iop._row_end(it) for it in items] == [1, 7, 10]
-    assert iop._row_end(("p", 3, {}, {"k": ("slice1", "k")})) == 4
+    assert iop._row_end(("p", 3, {}, {"k": ("slice", "k")})) == 4
 
     class Q:
         def __init__(self):

@@ -1,7 +1,7 @@
 """CPU suite for Pillow's bilinear resize (resize.py, csrc/resize.cu) and extract_all's extract_eigs options: the
 host-built window and weight tables, the fixed-point two-pass restatement against PIL.Image.resize itself, the RGB-file
-check of colour mode, and the argument refusals of the C entry point, the Python wrapper and extract_all, all raised
-before any device work."""
+check of colour mode, and the argument refusals of the C entry point, the Python wrapper, extract_all, extract_eigs and
+_extract_eig, all raised before any device work."""
 
 import numpy as np
 import pytest
@@ -172,36 +172,64 @@ def test_colour_mode_reader_refuses_files_that_are_not_rgb(tmp_path):
             lr.reshape(1, 30, 3)
 
 
-@pytest.mark.parametrize("kw, err, match", [
+EIGS_OPTION_REFUSALS = [        # extract_eigs' options: refused by every command that runs the eigen stage
     (dict(which_matrix="affinity_torch"), RuntimeError, "torch.eig"),
     (dict(which_matrix="nope"), ValueError, "unknown which_matrix"),
     (dict(image_color_lambda=10.0, which_color_matrix="nope"), ValueError, "unknown which_color_matrix"),
     (dict(image_downsample_factor=0), ValueError, "positive integer"),
+    (dict(image_downsample_factor=-8), ValueError, "positive integer"),
+]
+EXTRACT_ALL_REFUSALS = [
     (dict(image_downsample_factor=8, single_region_dir="S"), ValueError, "single_region_dir: .* cannot reshape"),
     (dict(image_downsample_factor=4, multi_region_dir="M"), ValueError, "multi_region_dir: .* twice as fine"),
     (dict(image_downsample_factor=12, multi_region_dir="M"), ValueError, "multi_region_dir"),
     (dict(model_name="resnet50"), ValueError, "Cannot get model"),
-])
-def test_extract_all_refuses_before_any_device_work(tmp_path, kw, err, match):
-    ex, _lib = load_pkg("extract"), load_pkg("_lib")
+]
+
+
+@pytest.mark.parametrize("command, kw, err, match",
+                         [(c, *row) for c in ("extract_all", "extract_eigs", "_extract_eig") for row in EIGS_OPTION_REFUSALS]
+                         + [("extract_all", *row) for row in EXTRACT_ALL_REFUSALS])
+def test_extract_all_refuses_before_any_device_work(tmp_path, command, kw, err, match):
+    """extract_all, extract_eigs and _extract_eig refuse unsupported options before any file or device work: no kernel
+    launch, no output directory."""
+    ex, _lib, iop = load_pkg("extract"), load_pkg("_lib"), load_pkg("io_pipeline")
+    out = str(tmp_path / "eigs")
+    features = tmp_path / "features"
+    features.mkdir()
+    (path, j, extra, fields), = ex._feature_files(str(features), [("a.jpg", 0, 64, 48)], [(0, 12)], "dino_vits16", 16)
+    torch.save(iop._materialise({"k": np.ones((12, 384), np.float32)}, j, extra, fields), path)
     n0 = _lib.launch_count()
-    args = dict(images_list=str(tmp_path / "missing.txt"), images_root=str(tmp_path), model_name="dino_vits16",
-                features_dir=None, eigs_dir=str(tmp_path / "eigs"))
-    args.update(kw)
-    for key in ("single_region_dir", "multi_region_dir"):
-        if key in args:
-            args[key] = str(tmp_path / args[key])
+    if command == "extract_all":
+        args, kwargs = (), dict(images_list=str(tmp_path / "missing.txt"), images_root=str(tmp_path),
+                                model_name="dino_vits16", features_dir=None, eigs_dir=out)
+        kwargs.update(kw)
+        for key in ("single_region_dir", "multi_region_dir"):
+            if key in kwargs:
+                kwargs[key] = str(tmp_path / kwargs[key])
+    elif command == "extract_eigs":
+        args, kwargs = (str(tmp_path), str(features), out), dict(K=4, **kw)
+    else:
+        args, kwargs = ((0, path), 4, str(tmp_path), out), kw
     with pytest.raises(err, match=match):
-        ex.extract_all(**args)
+        getattr(ex, command)(*args, **kwargs)
     assert _lib.launch_count() == n0
     assert not (tmp_path / "eigs").exists()      # refused before any output directory is made
 
 
-def test_extract_all_accepts_the_grids_the_segmentation_commands_read():
+def test_eig_options_accept_the_grids_the_segmentation_commands_read():
     """The patch grid, the grid twice as fine with multi_region_dir, and the affinity modes (their eigenvectors are on
     the patch grid whatever the factor) pass the option checks; the grid is the patch size divided by the factor."""
-    ex = load_pkg("extract")
-    check = ex._extract_all_options
+    ex, vit = load_pkg("extract"), load_pkg("vit")
+
+    def check(model_name, which_matrix, factor, lam, which_color_matrix, single_region, multi_region):
+        """-> (Laplacian mode, colour terms, factor) of options that pass every check."""
+        opts = ex._EigOptions(K=20, which_matrix=which_matrix, which_color_matrix=which_color_matrix, normalize=True,
+                              threshold_at_zero=True, lapnorm=True, image_downsample_factor=factor,
+                              image_color_lambda=lam)
+        ex._extract_all_options(model_name, opts, single_region, multi_region)
+        return opts.laplacian, opts.colour, opts.factor(vit.arch(model_name)[0])
+
     assert check("dino_vits16", "laplacian", None, 0.0, "knn", True, True) == (True, False, 16)
     assert check("dino_vits16", "laplacian", 16, 10.0, "rw", True, True) == (True, True, 16)
     assert check("dino_vits16", "laplacian", 8, 10.0, "knn", False, True) == (True, True, 8)

@@ -133,7 +133,7 @@ def test_extract_all_mode_equals_the_file_based_commands(cuda, tmp_path, mode, m
             assert im.shape == (2 * (H // P), 2 * (W // P))
 
 
-def test_extract_all_colour_mode_does_not_read_images_twice(cuda, tmp_path, monkeypatch):
+def test_extract_all_colour_mode_reads_each_image_once(cuda, tmp_path, monkeypatch):
     ex = load_pkg("extract")
     root = tmp_path / "images"
     names = _write_images(root, "dino_vits16")
@@ -144,7 +144,6 @@ def test_extract_all_colour_mode_does_not_read_images_twice(cuda, tmp_path, monk
         raise AssertionError("extract_all called the host colour route")
     monkeypatch.setattr(ex, "_color_inputs", host_route)
     monkeypatch.setattr(ex, "_load_image_lr_u8", host_route)
-    monkeypatch.setattr(ex, "_load_image_lr", host_route)
     for matrix in ("knn", "rw"):
         out = tmp_path / f"eigs_{matrix}"
         st = ex.extract_all(str(lst), str(root), "dino_vits16", None, str(out), K=K, batch_size=4, seed=0,

@@ -25,6 +25,7 @@ import subprocess
 import sys
 import tempfile
 import time
+import types
 from pathlib import Path
 
 import torch
@@ -58,21 +59,32 @@ def write_images(root: Path, n: int):
 
 class HostColourRoute:
     """The former colour route inside extract_all: _color_inputs (PIL open + resize of every file on the launching
-    thread) in place of the device resize, and the decoder without the RGB-file check."""
+    thread) in place of the device resize extract_all calls for its colour images (resize.resize), and the decoder
+    without the RGB-file check. That resize sees only the decoded batch: the files it stands for are those of the batch
+    the decoders handed over last, which is the one extract_all is launching."""
 
     def __init__(self, images_root: str):
         self.root = images_root
 
     def __enter__(self):
-        self.saved = ex._device_color_inputs, utils.ImagesDataset.load_raw_rgb_file
-        root = self.root
-        ex._device_color_inputs = lambda images_d, files, H_lr, W_lr, m: ex._color_inputs(
-            root, [f[:-4] for f in files], W_lr, H_lr, m, images_d.device)
+        iop = ex.io_pipeline
+        self.saved = ex.resize, iop.BatchAssembler, utils.ImagesDataset.load_raw_rgb_file
+        root, launching = self.root, []
+
+        class Assembler(iop.BatchAssembler):
+            def __iter__(self_):
+                for batch in super().__iter__():
+                    launching[:] = [file[:-4] for file, _ in batch.items]
+                    yield batch
+
+        def host_resize(images_d, H_lr, W_lr, kind):
+            return ex._color_inputs(root, launching, W_lr, H_lr, "rw" if kind == "u8" else "knn", images_d.device)
+        ex.resize, iop.BatchAssembler = types.SimpleNamespace(resize=host_resize), Assembler
         utils.ImagesDataset.load_raw_rgb_file = utils.ImagesDataset.load_raw
         return self
 
     def __exit__(self, *exc):
-        ex._device_color_inputs, utils.ImagesDataset.load_raw_rgb_file = self.saved
+        ex.resize, ex.io_pipeline.BatchAssembler, utils.ImagesDataset.load_raw_rgb_file = self.saved
         return False
 
 
