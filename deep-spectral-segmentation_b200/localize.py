@@ -1,16 +1,19 @@
 """Object localization (the reference's object-localization/main.py with object_discovery.py and datasets.py): boxes
-from the eigenvectors (eigen-segmentation), and the LOST and DINO-seg baselines, scored by CorLoc on Pascal VOC.
+from the eigenvectors (eigen-segmentation), and the LOST and DINO-seg baselines, scored by CorLoc on Pascal VOC and
+COCO20k.
 
 Device work: csrc/localize.cu (the three box kernels, one CTA per image) and the last-block ViT outputs of csrc/vit.cu
 (zero-padded grid, q / k / v features, the CLS attention row). LOST and DINO-seg run ``--batch_size`` images per ViT
 forward in list order whatever their sizes (a ragged forward with outputs padded to the batch's largest grid, then one
 box kernel over the batch); eigen-segmentation from images batches images of one size. The host reads VOC annotations
-with ElementTree, JPEG sizes from their headers and images on reader threads, and keeps the reference's output files:
-``{output_dir}/{dataset}/{exp_name}/preds.pkl``, ``gt.pkl`` (dict image file name -> int64 boxes [xmin, ymin, xmax,
-ymax]) and ``results.txt``. Single process: there is no multi-GPU sharding of this command."""
+with ElementTree and the COCO20k selection with json, JPEG sizes from their headers and images on reader threads, and
+keeps the reference's output files: ``{output_dir}/{dataset}/{exp_name}/preds.pkl``, ``gt.pkl`` (dict image name ->
+int64 boxes [xmin, ymin, xmax, ymax]; the VOC file name or the COCO image id) and ``results.txt``. Single process:
+there is no multi-GPU sharding of this command."""
 from __future__ import annotations
 
 import argparse
+import json
 import os
 import pickle
 import sys
@@ -190,6 +193,82 @@ def extract_gt_voc(ann: dict, remove_hards: bool = False):
     return np.asarray(boxes), classes
 
 
+def extract_gt_coco(anns: Sequence[dict]) -> np.ndarray:
+    """datasets.py:218-235: int64 boxes [n, 4] of the non-crowd annotations in their JSON order; COCO's float
+    [x, y, w, h] becomes [x, y, x + w, y + h], each rounded half to even by Python's round on float64."""
+    boxes = []
+    for a in anns:
+        if a["iscrowd"] == 1:
+            continue
+        x, y, w, h = (float(v) for v in a["bbox"])
+        boxes.append([int(round(v)) for v in (x, y, x + w, y + h)])
+    return np.asarray(boxes, dtype=np.int64).reshape(-1, 4)
+
+
+# COCO20k: the reference's layout under the data-set directory (datasets.py:50-66)
+COCO_IMAGES = Path("COCO") / "images" / "train2014"
+COCO_ALL_ANNOTATIONS = Path("COCO") / "annotations" / "instances_train2014.json"
+COCO_SELECTION_LIST = "coco_20k_filenames.txt"
+COCO_SELECTION_CACHE = "instances_train2014_sel20k.json"
+
+
+def read_coco20k_ids(path) -> List[int]:
+    """The image ids of the selection list in list order, each once: ``COCO_train2014_000000000123.jpg`` -> 123."""
+    with open(path) as f:
+        ids = [int(line.replace("\n", "").split("_")[-1].split(".")[0]) for line in f if line.strip()]
+    return list(dict.fromkeys(ids))
+
+
+def _check_coco20k_cache(sel: dict, ids: Sequence[int], path) -> None:
+    fix = f"{path}: delete it so that it is rebuilt from the full train2014 annotations"
+    images, anns = sel.get("images"), sel.get("annotations")
+    if (not isinstance(images, list) or not isinstance(anns, list) or "categories" not in sel
+            or any(not isinstance(im, dict) or "file_name" not in im for im in images)
+            or any(not isinstance(a, dict) for a in anns)):
+        raise ValueError(f"{fix}: it is not a COCO annotation file of image records (the format the reference's "
+                         "select_coco_20k writes holds annotations where image records belong)")
+    if sorted(im["id"] for im in images) != sorted(ids):
+        raise ValueError(f"{fix}: its image ids differ from the selection list's")
+
+
+def select_coco20k(root) -> dict:
+    """The COCO20k annotations: the cache ``{root}/instances_train2014_sel20k.json`` if it exists (checked against the
+    selection list, never overwritten), else built from the full train2014 file and written there. The cache is a COCO
+    file: the selected image records in list order, every annotation of those images in the full file's order, and
+    the full file's categories."""
+    root = Path(root)
+    ids = read_coco20k_ids(root / COCO_SELECTION_LIST)
+    cache = root / COCO_SELECTION_CACHE
+    if cache.exists():
+        with open(cache) as f:
+            sel = json.load(f)
+        _check_coco20k_cache(sel, ids, cache)
+        return sel
+    with open(root / COCO_ALL_ANNOTATIONS) as f:
+        full = json.load(f)
+    records = {im["id"]: im for im in full["images"]}
+    missing = [i for i in ids if i not in records]
+    if missing:
+        raise ValueError(f"{root / COCO_SELECTION_LIST}: image id {missing[0]} has no image record in "
+                         f"{root / COCO_ALL_ANNOTATIONS}")
+    wanted = set(ids)
+    sel = {"images": [records[i] for i in ids], "annotations": [a for a in full["annotations"] if a["image_id"] in wanted],
+           "categories": full["categories"]}
+    text = json.dumps(sel)
+    with open(cache, "x") as f:   # "x": a cache another process wrote meanwhile is not overwritten
+        f.write(text)
+    return sel
+
+
+def coco20k_targets(sel: dict) -> List[Tuple[dict, List[dict]]]:
+    """(image record, annotations) per image in torchvision's CocoDetection order: ascending image id, each image's
+    annotations in file order (pycocotools' getAnnIds / loadAnns)."""
+    anns: Dict[int, List[dict]] = {}
+    for a in sel["annotations"]:
+        anns.setdefault(a["image_id"], []).append(a)
+    return [(im, anns.get(im["id"], [])) for im in sorted(sel["images"], key=lambda im: im["id"])]
+
+
 def bbox_iou(box1: torch.Tensor, box2: torch.Tensor, eps: float = 1e-7) -> torch.Tensor:
     """IoU of box1 [4] with each row of box2 [n, 4] in the reference's arithmetic (datasets.py:269-294): torch ops on
     the int64 boxes, eps added to each height and to the union, so the result is float32 exactly as the reference's.
@@ -264,8 +343,11 @@ def parse_args(argv=None):
                         help="Which matrix to use for eigenvector calculation")
     # additions of this implementation
     parser.add_argument("--dataset_root", type=str, default=None,
-                        help="Data-set directory (default: datasets/VOC2007 or datasets/VOC2012 in the working "
-                             "directory, as the reference hard-codes), holding VOCdevkit/VOC<year>/.")
+                        help="Data-set directory, by default the one the reference hard-codes in the working "
+                             "directory. VOC07 / VOC12: datasets/VOC2007 or datasets/VOC2012, holding "
+                             "VOCdevkit/VOC<year>/. COCO20k: datasets, holding COCO/images/train2014/, "
+                             "COCO/annotations/instances_train2014.json, coco_20k_filenames.txt and the selection "
+                             "cache instances_train2014_sel20k.json (written on the first run).")
     parser.add_argument("--checkpoint", type=str, default=None,
                         help="DINO weights (.pth). Default: $DSS_DINO_CHECKPOINT or the torch.hub cache. Note: for "
                              "vit_small/8 the reference loads dino_deitsmall8_300ep_pretrain.pth, not the hub file "
@@ -295,9 +377,8 @@ def check_supported(args) -> None:
         raise ValueError(f"--arch {args.arch} --patch_size {args.patch_size}: patch size must be 8 or 16")
     if args.visualize:
         raise ValueError("--visualize is not supported (it needs skimage and writes matplotlib figures)")
-    if args.dataset == "COCO20k":
-        raise ValueError("--dataset COCO20k is not supported: it needs pycocotools, and the reference's "
-                         "select_coco_20k writes annotation dicts where image records belong")
+    if args.dataset == "COCO20k" and args.set != "train":
+        raise ValueError(f"--dataset COCO20k --set {args.set}: COCO20k is a selection of train2014, pass --set train")
     if args.dinoseg and args.eigenseg:
         raise ValueError("--dinoseg and --eigenseg are exclusive (the reference runs DINO-seg and ignores --eigenseg)")
     if args.eigenseg and args.precomputed_eigs_dir is None and args.which_matrix == "infer":
@@ -316,16 +397,19 @@ def experiment_name(args) -> str:
 
 
 class _Item:
-    __slots__ = ("name", "path", "gt")
+    __slots__ = ("name", "path", "gt", "eig_file")
 
-    def __init__(self, name, path, gt):
+    def __init__(self, name, path, gt, eig_file=None):
         self.name, self.path, self.gt = name, path, gt
+        self.eig_file = eig_file if eig_file is not None else name.replace(".jpg", ".pth")   # main.py:255-258
 
 
 def _dataset_items(args):
     """(data-set name, [items]) in list order; images whose GT is empty under --no_hard are dropped (main.py:245-249)."""
     if args.image_path is not None:
         return args.image_path.split("/")[-1], [_Item(args.image_path.split("/")[-1].split(".")[0], args.image_path, None)]
+    if args.dataset == "COCO20k":
+        return _coco20k_items(args)
     year = VOC_YEARS[args.dataset]
     root_dir = args.dataset_root or f"datasets/VOC{year}"
     if not os.path.exists(root_dir):
@@ -346,6 +430,30 @@ def _dataset_items(args):
     return name, items
 
 
+def _coco20k_items(args):
+    """COCO20k in CocoDetection order, named by image id. An image without a non-crowd box is dropped under --no_hard
+    (as the reference drops it); without --no_hard it is refused here, before any device work, where the reference
+    crashes in bbox_iou or get_image_name."""
+    root_dir = args.dataset_root or "datasets"
+    if not os.path.exists(Path(root_dir) / COCO_IMAGES):
+        raise ValueError(f"{Path(root_dir) / COCO_IMAGES}: please follow the README to set up the datasets "
+                         "(or pass --dataset_root)")
+    name = f"COCO20k_{args.set}" + ("-nohards" if args.no_hard else "")
+    items = []
+    for im, anns in coco20k_targets(select_coco20k(root_dir)):
+        gt = None
+        if not args.no_evaluation:
+            gt = extract_gt_coco(anns)
+            if gt.shape[0] == 0:
+                if args.no_hard:
+                    continue
+                raise ValueError(f"COCO20k image id {im['id']} has no box that is not a crowd, so CorLoc is undefined "
+                                 "for it: pass --no_hard to skip such images (or --no_evaluation)")
+        items.append(_Item(str(im["id"]), str(Path(root_dir) / COCO_IMAGES / im["file_name"]), gt,
+                           f"COCO_train2014_{int(im['id']):012d}.pth"))
+    return name, items
+
+
 def _eigseg_precomputed(args, items) -> Dict[str, np.ndarray]:
     """--eigenseg --precomputed_eigs_dir: JPEG headers and eigenvector files on reader threads, one kernel call per
     distinct (K, N)."""
@@ -355,7 +463,7 @@ def _eigseg_precomputed(args, items) -> Dict[str, np.ndarray]:
     row = SEGMENT_INDEX[which_matrix]
 
     def load(it):
-        ev = torch.load(os.path.join(args.precomputed_eigs_dir, it.name.replace(".jpg", ".pth")), map_location="cpu")
+        ev = torch.load(os.path.join(args.precomputed_eigs_dir, it.eig_file), map_location="cpu")
         return jpeg_size(it.path), ev["eigenvectors"].to(torch.float32)
 
     with ThreadPoolExecutor(max_workers=io_pipeline.default_workers()) as ex:
@@ -376,35 +484,48 @@ def _eigseg_precomputed(args, items) -> Dict[str, np.ndarray]:
     return preds
 
 
-def _list_batches(items, batch_size: int, load=None, ahead: int = 2):
-    """Decode on reader threads in list order; yields (indices, [uint8 [H, W, 3] numpy]) of batch_size consecutive
-    items whatever their sizes. At most ``ahead`` batches past the one yielded are decoded or queued, so host memory
-    stays bounded by the batches in flight."""
-    load = load or (lambda it: load_rgb(it.path))
-    window = batch_size * (ahead + 1)
+def _decode_batches(items, batches, load, ahead: int):
+    """Decode on reader threads; yields (indices, [uint8 [H, W, 3] numpy]) for each index list of ``batches`` in
+    order. At most ``ahead`` batches past the one yielded are decoded or queued, so host memory stays bounded by the
+    batches in flight."""
     futs = deque()
     with ThreadPoolExecutor(max_workers=io_pipeline.default_workers()) as ex:
         nxt = 0
-        for start in range(0, len(items), batch_size):
-            while nxt < min(len(items), start + window):
-                futs.append(ex.submit(load, items[nxt]))
+        for k, idx in enumerate(batches):
+            while nxt < min(len(batches), k + ahead + 1):
+                futs.append([ex.submit(load, items[j]) for j in batches[nxt]])
                 nxt += 1
-            idx = list(range(start, min(start + batch_size, len(items))))
-            yield idx, [futs.popleft().result() for _ in idx]
+            yield idx, [f.result() for f in futs.popleft()]
 
 
-def _image_batches(items, batch_size: int):
-    """Decode on reader threads, group images by (H, W); yields (indices, uint8 [B, H, W, 3] numpy)."""
-    pending: Dict[Tuple[int, int], List[Tuple[int, np.ndarray]]] = {}
+def _list_batches(items, batch_size: int, load=None, ahead: int = 2):
+    """_decode_batches of batch_size consecutive items in list order, whatever their sizes."""
+    batches = [list(range(s, min(s + batch_size, len(items)))) for s in range(0, len(items), batch_size)]
+    yield from _decode_batches(items, batches, load or (lambda it: load_rgb(it.path)), ahead)
+
+
+def _size_batches(sizes: Sequence[Tuple[int, int]], batch_size: int) -> List[List[int]]:
+    """Indices grouped by size into batches of at most batch_size: each full batch in the order its last image comes
+    in the list, then the partial ones in the order of their first images."""
+    full, pending = [], {}
+    for j, size in enumerate(sizes):
+        group = pending.setdefault(size, [])
+        group.append(j)
+        if len(group) == batch_size:
+            full.append(pending.pop(size))
+    return full + list(pending.values())
+
+
+def _image_batches(items, batch_size: int, load=None, ahead: int = 2):
+    """Images of one size per batch; yields (indices, uint8 [B, H, W, 3] numpy). The sizes come from the image
+    headers first, so only the batches in flight are decoded however many sizes the list has."""
     with ThreadPoolExecutor(max_workers=io_pipeline.default_workers()) as ex:
-        for j, img in enumerate(ex.map(lambda it: load_rgb(it.path), items)):
-            key = img.shape[:2]
-            pending.setdefault(key, []).append((j, img))
-            if len(pending[key]) >= batch_size:
-                group = pending.pop(key)
-                yield [g[0] for g in group], np.stack([g[1] for g in group])
-    for group in pending.values():
-        yield [g[0] for g in group], np.stack([g[1] for g in group])
+        sizes = list(ex.map(lambda it: jpeg_size(it.path), items))
+    for idx, imgs in _decode_batches(items, _size_batches(sizes, batch_size), load or (lambda it: load_rgb(it.path)),
+                                     ahead):
+        batch = np.stack(imgs)
+        del imgs   # only the stacked copy stays alive while the caller runs and the next batches decode
+        yield idx, batch
 
 
 def _from_images_ragged(args, items, model, load=None) -> Dict[str, np.ndarray]:
